@@ -4,13 +4,13 @@ GPUS ?= 1
 
 .PHONY: build test test-gpu bench bench-scaling smoke clean-shm clean
 
-build:            ## compile csrc/*.cu for sm_100a into photon_b200/_C*.so (works without a GPU)
+build:            ## compile csrc/*.cu for sm_90a into photon_b200/_C*.so (works without a GPU)
 	$(PY) -m photon_b200.build
 
 test:             ## CPU suite (gloo multi-process, node-manager processes included)
 	$(PY) -m pytest tests -q -m "not gpu"
 
-test-gpu:         ## kernel numerics, engine vs torch, NVLink kernels (needs B200s; multi-GPU tests skip on one GPU)
+test-gpu:         ## kernel numerics, engine vs torch, NVLink kernels (needs H100s; multi-GPU tests skip on one GPU)
 	$(PY) -m pytest tests -q -m gpu
 
 bench:            ## headline metric, one JSON line (GPUS=1|2|4|8)

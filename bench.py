@@ -1,17 +1,17 @@
 #!/usr/bin/env python
-"""Headline benchmark of photon_b200 — one script for every BASELINE.json config.
+"""Headline benchmark of photon_b200 — one script for every benchmark configuration below.
 
-    python bench.py --gpus 1 --steps 4 --warmup 3                       # config #2 (default): MPT-125M, 8 federated clients
+    python bench.py --gpus 1 --steps 4 --warmup 3                       # default: MPT-125M, 8 federated clients
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W [--mode fed|ddp|fed4x2] [--model mpt-1b --server fedadam --precision amp_fp8]
 
-``--mode fed``  (configs #2 / #4)  ``fed_125m_example``: 8 clients per round spread over the N GPUs (8/N per GPU, time-multiplexed on the
+``--mode fed``  ``fed_125m_example``: 8 clients per round spread over the N GPUs (8/N per GPU, time-multiplexed on the
     node's persistent Trainer), local batch 32 × 2048, ADOPT (125M) / DecoupledAdamW (1B+), FedAvg ≡ Nesterov η=1 μ=0 or FedAdam;
     one "step" = every client advances one local optimizer step (8 × 32 × 2048 tokens); the timed region is ONE full round of K
     local steps per client PLUS the round's aggregate + server optimizer + broadcast (the fused NVLink kernel).
-``--mode ddp``  (config #3)  ``cen_125m_example``: centralised training, global batch 256 over the N GPUs, DecoupledAdamW, no clipping,
+``--mode ddp``  ``cen_125m_example``: centralised training, global batch 256 over the N GPUs, DecoupledAdamW, no clipping,
     DDP with the fused NVLink all-reduce on the flat gradient bucket; one step = one optimizer step (256 × 2048 tokens).
-``--mode fed4x2`` (config #5)  4 clients × 2 GPUs: DDP inside every client (fused all-reduce), federated round across the clients.
+``--mode fed4x2``  4 clients × 2 GPUs: DDP inside every client (fused all-reduce), federated round across the clients.
 
 Total work per step is fixed in every mode → ``"scaling": "strong"``.  Two measurements of the same work:
 * ``value``      device time (CUDA events on the launching stream, max over ranks; per-rank min/max printed as ``rank_dev_ms``);
@@ -127,7 +127,7 @@ def fed_cfg(args, impl: str, steps: int, n_clients: int, microbatch):
         "llm_config.scheduler.schedulers.lr.t_warmup=800ba", "photon.comm_stack.shm=false"]
     if args.mode == "fed4x2":
         ov += ["~llm_config.fsdp_config"]      # plain DDP inside the client (the launch scripts' choice, ref: cen_125m_example.sh:87)
-    if args.server == "fedadam":   # BASELINE config #4 flavour
+    if args.server == "fedadam":   # the FedAdam server configuration
         ov += ["fl.strategy_name=fedadam", "fl.strategy_kwargs={eta: 0.1, beta_1: 0.9, beta_2: 0.95, tau: 1.0e-9}", "fl.reset_optimizer=true"]
     ov += ["photon.comm_stack.nvl=true"] if impl == "ours" else ["photon.comm_stack.shm=true"]
     return compose(ov)
@@ -153,6 +153,35 @@ def ddp_cfg(args, impl: str, microbatch):
     return compose(ov)
 
 
+# ------------------------------------------------------------------------------------------------------------------ outputs
+DUMP_ELEMS = 1 << 22    # 16 MiB of float32 per dumped array
+
+
+def output_sample(flat) -> dict:
+    """The model the timed path produced, as host arrays: all of it when small, else a fixed sample (indices drawn once from a
+    seeded generator, so two builds of the project dump the same positions). Sharded (ZeRO) parameters are this rank's slice."""
+    import numpy as np
+    import torch
+
+    n = int(flat.numel())
+    if n <= DUMP_ELEMS:
+        idx = np.arange(n, dtype=np.int64)
+    else:
+        idx = np.sort(np.random.default_rng(0).choice(n, size=DUMP_ELEMS, replace=False))
+    vals = flat.detach().float()[torch.from_numpy(idx).to(flat.device)].cpu().numpy()
+    return {"params": vals.astype(np.float32), "params_index": idx.astype(np.float64),
+            "params_l2": np.array([float(flat.detach().double().norm())], dtype=np.float64)}
+
+
+def write_outputs(out_dir: str, outputs: dict) -> None:
+    import numpy as np
+
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    for name, arr in outputs.items():
+        np.save(d / f"{name}.npy", arr)
+
+
 # ------------------------------------------------------------------------------------------------------------------ arms
 class Env:
     """Process-wide state shared by the arms of one invocation."""
@@ -166,7 +195,7 @@ class Env:
         if self.world != args.gpus:
             raise SystemExit(f"--gpus {args.gpus} but WORLD_SIZE={self.world}: launch with torchrun --nproc-per-node {args.gpus}")
         if not torch.cuda.is_available():
-            raise SystemExit("bench.py measures the sm_100a engine: it needs a CUDA (B200) device and does not fall back to the CPU")
+            raise SystemExit("bench.py measures the sm_90a engine: it needs a CUDA (H100) device and does not fall back to the CPU")
         torch.cuda.set_device(self.local)
         self.dev = torch.device("cuda", self.local)
         if self.world > 1:
@@ -253,6 +282,7 @@ def run_fed(env: Env, args, impl: str, K: int, W: int) -> dict:
     e1.record()
     env.sync()
     dev_ms, own_ms = e0.elapsed_time(e1), e0.elapsed_time(mid["ev"])     # whole round / this rank's local training only
+    outputs = output_sample(rt.round_backend.global_params()[: rt.model_layout.total]) if args.dump_outputs else None
     launches = ops.launch_count() if impl == "ours" else 0
     failed = [r for r in res if r.status.code != 0]
     if failed:
@@ -283,7 +313,7 @@ def run_fed(env: Env, args, impl: str, K: int, W: int) -> dict:
                flops_per_token=float(mcfg.flops_per_token(SEQ)), optimizer=str(rt.cfg["llm_config"]["optimizer"]["name"]),
                comm_stack=rt.round_backend.name, microbatch=int(getattr(rt.trainer, "_auto_mb", None) or rt.trainer.microbatch),
                clients_per_node=n_clients // rt.n_nodes, gpus_per_client=gpc, n_clients=n_clients,
-               h2d=(n_clients // rt.n_nodes) * (LOCAL_BATCH // gpc) * SEQ * 8, d2h=(n_clients // rt.n_nodes) * 2 * 8)
+               h2d=(n_clients // rt.n_nodes) * (LOCAL_BATCH // gpc) * SEQ * 8, d2h=(n_clients // rt.n_nodes) * 2 * 8, outputs=outputs)
     rt.close()
     return out
 
@@ -312,6 +342,7 @@ def run_ddp(env: Env, args, impl: str, K: int, W: int) -> dict:
         ops.reset_launch_count()
     clk = ClockSampler(env.local, enabled=(env.rank == 0)).start()
     dev_ms, _ = env.timed(lambda: tr.fit(duration=f"{K}ba"))
+    outputs = output_sample(tr.state.flat.params[: tr.state.flat.layout.total]) if args.dump_outputs else None
     launches = ops.launch_count() if impl == "ours" else 0
     e2e_s, _ = env.walled(lambda: tr.fit(duration=f"{K}ba"))
     clk.stop()
@@ -335,7 +366,7 @@ def run_ddp(env: Env, args, impl: str, K: int, W: int) -> dict:
                clocks=clk.summary(), tokens=K * DDP_GLOBAL_BATCH * SEQ, flops_per_token=float(tr.model_cfg.flops_per_token(SEQ)),
                optimizer="decoupled_adamw", comm_stack=type(tr.grad_comm).__name__ if tr.grad_comm is not None else "none",
                microbatch=int(getattr(tr, "_auto_mb", None) or tr.microbatch), clients_per_node=1, gpus_per_client=env.world, n_clients=1,
-               h2d=per_gpu * SEQ * 8, d2h=2 * 8)
+               h2d=per_gpu * SEQ * 8, d2h=2 * 8, outputs=outputs)
     free_b, total_b = torch.cuda.mem_get_info(env.dev)
     out["gpu_mem_used_gb"] = round((total_b - free_b) / 2**30, 1)     # whole device, arena planes included (after the run)
     out["torch_peak_alloc_gb"] = round(torch.cuda.max_memory_allocated(env.dev) / 2**30, 1)
@@ -361,9 +392,11 @@ def main() -> None:
     ap.add_argument("--sharding", default="auto", choices=["auto", "none", "zero1", "zero3"],
                     help="ddp mode: none = replicated DDP, zero1 = fused sharded-optimizer step, zero3 = full parameter sharding "
                          "(auto = zero3 for mpt-7b, none otherwise)")
-    ap.add_argument("--global-batch", type=int, default=0, help="ddp mode: sequences per optimizer step (default 256, BASELINE config #3)")
+    ap.add_argument("--global-batch", type=int, default=0, help="ddp mode: sequences per optimizer step (default 256)")
     ap.add_argument("--torch-arm", default="auto", choices=["auto", "on", "off"],
                     help="also measure the reference-equivalent stock-PyTorch arm in this invocation (auto = yes for mpt-125m)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write what the timed path computed in its last step (the model after the timed round / steps) as DIR/<name>.npy")
     args = ap.parse_args()
     if args.global_batch:
         global DDP_GLOBAL_BATCH
@@ -377,6 +410,8 @@ def main() -> None:
     t_ours = time.time()
     r = run(env, args, args.impl, K, W)
     t_ours = time.time() - t_ours
+    if args.dump_outputs and env.rank == 0:
+        write_outputs(args.dump_outputs, r["outputs"])
 
     def emit(torch_arm) -> None:
         if env.rank == 0:

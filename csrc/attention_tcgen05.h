@@ -1,4 +1,4 @@
-// Host API of the tcgen05 flash-attention kernels (see attention_tcgen05.cu).
+// Host API of the wgmma flash-attention kernels (see attention_tcgen05.cu).
 #pragma once
 #include <cuda_runtime.h>
 

@@ -1,4 +1,4 @@
-// Python bindings (torch extension `photon_b200._C`) for the sm_100a kernels in this directory.
+// Python bindings (torch extension `photon_b200._C`) for the sm_90a kernels in this directory.
 // Tensors are passed as torch::Tensor; every op runs on the current CUDA stream of the tensor's device.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -151,6 +151,20 @@ void gemm_fp8(const Tensor& a, const Tensor& b, Tensor& d, int a_mn, int b_mn, i
   }
   g.num_sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
   g.cluster = cluster;
+  // wgmma reads 8-bit operands K-major only: an MN-major operand is transposed into scratch first
+  Tensor at_, bt_;
+  if (a_mn) {
+    at_ = torch::empty({g.M, g.K}, a.options().dtype(at::kByte));
+    pb::transpose_u8(a.data_ptr(), a.stride(0), at_.data_ptr(), g.K, g.M, stream_of(a));
+    g.A = at_.data_ptr(), g.lda = g.K, g.a_mn = 0;
+    g_launches += 1;
+  }
+  if (b_mn) {
+    bt_ = torch::empty({g.N, g.K}, b.options().dtype(at::kByte));
+    pb::transpose_u8(b.data_ptr(), b.stride(0), bt_.data_ptr(), g.K, g.N, stream_of(a));
+    g.B = bt_.data_ptr(), g.ldb = g.K, g.b_mn = 0;
+    g_launches += 1;
+  }
   pb::gemm_launch(g, stream_of(a));
   g_launches += 1;
 }
@@ -586,7 +600,7 @@ void add_launch_count(long long n) { g_launches += n; }  // launches replayed fr
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "photon_b200 sm_100a kernels (tcgen05/TMEM/TMA GEMM + attention, fused norm/loss/optimizer, NVLink collectives)";
+  m.doc() = "photon_b200 sm_90a kernels (wgmma/TMA GEMM + attention, fused norm/loss/optimizer, NVLink collectives)";
   m.def("gemm", &gemm, py::arg("a"), py::arg("b"), py::arg("d"), py::arg("a_mn") = 0, py::arg("b_mn") = 0, py::arg("epi") = 0,
         py::arg("bias") = py::none(), py::arg("aux") = py::none(), py::arg("d2") = py::none(), py::arg("accumulate") = false,
         py::arg("alpha") = 1.0, py::arg("cluster") = 0);

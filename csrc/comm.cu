@@ -531,7 +531,7 @@ static int sm_count(int num_sms) {   // one CTA per SM (co-residency is what mak
   int dev = 0, n = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  return n > 0 ? n : 148;
+  return n > 0 ? n : 132;
 }
 
 int ctl_sums_word_offset() { return CP_SUMS; }

@@ -1,4 +1,4 @@
-// FP8 (E4M3 / E5M2) producers for the kind::f8f6f4 GEMMs of `precision: amp_fp8` on sm_100a.
+// FP8 (E4M3 / E5M2) producers for the fp8 wgmma GEMMs of `precision: amp_fp8` on sm_90a.
 //
 // The recipe is per-tensor scaling (photon_b200/train/fp8.py is the numerics oracle): activations and weights are cast to
 // E4M3, gradients flowing backward to E5M2; every cast multiplies by the tensor role's scale and saturates; the GEMM epilogue
@@ -284,7 +284,7 @@ void colsum_quant(const void* dy, long long ld, float* out_sum, void* y8, long l
                   long long T, int d, cudaStream_t st) {
   if (d % 8) throw std::runtime_error("colsum_quant: the row length must be a multiple of 8");
   const int col_blocks = (d + 255) / 256;
-  int strips = (148 * 4 + col_blocks - 1) / col_blocks;
+  int strips = (132 * 4 + col_blocks - 1) / col_blocks;
   if (strips > T) strips = int(T);
   const int rows_per = int((T + strips - 1) / strips);
   dim3 grid(col_blocks, int((T + rows_per - 1) / rows_per));
@@ -300,7 +300,7 @@ void quantize_segments(const void* src_bf16, void* dst8, const long long* seg_de
   if (n_seg <= 0) return;
   cudaError_t e = cudaMemsetAsync(amax, 0, sizeof(float) * n_seg, st);
   if (e != cudaSuccess) throw std::runtime_error(std::string("quantize_segments memset: ") + cudaGetErrorString(e));
-  int bx = (148 * 8 + n_seg - 1) / n_seg;
+  int bx = (132 * 8 + n_seg - 1) / n_seg;
   if (bx < 1) bx = 1;
   if (bx > 64) bx = 64;
   seg_amax_kernel<<<dim3(bx, n_seg), 256, 0, st>>>((const __nv_bfloat16*)src_bf16, seg_dev, amax);

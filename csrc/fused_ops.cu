@@ -1,4 +1,4 @@
-// Memory-bound fused kernels of the MPT training step for sm_100a (everything that is not a GEMM or
+// Memory-bound fused kernels of the MPT training step for sm_90a (everything that is not a GEMM or
 // attention): embedding gather/scatter, LayerNorm fwd/bwd (+residual-gradient add), column reductions for
 // bias / LN-affine gradients, fused cross-entropy (loss + in-place dlogits), flat-buffer L2 norm,
 // ADOPT / DecoupledAdamW multi-tensor step with bf16 shadow emit, axpby for the streaming client mean.
@@ -651,7 +651,7 @@ __global__ void __launch_bounds__(256) optim_kernel(float* __restrict__ p, const
   }
 }
 
-inline int grid_for(long long work_items, int block, int max_blocks = 148 * 8) {
+inline int grid_for(long long work_items, int block, int max_blocks = 132 * 8) {
   long long b = (work_items + block - 1) / block;
   if (b < 1) b = 1;
   return int(b < max_blocks ? b : max_blocks);
@@ -666,12 +666,12 @@ inline int grid_for(long long work_items, int block, int max_blocks = 148 * 8) {
   } while (0)
 
 void embed_fwd(const int64_t* ids, const void* wte, const void* wpe, void* out, long long T, int S, int d, int V, cudaStream_t st) {
-  embed_fwd_kernel<<<grid_for(T, 1, 148 * 16), 128, 0, st>>>(ids, (const __nv_bfloat16*)wte, (const __nv_bfloat16*)wpe,
+  embed_fwd_kernel<<<grid_for(T, 1, 132 * 16), 128, 0, st>>>(ids, (const __nv_bfloat16*)wte, (const __nv_bfloat16*)wpe,
                                                             (__nv_bfloat16*)out, T, S, d, V);
   PB_CHECK_LAUNCH("embed_fwd");
 }
 void embed_bwd(const int64_t* ids, const void* dh, float* dwte, float* dwpe, long long T, int S, int d, int V, cudaStream_t st) {
-  embed_bwd_wte_kernel<<<grid_for(T, 1, 148 * 16), 128, 0, st>>>(ids, (const __nv_bfloat16*)dh, dwte, T, d, V);
+  embed_bwd_wte_kernel<<<grid_for(T, 1, 132 * 16), 128, 0, st>>>(ids, (const __nv_bfloat16*)dh, dwte, T, d, V);
   PB_CHECK_LAUNCH("embed_bwd_wte");
   if (dwpe) {
     embed_bwd_wpe_kernel<<<S, 128, 0, st>>>((const __nv_bfloat16*)dh, dwpe, int(T / S), S, d);
@@ -694,7 +694,7 @@ void layernorm_fwd(const void* x, const float* gamma, const float* beta, void* y
 void col_reduce(const void* dy, long long ld, const void* x, const float* mean, const float* rstd, float* out_sum, float* out_dot,
                 long long T, int d, cudaStream_t st) {
   const int col_blocks = (d + 255) / 256;
-  int strips = (148 * 4 + col_blocks - 1) / col_blocks;
+  int strips = (132 * 4 + col_blocks - 1) / col_blocks;
   if (strips > T) strips = int(T);
   const int rows_per = int((T + strips - 1) / strips);
   dim3 grid(col_blocks, int((T + rows_per - 1) / rows_per));
@@ -708,7 +708,7 @@ void layernorm_bwd(const void* dy, const void* x, const float* gamma, const floa
   const int nch = (d + 255) / 256;
   if ((dgamma || dbeta) && nch <= 4) {
     // d <= 1024: dx and the dgamma / dbeta column sums in ONE pass over dy and x
-    const int grid = int(std::min<long long>((T + 7) / 8, 148 * 2));   // 2 resident blocks per SM
+    const int grid = int(std::min<long long>((T + 7) / 8, 132 * 2));   // 2 resident blocks per SM
 #define PB_LN_FUSED(N)                                                                                                      \
   if (nch <= N) {                                                                                                           \
     ln_bwd_fused_kernel<N><<<grid, 256, 0, st>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, gamma, mean, rstd,           \
@@ -754,7 +754,7 @@ void cross_entropy(void* logits, long long ld, const int64_t* targets, long long
   PB_CHECK_LAUNCH("cross_entropy");
 }
 void flat_sqnorm(const float* x, long long n, double* out_accum, cudaStream_t st) {
-  sqnorm_kernel<<<grid_for(n / 4, 256, 148 * 4), 256, 0, st>>>(x, n, out_accum);
+  sqnorm_kernel<<<grid_for(n / 4, 256, 132 * 4), 256, 0, st>>>(x, n, out_accum);
   PB_CHECK_LAUNCH("flat_sqnorm");
 }
 void sqrt_finalize(const double* in, float* out, cudaStream_t st) {
@@ -762,16 +762,16 @@ void sqrt_finalize(const double* in, float* out, cudaStream_t st) {
   PB_CHECK_LAUNCH("sqrt_finalize");
 }
 void axpby(float* acc, const float* x, float a, float b, long long n, cudaStream_t st) {
-  axpby_kernel<<<grid_for(n / 4, 256, 148 * 8), 256, 0, st>>>(acc, x, a, b, n / 4);
+  axpby_kernel<<<grid_for(n / 4, 256, 132 * 8), 256, 0, st>>>(acc, x, a, b, n / 4);
   PB_CHECK_LAUNCH("axpby");
 }
 void cast_fp32_to_bf16(const float* src, void* dst, long long n, cudaStream_t st) {
-  cast_bf16_kernel<<<grid_for(n / 4, 256, 148 * 8), 256, 0, st>>>(src, (__nv_bfloat16*)dst, n / 4);
+  cast_bf16_kernel<<<grid_for(n / 4, 256, 132 * 8), 256, 0, st>>>(src, (__nv_bfloat16*)dst, n / 4);
   PB_CHECK_LAUNCH("cast_bf16");
 }
 void fused_optimizer(float* p, const float* g, float* m, float* v, void* shadow, long long n, const OptimHyper& h,
                      const float* grad_mult, cudaStream_t st) {
-  optim_kernel<<<grid_for(n / 4, 256, 148 * 8), 256, 0, st>>>(p, g, m, v, (__nv_bfloat16*)shadow, n / 4, h, grad_mult);
+  optim_kernel<<<grid_for(n / 4, 256, 132 * 8), 256, 0, st>>>(p, g, m, v, (__nv_bfloat16*)shadow, n / 4, h, grad_mult);
   PB_CHECK_LAUNCH("fused_optimizer");
 }
 

@@ -1,17 +1,14 @@
-// Block-scaled FP8 GEMM for sm_100a:  D[M,N] = (A .* SFA)[M,K] * (B .* SFB)[N,K]^T (+ bias), bf16 out
+// Block-scaled FP8 GEMM for sm_90a:  D[M,N] = (A .* SFA)[M,K] * (B .* SFB)[N,K]^T (+ bias), bf16 out
 //
-//   tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale — OCP MXFP8: E4M3 elements, one E8M0 scale per 32 consecutive K elements
-//   of every row of A and of B, applied INSIDE the tensor core (the scale factors are operands of the instruction, read from TMEM).
+//   OCP MXFP8: E4M3 elements, one E8M0 scale per 32 consecutive K elements of every row of A and of B. Hopper's tensor cores
+//   take no scale operands, so every 32-K group is one wgmma.m64n128k32 into a partial accumulator, which is then multiplied by
+//   scale_a(row) * scale_b(column) of that group and added to the running fp32 sum in registers.
 //
-//   * A / B tiles: TMA (128-byte swizzle) into a 3-stage mbarrier ring, 128 K-elements per stage, as in gemm_tcgen05.cu;
-//   * scale factors: stored in global memory already in the layout the tensor core wants — per (128 rows x 128 K) block a 512-byte
-//     atom [32][4][4]: byte (r % 32) * 16 + (r / 32) * 4 + (k / 32) holds the scale of row r, K-group k/32 — so a stage's scales
-//     are ONE contiguous bulk copy per operand (cp.async.bulk, counted on the same mbarrier as the tiles); from shared memory they
-//     go to TMEM with tcgen05.cp.32x128b.warpx4 (4 columns per 128 rows), issued by the MMA thread right before the stage's four
-//     MMAs (cp and mma execute in issue order, so one TMEM scale slot serves every stage);
-//   * instruction descriptor: scale format E8M0, a_sf_id / b_sf_id = which of the 4 bytes of the TMEM word (K-group inside the stage);
-//   * accumulator: 256 fp32 TMEM columns (the scale factors take 12 more, so there is ONE accumulator stage here — the per-tensor
-//     fp8 kernel keeps the double-buffered, CTA-pair pipeline); epilogue: tcgen05.ld -> bias -> bf16 -> swizzled smem -> TMA store.
+//   * A / B tiles: TMA (128-byte swizzle) into a 4-stage mbarrier ring, 128 K-elements per stage, as in gemm_tcgen05.cu;
+//   * scale factors: stored in global memory as per (128 rows x 128 K) block a 512-byte atom [32][4][4]: byte
+//     (r % 32) * 16 + (r / 32) * 4 + (k / 32) holds the scale of row r, K-group k/32 — so a stage's scales are ONE contiguous
+//     bulk copy per operand (cp.async.bulk, counted on the same mbarrier as the tiles);
+//   * two MMA warpgroups (64 rows of the 128 x 128 tile each), epilogue from registers: bias -> bf16 -> global.
 //
 // mx_quantize_kernel produces both the E4M3 data and the scale atoms from a bf16 matrix in one pass (scale = 2^(floor(log2 amax) - 8)).
 // North-star item "block-scaled fp8 for the GEMMs"; numerics oracle: de-quantise and multiply in fp32 (tests/test_fp8_gpu.py).
@@ -24,27 +21,27 @@
 
 #include "gemm_tcgen05.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace pb {
 
 namespace {
 
-constexpr int BM = 128, BN = 256, BK = 128;             // BK in elements = bytes
-constexpr int A_STAGE = BM * 128, B_STAGE = BN * 128;    // 16 KiB, 32 KiB
-constexpr int SFA_BYTES = 512, SFB_BYTES = 1024;         // one / two 128-row scale atoms per stage
-constexpr int STAGE_BYTES = A_STAGE + B_STAGE + SFA_BYTES + SFB_BYTES;
-constexpr int STAGES = 3;
-constexpr int EPI_BUF = 128 * 128, EPI_BUFS = 2;
-constexpr int SMEM_BYTES = STAGES * (A_STAGE + B_STAGE) + STAGES * (SFA_BYTES + SFB_BYTES) + EPI_BUFS * EPI_BUF + 256 + 1024;
-constexpr int NUM_THREADS = 256;   // warp 0 TMA, 1 MMA, 2 TMEM alloc, 3 idle, 4-7 epilogue
-constexpr int TMEM_COLS = 512;
-constexpr int COL_SFA = 256, COL_SFB = 260;
+constexpr int BM = 128, BN = 128, BK = 128;             // BK in elements = bytes
+constexpr int A_STAGE = BM * 128, B_STAGE = BN * 128;    // 16 KiB each
+constexpr int SF_BYTES = 512;                            // one 128-row scale atom per operand and stage
+constexpr int STAGE_BYTES = A_STAGE + B_STAGE + 2 * SF_BYTES;
+constexpr int STAGES = 4;
+constexpr int SMEM_BYTES = STAGES * (A_STAGE + B_STAGE) + STAGES * 2 * SF_BYTES + 256 + 1024;
+constexpr int NUM_THREADS = 384;   // warpgroup 0: TMA producer (one thread); warpgroups 1, 2: MMA + epilogue
 
 struct MxParams {
   int M, N, K, tiles_m, tiles_n, mblk128, nblk128;
   const uint8_t* sfa;   // [K/128][ceil(M/128)][512]
   const uint8_t* sfb;   // [K/128][ceil(N/128) padded to even][512]
   const float* bias;
+  __nv_bfloat16* d;
+  long long ldd;
 };
 
 __device__ __forceinline__ void bulk_load(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
@@ -52,80 +49,39 @@ __device__ __forceinline__ void bulk_load(void* smem_dst, const void* gsrc, uint
                "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-// shared-memory descriptor of a scale atom for tcgen05.cp: 32 rows of 16 bytes, no swizzle, 8-row groups 128 bytes apart
-__device__ __forceinline__ uint64_t sf_smem_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(16 >> 4) << 16;     // leading byte offset (one 16-byte column only)
-  d |= static_cast<uint64_t>(128 >> 4) << 32;    // stride byte offset between 8-row groups
-  d |= static_cast<uint64_t>(1) << 46;           // descriptor version 1 (Blackwell); layout type 0 = no swizzle
-  return d;
-}
-__device__ __forceinline__ void tmem_cp_32x128b_warpx4(uint32_t taddr, uint64_t sdesc) {
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(taddr), "l"(sdesc) : "memory");
-}
-__device__ __forceinline__ void tc_mma_mxf8_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate,
-                                               uint32_t sfa_tmem, uint32_t sfb_tmem) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(sfa_tmem), "r"(sfb_tmem)
-      : "memory");
-}
-// kind::mxf8f6f4.block_scale instruction descriptor: E4M3 x E4M3, both K-major, E8M0 scales
-__device__ __forceinline__ uint32_t make_idesc_mx(int M, int N, uint32_t a_sf_id, uint32_t b_sf_id) {
-  return (b_sf_id << 4)                   // B scale-factor id (byte of the TMEM word)
-         | (0u << 7) | (0u << 10)         // A, B format = E4M3
-         | (uint32_t(N >> 3) << 17)       // N / 8
-         | (1u << 23)                     // scale format = E8M0
-         | (uint32_t(M >> 4) << 24)       // M / 16
-         | (a_sf_id << 29);               // A scale-factor id
-}
+// E8M0 -> fp32: 2^(e - 127); e = 0 is 2^-127 (a denormal)
+__device__ __forceinline__ float e8m0(uint32_t e) { return e ? __uint_as_float(e << 23) : __uint_as_float(0x00400000u); }
 
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_mx_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmD,
-               const MxParams p) {
+gemm_mx_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const MxParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = sA + STAGES * A_STAGE;
-  uint8_t* sE = sB + STAGES * B_STAGE;
-  uint8_t* sSFA = sE + EPI_BUFS * EPI_BUF;
-  uint8_t* sSFB = sSFA + STAGES * SFA_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(sSFB + STAGES * SFB_BYTES);
+  uint8_t* sSFA = sB + STAGES * B_STAGE;
+  uint8_t* sSFB = sSFA + STAGES * SF_BYTES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(sSFB + STAGES * SF_BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint64_t* tempty = tfull + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(full + 16);
 
-  const int warp = __shfl_sync(0xffffffff, threadIdx.x >> 5, 0);
+  const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
-    prefetch_tmap(&tmD);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 8);   // one arrival per MMA warp
     }
-    mbar_init(tfull, 1);
-    mbar_init(tempty, 4);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc<TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int num_tiles = p.tiles_m * p.tiles_n;
   const int num_kb = (p.K + BK - 1) / BK;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    regs_dealloc<40>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
@@ -135,8 +91,8 @@ gemm_mx_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           mbar_expect_tx(&full[stage], STAGE_BYTES);
           tma_load_2d(sA + stage * A_STAGE, &tmA, &full[stage], kb * BK, m_blk * BM);
           tma_load_2d(sB + stage * B_STAGE, &tmB, &full[stage], kb * BK, n_blk * BN);
-          bulk_load(sSFA + stage * SFA_BYTES, p.sfa + ((long long)kb * p.mblk128 + m_blk) * 512, SFA_BYTES, &full[stage]);
-          bulk_load(sSFB + stage * SFB_BYTES, p.sfb + ((long long)kb * p.nblk128 + 2 * n_blk) * 512, SFB_BYTES, &full[stage]);
+          bulk_load(sSFA + stage * SF_BYTES, p.sfa + ((long long)kb * p.mblk128 + m_blk) * 512, SF_BYTES, &full[stage]);
+          bulk_load(sSFB + stage * SF_BYTES, p.sfb + ((long long)kb * p.nblk128 + n_blk) * 512, SF_BYTES, &full[stage]);
           if (++stage == STAGES) {
             stage = 0;
             phase ^= 1;
@@ -144,107 +100,67 @@ gemm_mx_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
+  } else {
+    regs_alloc<232>();
+    const int cw = wg - 1;
+    const int wq = (threadIdx.x >> 5) & 3;
+    const int g = lane >> 2, t4 = lane & 3;
+    const int r0 = cw * 64 + wq * 16 + g;        // this thread's rows inside the tile: r0, r0 + 8
     int stage = 0;
-    uint32_t phase = 0, acc_phase = 0;
+    uint32_t phase = 0;
+    float acc[64], part[64];
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      mbar_wait(tempty, acc_phase ^ 1);
-      tc_fence_after();
+      const int m_blk = t % p.tiles_m, n_blk = t / p.tiles_m;
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        const uint32_t a_base = smem_u32(sA + stage * A_STAGE), b_base = smem_u32(sB + stage * B_STAGE);
-        if (elect_one()) {
-          // this stage's scale factors: shared memory -> TMEM (ordered before the MMAs below by the tcgen05 pipe)
-          tmem_cp_32x128b_warpx4(tmem_base + COL_SFA, sf_smem_desc(smem_u32(sSFA + stage * SFA_BYTES)));
-          tmem_cp_32x128b_warpx4(tmem_base + COL_SFB, sf_smem_desc(smem_u32(sSFB + stage * SFB_BYTES)));
-          tmem_cp_32x128b_warpx4(tmem_base + COL_SFB + 4, sf_smem_desc(smem_u32(sSFB + stage * SFB_BYTES + 512)));
+        const uint64_t ad = desc_sw128(sA + stage * A_STAGE + cw * 64 * 128, 16);
+        const uint64_t bd = desc_sw128(sB + stage * B_STAGE, 16);
+        const uint8_t* sfa = sSFA + stage * SF_BYTES;
+        const uint8_t* sfb = sSFB + stage * SF_BYTES;
+#pragma unroll 1
+        for (int kg = 0; kg < 4; ++kg) {
+          wgmma_fence();
+          wgmma_e4m3_e4m3_n128(part, desc_add(ad, kg * 32), desc_add(bd, kg * 32), 0u);
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_regs(part);
+          const float sa0 = e8m0(sfa[(r0 % 32) * 16 + (r0 / 32) * 4 + kg]);
+          const float sa1 = e8m0(sfa[((r0 + 8) % 32) * 16 + ((r0 + 8) / 32) * 4 + kg]);
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t adesc = (uint64_t(kDescHiSw128) << 32) | (smem_desc_lo(a_base, 16) + uint32_t((k * 32) >> 4));
-            const uint64_t bdesc = (uint64_t(kDescHiSw128) << 32) | (smem_desc_lo(b_base, 16) + uint32_t((k * 32) >> 4));
-            tc_mma_mxf8_ss(tmem_base, adesc, bdesc, make_idesc_mx(BM, BN, k, k), (kb > 0 || k > 0) ? 1u : 0u, tmem_base + COL_SFA,
-                           tmem_base + COL_SFB);
+          for (int j = 0; j < 16; ++j) {
+            const int c = 8 * j + 2 * t4;
+            const float sb0 = e8m0(sfb[(c % 32) * 16 + (c / 32) * 4 + kg]);
+            const float sb1 = e8m0(sfb[((c + 1) % 32) * 16 + ((c + 1) / 32) * 4 + kg]);
+            acc[4 * j] = fmaf(part[4 * j], sa0 * sb0, acc[4 * j]);
+            acc[4 * j + 1] = fmaf(part[4 * j + 1], sa0 * sb1, acc[4 * j + 1]);
+            acc[4 * j + 2] = fmaf(part[4 * j + 2], sa1 * sb0, acc[4 * j + 2]);
+            acc[4 * j + 3] = fmaf(part[4 * j + 3], sa1 * sb1, acc[4 * j + 3]);
           }
-          tc_commit(&empty[stage]);
         }
         __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[stage]);
         if (++stage == STAGES) {
           stage = 0;
           phase ^= 1;
         }
       }
-      if (elect_one()) tc_commit(tfull);
-      __syncwarp();
-      acc_phase ^= 1;
-    }
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    const int row_in_tile = q * 32 + lane;
-    const bool issuer = (threadIdx.x == 128);
-    const uint32_t swz = (row_in_tile & 7);
-    int ebuf = 0;
-    uint32_t acc_phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const int m_blk = t % p.tiles_m, n_blk = t / p.tiles_m;
-      mbar_wait(tfull, acc_phase);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < BN / 64; ++c) {
-        const int col0 = n_blk * BN + c * 64;
-        if (col0 >= p.N) break;
-        float v[64];
-        {
-          uint32_t r[32];
-          const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16) + c * 64;
-          tmem_ld_32x32(taddr, r);
-          tmem_ld_wait();
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-          tmem_ld_32x32(taddr + 32, r);
-          tmem_ld_wait();
+      for (int h = 0; h < 2; ++h) {
+        const long long row = (long long)m_blk * BM + r0 + 8 * h;
+        if (row >= p.M) continue;
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[32 + j] = __uint_as_float(r[j]);
+        for (int j = 0; j < 16; ++j) {
+          const int col = n_blk * BN + 8 * j + 2 * t4;
+          if (col >= p.N) continue;
+          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          if (p.bias != nullptr) v0 += __ldg(p.bias + col), v1 += __ldg(p.bias + col + 1);
+          *reinterpret_cast<uint32_t*>(p.d + row * p.ldd + col) = pack_bf16(v0, v1);
         }
-        if (p.bias != nullptr) {
-#pragma unroll
-          for (int j = 0; j < 64; j += 4) {
-            if (col0 + j < p.N) {
-              const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + j));
-              v[j] += b.x, v[j + 1] += b.y, v[j + 2] += b.z, v[j + 3] += b.w;
-            }
-          }
-        }
-        uint8_t* buf = sE + ebuf * EPI_BUF;
-        if (issuer) tma_wait_read<EPI_BUFS - 1>();
-        named_bar_sync(1, 128);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          uint4 o;
-          o.x = pack_bf16(v[8 * j], v[8 * j + 1]);
-          o.y = pack_bf16(v[8 * j + 2], v[8 * j + 3]);
-          o.z = pack_bf16(v[8 * j + 4], v[8 * j + 5]);
-          o.w = pack_bf16(v[8 * j + 6], v[8 * j + 7]);
-          *reinterpret_cast<uint4*>(buf + row_in_tile * 128 + ((j ^ swz) << 4)) = o;
-        }
-        fence_proxy_async_smem();
-        named_bar_sync(1, 128);
-        if (issuer) {
-          tma_store_2d(&tmD, buf, col0, m_blk * BM);
-          tma_commit();
-        }
-        ebuf = (ebuf + 1) % EPI_BUFS;
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty);
-      acc_phase ^= 1;
     }
-    if (issuer) tma_wait_all<0>();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc<TMEM_COLS>(tmem_base);
 }
 
 // bf16 [R, K] (row stride ld) -> E4M3 [R, K] + E8M0 scale atoms [K/128][ceil(R/128) (padded to rblk)][512]; one thread = 8 elements,
@@ -294,7 +210,7 @@ void mx_quantize(const void* x_bf16, long long ld, void* q8, void* sf, long long
   if (K % 128) throw std::runtime_error("mx_quantize: K must be a multiple of 128");
   const long long groups = R * (K / 8);
   long long blocks = (groups + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   mx_quantize_kernel<<<int(blocks), 256, 0, st>>>((const __nv_bfloat16*)x_bf16, ld, (uint8_t*)q8, (uint8_t*)sf, R, K, rblk);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) throw std::runtime_error(std::string("mx_quantize launch: ") + cudaGetErrorString(e));
@@ -305,21 +221,21 @@ void gemm_mxfp8_launch(const void* A, const void* B, void* D, const void* sfa, c
   if (K % 128 || N % 8) throw std::runtime_error("gemm_mxfp8: K must be a multiple of 128 and N of 8");
   CUtensorMap ta = make_tmap_2d(A, 1, false, K, M, K, BK, BM);
   CUtensorMap tb = make_tmap_2d(B, 1, false, K, N, K, BK, BN);
-  CUtensorMap td = make_tmap_2d(D, 2, false, N, M, ldd * 2, 64, BM);
   MxParams p{};
   p.M = M, p.N = N, p.K = K;
   p.tiles_m = (M + BM - 1) / BM, p.tiles_n = (N + BN - 1) / BN;
-  p.mblk128 = p.tiles_m, p.nblk128 = 2 * p.tiles_n;
+  p.mblk128 = p.tiles_m, p.nblk128 = 2 * ((N + 255) / 256);
   p.sfa = reinterpret_cast<const uint8_t*>(sfa), p.sfb = reinterpret_cast<const uint8_t*>(sfb), p.bias = bias;
+  p.d = reinterpret_cast<__nv_bfloat16*>(D), p.ldd = ldd;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(gemm_mx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e != cudaSuccess) throw std::runtime_error(std::string("gemm_mxfp8 smem attr: ") + cudaGetErrorString(e));
     configured = true;
   }
-  int sms = num_sms > 0 ? num_sms : 148;
+  int sms = num_sms > 0 ? num_sms : 132;
   const int tiles = p.tiles_m * p.tiles_n;
-  gemm_mx_kernel<<<tiles < sms ? tiles : sms, NUM_THREADS, SMEM_BYTES, stream>>>(ta, tb, td, p);
+  gemm_mx_kernel<<<tiles < sms ? tiles : sms, NUM_THREADS, SMEM_BYTES, stream>>>(ta, tb, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) throw std::runtime_error(std::string("gemm_mxfp8 launch: ") + cudaGetErrorString(e));
 }

@@ -1,12 +1,15 @@
-// Persistent, warp-specialised bf16 GEMM for sm_100a:  D[M,N] = A[M,K] * B[N,K]^T  (+ fused epilogue)
+// Persistent, warp-specialised GEMM for sm_90a:  D[M,N] = A[M,K] * B[N,K]^T  (+ fused epilogue)
 //
-//   * operands staged global->shared by TMA (cp.async.bulk.tensor, 128B swizzle), 3-stage mbarrier ring
-//   * tcgen05.mma (kind::f16, M=128 N=256 K=16) issued by ONE thread, accumulators in TMEM
-//     (2 x 256 fp32 columns, double-buffered so tile i's epilogue overlaps tile i+1's MMAs)
-//   * epilogue warps: tcgen05.ld TMEM->registers, fused bias / residual / GELU / dGELU, pack,
-//     swizzled st.shared, TMA store (or TMA reduce-add for fp32 weight-gradient accumulation)
-//   * either operand may be K-major ([rows,K] row-major) or MN-major ([K,rows] row-major) so forward,
-//     dgrad (B = W as stored) and wgrad (A = dY^T, B = X^T as stored) need no transposes.
+//   * operands staged global->shared by TMA (cp.async.bulk.tensor, 128B swizzle), 4-stage mbarrier ring filled by one
+//     producer thread (its warpgroup hands its registers to the MMA warpgroups with setmaxnreg)
+//   * two MMA warpgroups, 64 rows of the 128 x 256 tile each: wgmma.mma_async (bf16: m64n256k16, fp8: m64n256k32) with the
+//     fp32 accumulators in registers; a stage is released as soon as the next stage's MMAs are issued (wait_group 1)
+//   * epilogue straight from the accumulator registers: bias / residual / GELU / dGELU / fp8 re-quantisation, bf16 or fp32
+//     stores (fp32 weight-gradient accumulation and split-K partials by red.global.add)
+//   * bf16 operands may be K-major ([rows,K] row-major) or MN-major ([K,rows] row-major) so forward, dgrad (B = W as stored)
+//     and wgrad (A = dY^T, B = X^T as stored) need no transposes; wgmma reads 8-bit operands K-major only, so an MN-major fp8
+//     operand is transposed into scratch first (transpose_u8)
+//   * cluster 2: two CTAs on M-adjacent tiles share the B tile - each loads half of it and TMA multicasts it to both
 //
 // Replaces the cuBLASLt calls the reference reaches through torch (SURVEY §2.5 K3,K5-K8,K10).
 #include <cuda.h>
@@ -18,48 +21,38 @@
 
 #include "gemm_tcgen05.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace pb {
 
 namespace {
 
 constexpr int BM = 128, BN = 256;
-// A stage holds 128 BYTES of K per row for either operand type: 64 bf16 (4 UMMA k-steps of 16) or 128 fp8 (4 k-steps of 32),
-// so the shared-memory plan, the TMA box bytes and the descriptor arithmetic are the same for kind::f16 and kind::f8f6f4.
+// A stage holds 128 BYTES of K per row for either operand type: 64 bf16 (4 k-steps of 16) or 128 fp8 (4 k-steps of 32),
+// so the shared-memory plan, the TMA box bytes and the descriptor arithmetic are the same for both.
 constexpr int ROW_BYTES = 128;
-constexpr int A_STAGE = BM * ROW_BYTES;  // 16 KiB
-constexpr int EPI_BUF = 128 * 128;    // 128 rows x 128 B (one swizzle atom wide)
-constexpr int NUM_THREADS = 384;   // warp 0 TMA, 1 MMA, 2 TMEM alloc, 3 idle, 4-11 epilogue (two groups of four)
-constexpr int TMEM_COLS = 512;
-
-// Shared-memory plan per (epilogue, cluster) variant. A CTA of a pair stages only HALF of the B tile, so a stage is
-// 32 instead of 48 KiB and the same 227 KiB hold a 5-deep instead of a 3-deep TMA pipeline (plus 64 KiB of epilogue
-// staging): ~2500 instead of ~1500 tensor-core clocks of loads in flight per SM.
-template <int EPI, int CL>
-struct Cfg {
-  static constexpr int B_STAGE = (BN / CL) * ROW_BYTES;   // 32 KiB (CL=1) / 16 KiB (CL=2)
-  static constexpr int STAGE_BYTES = A_STAGE + B_STAGE;
-  static constexpr int STORES = (EPI == EPI_GELU_DUAL || EPI == EPI_GELU_GRAD) ? 2 : 1;   // staging buffers consumed per epilogue chunk
-  // two epilogue groups (even / odd column chunks of a tile), two staging buffers each: the exact-erf GELU epilogues
-  // measured ALU-bound with one epilogue warp per SM sub-partition (dGELU dgrad 634 TFLOP/s against 1400+ for the
-  // plain epilogue on the same shape)
-  static constexpr int EPI_BUFS_G = 2;
-  static constexpr int EPI_BUFS = 2 * EPI_BUFS_G;
-  static constexpr int STAGES = (CL == 1) ? 3 : 5;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BUFS * EPI_BUF + 256 + 1024;
-  static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KiB dynamic shared memory of sm_100");
-};
+constexpr int A_STAGE = BM * ROW_BYTES;   // 16 KiB
+constexpr int B_STAGE = BN * ROW_BYTES;   // 32 KiB
+constexpr int STAGE_BYTES = A_STAGE + B_STAGE;
+constexpr int STAGES = 4;
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;
+static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KiB dynamic shared memory of sm_90");
+constexpr int NUM_THREADS = 384;   // warpgroup 0: TMA producer (one thread); warpgroups 1, 2: MMA + epilogue
 
 struct Params {
   int M, N, K;
   int tiles_m, tiles_n, m_fastest;
   const float* bias;            // [N] fp32 or nullptr
-  const __nv_bfloat16* aux;     // residual (EPI_RESIDUAL) or pre-activation z (EPI_DGELU)
+  const __nv_bfloat16* aux;     // residual (EPI_RESIDUAL) or pre-activation z (EPI_DGELU) or multiplier (EPI_MUL)
   long long ld_aux;             // row stride of aux, elements
+  void* d;                      // primary output (bf16, or fp32 for EPI_F32)
+  long long ldd;
+  __nv_bfloat16* d2;            // second output of the two-output epilogues
+  long long ldd2;
   int accumulate;               // EPI_F32: reduce-add into D instead of overwrite
   float alpha;                  // scale applied to the accumulator before the epilogue
   int splits, kb_per_split;     // split-K (EPI_F32 + accumulate): work item = (tile, k-range)
-  // fp8 (kind::f8f6f4) operands: element formats (0 = E4M3, 1 = E5M2) and the per-tensor de-scales, read from device memory
+  // fp8 operands: element formats (0 = E4M3, 1 = E5M2) and the per-tensor de-scales, read from device memory
   // (delayed scaling keeps them on the device so the whole step stays CUDA-graph capturable)
   int a_fmt, b_fmt;
   const float* sinv_a;
@@ -71,63 +64,44 @@ struct Params {
   float* out_amax;
 };
 
-// CL = 1: one CTA per 128x256 tile (tcgen05 cta_group::1).
-// CL = 2: a CTA PAIR (two SMs of one TPC, cluster 2x1x1) computes a 256x256 tile with ONE tcgen05.mma.cta_group::2
-//         per k-step, issued by the leader CTA: each CTA stages its own 128 A rows and HALF of the B tile (128 of the
-//         256 N rows), the tensor cores of both SMs read both halves, each SM accumulates its 128 rows in its own TMEM.
-//         Per SM this halves the B traffic through shared memory (the 1-CTA form is smem-bandwidth bound: 96 B/clk of
-//         MMA operand reads + 96 B/clk of TMA writes against a 128 B/clk port) and needs 32 instead of 48 KiB per stage.
+__device__ __forceinline__ uint16_t pack_e4m3x2(float a, float b) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(b), "f"(a));   // first source -> upper byte
+  return r;
+}
+
+// CL = 1: one CTA per 128x256 tile.
+// CL = 2: a cluster of two CTAs computes two M-adjacent 128x256 tiles that share their B tile: each CTA loads 128 of the 256
+//         B rows and multicasts them into both CTAs' shared memory, halving the L2 -> SM traffic of B. A stage may only be
+//         refilled when the MMA warpgroups of BOTH CTAs released it, so every consumer warp arrives on both empty barriers.
 template <int A_MN, int B_MN, int EPI, int CL, int F8>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmD2, const Params p) {
-  using C = Cfg<EPI, CL>;
-  constexpr int STAGES = C::STAGES, B_STAGE = C::B_STAGE, STAGE_BYTES = C::STAGE_BYTES, EPI_BUFS = C::EPI_BUFS;
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Params p) {
   constexpr int BK = F8 ? 128 : 64;            // K elements per stage (128 bytes per row)
-  constexpr int UK = F8 ? 32 : 16;             // K elements per tcgen05.mma
   constexpr int MNC = F8 ? 128 : 64;           // MN elements in one 128-byte row of an MN-major tile
   constexpr int CHUNK = BK * ROW_BYTES;        // bytes of one MN-major chunk: BK k-rows of 128 bytes
+  static_assert(!F8 || (!A_MN && !B_MN), "8-bit wgmma operands are K-major");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = sA + STAGES * A_STAGE;
-  uint8_t* sE = sB + STAGES * B_STAGE;
-  uint64_t* full = reinterpret_cast<uint64_t*>(sE + EPI_BUFS * EPI_BUF);
+  uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * B_STAGE);
   uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(full + 24);   // own 64-byte line, away from the mbarrier words (<= 18 of them)
 
-  const int warp = __shfl_sync(0xffffffff, threadIdx.x >> 5, 0);
+  const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
+  const uint32_t crank = (CL > 1) ? cluster_ctarank() : 0;
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
-    prefetch_tmap(&tmD);
-    if (EPI == EPI_GELU_DUAL || EPI == EPI_GELU_GRAD || EPI == EPI_GELU_GRAD_Q8) prefetch_tmap(&tmD2);
-  }
-  const uint32_t crank = (CL > 1) ? cluster_ctarank() : 0;
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full[s], CL);   // CL = 2: leader's arrive.expect_tx + the peer's remote arrive (bytes of both land here)
-      mbar_init(&empty[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull[a], 1);
-      mbar_init(&tempty[a], 8 * CL);  // one arrival per epilogue warp (of both CTAs: the leader's MMA warp waits for the pair)
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 8 * CL);   // one arrival per MMA warp of every CTA that reads the stage
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    if (CL > 1) tmem_alloc_2sm<TMEM_COLS>(tmem_slot);
-    else tmem_alloc<TMEM_COLS>(tmem_slot);
-  }
-  tc_fence_before();
   __syncthreads();
-  if (CL > 1) cluster_sync_all();  // peer barriers initialised before any remote arrive / 2-SM TMA / multicast commit
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (CL > 1) cluster_sync_all();   // peer barriers initialised before any multicast / remote arrive
 
   // work decomposition: units of CL M-adjacent tiles; every CTA of a cluster walks the same unit sequence
   const int tiles_mu = (p.tiles_m + CL - 1) / CL;
@@ -136,9 +110,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const int num_work = num_tiles * p.splits;
   const int w0 = blockIdx.x / CL, wstride = gridDim.x / CL;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ======================= TMA producer (one thread) =======================
-    if (lane == 0) {
+    regs_dealloc<40>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int w = w0; w < num_work; w += wstride) {
@@ -147,321 +122,194 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const int n_blk = p.m_fastest ? tile / tiles_mu : tile % p.tiles_n;
         const int kb0 = sp * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
         for (int kb = kb0; kb < kb1; ++kb) {
-          if (CL > 1) {
-            // CTA pair: stage = own A rows (16 KiB) + own half of B (16 KiB); all bytes are credited to the LEADER's
-            // full barrier, which expects 2 x 32 KiB; the peer additionally arrives remotely
-            mbar_wait(&empty[stage], phase ^ 1);
-            uint8_t* a_dst = sA + stage * A_STAGE;
-            uint8_t* b_dst = sB + stage * B_STAGE;
-            if (crank == 0) mbar_expect_tx(&full[stage], 2 * STAGE_BYTES);
-            if (A_MN) {
-#pragma unroll
-              for (int j = 0; j < BM / MNC; ++j)
-                tma_load_2d_2sm(a_dst + j * CHUNK, &tmA, &full[stage], m_blk * BM + j * MNC, kb * BK);
-            } else {
-              tma_load_2d_2sm(a_dst, &tmA, &full[stage], kb * BK, m_blk * BM);
-            }
-            if (B_MN) {
-#pragma unroll
-              for (int j = 0; j < BN / 2 / MNC; ++j)
-                tma_load_2d_2sm(b_dst + j * CHUNK, &tmB, &full[stage], n_blk * BN + (crank * (BN / 2 / MNC) + j) * MNC, kb * BK);
-            } else {
-              tma_load_2d_2sm(b_dst, &tmB, &full[stage], kb * BK, n_blk * BN + crank * (BN / 2));
-            }
-            if (crank != 0) mbar_arrive_remote(&full[stage], 0);
-            if (++stage == STAGES) {
-              stage = 0;
-              phase ^= 1;
-            }
-            continue;
-          }
           mbar_wait(&empty[stage], phase ^ 1);
           mbar_expect_tx(&full[stage], STAGE_BYTES);
           uint8_t* a_dst = sA + stage * A_STAGE;
           uint8_t* b_dst = sB + stage * B_STAGE;
           if (A_MN) {
 #pragma unroll
-            for (int j = 0; j < BM / MNC; ++j)
-              tma_load_2d(a_dst + j * CHUNK, &tmA, &full[stage], m_blk * BM + j * MNC, kb * BK);
+            for (int j = 0; j < BM / MNC; ++j) tma_load_2d(a_dst + j * CHUNK, &tmA, &full[stage], m_blk * BM + j * MNC, kb * BK);
           } else {
             tma_load_2d(a_dst, &tmA, &full[stage], kb * BK, m_blk * BM);
           }
-          if (B_MN) {
+          if (CL == 1) {
+            if (B_MN) {
 #pragma unroll
-            for (int j = 0; j < BN / MNC; ++j)
-              tma_load_2d(b_dst + j * CHUNK, &tmB, &full[stage], n_blk * BN + j * MNC, kb * BK);
+              for (int j = 0; j < BN / MNC; ++j) tma_load_2d(b_dst + j * CHUNK, &tmB, &full[stage], n_blk * BN + j * MNC, kb * BK);
+            } else {
+              tma_load_2d(b_dst, &tmB, &full[stage], kb * BK, n_blk * BN);
+            }
           } else {
-            tma_load_2d(b_dst, &tmB, &full[stage], kb * BK, n_blk * BN);
-          }
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ======================= MMA issuer =======================
-    // The whole warp walks the loop (waits included) so every operand is warp-uniform; one elected lane issues the
-    // tcgen05 instructions. (`if (lane == 0)` around the loop costs a ~20-instruction elect/broadcast round trip per MMA.)
-    if (crank == 0) {
-      const uint32_t idesc = F8 ? make_idesc_f8(BM * CL, BN, A_MN, B_MN, p.a_fmt, p.b_fmt) : make_idesc_bf16(BM * CL, BN, A_MN, B_MN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int w = w0; w < num_work; w += wstride) {
-        const int sp = w / num_tiles;
-        const int kb0 = sp * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
-        mbar_wait(&tempty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t a_base = smem_u32(sA + stage * A_STAGE);
-          const uint32_t b_base = smem_u32(sB + stage * B_STAGE);
-          const uint32_t ad0 = smem_desc_lo(a_base, A_MN ? CHUNK : 16);
-          const uint32_t bd0 = smem_desc_lo(b_base, B_MN ? CHUNK : 16);
+            // this CTA's half of B lands in both CTAs and completes bytes on both CTAs' full barrier of this stage
+            if (B_MN) {
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {   // BK / UK = 4 for both operand types
-            // k-step inside the stage: UK rows of 128 B (MN-major) or 32 bytes of K (K-major), in 16-byte descriptor units
-            const uint32_t adesc = ad0 + uint32_t(A_MN ? (k * UK * 128) >> 4 : (k * 32) >> 4);
-            const uint32_t bdesc = bd0 + uint32_t(B_MN ? (k * UK * 128) >> 4 : (k * 32) >> 4);
-            if (elect_one()) {
-              const uint32_t accum = (kb > kb0 || k > 0) ? 1u : 0u;
-              if (F8) {
-                if (CL > 1) tc_mma_f8_ss_2sm_lo(d_tmem, adesc, bdesc, idesc, accum);
-                else tc_mma_f8_ss_lo(d_tmem, adesc, bdesc, idesc, accum);
-              } else {
-                if (CL > 1) tc_mma_f16_ss_2sm_lo(d_tmem, adesc, bdesc, idesc, accum);
-                else tc_mma_f16_ss_lo(d_tmem, adesc, bdesc, idesc, accum);
+              for (int j = 0; j < BN / 2 / MNC; ++j) {
+                const int c = crank * (BN / 2 / MNC) + j;
+                tma_load_2d_mc(b_dst + c * CHUNK, &tmB, &full[stage], n_blk * BN + c * MNC, kb * BK, 0x3);
               }
+            } else {
+              tma_load_2d_mc(b_dst + crank * (BN / 2) * ROW_BYTES, &tmB, &full[stage], kb * BK, n_blk * BN + crank * (BN / 2), 0x3);
             }
           }
-          if (elect_one()) {
-            if (CL > 1) tc_commit_2sm(&empty[stage], 0x3);  // release the stage in BOTH CTAs
-            else tc_commit(&empty[stage]);                  // frees the smem slot once these MMAs retire
-          }
-          __syncwarp();
           if (++stage == STAGES) {
             stage = 0;
             phase ^= 1;
           }
         }
-        if (elect_one()) {
-          if (CL > 1) tc_commit_2sm(&tfull[acc], 0x3);  // accumulator complete -> both CTAs' epilogues
-          else tc_commit(&tfull[acc]);
-        }
-        __syncwarp();
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
       }
     }
-  } else if (warp >= 4) {
-    // ======================= epilogue (2 groups x 4 warps, one TMEM lane quadrant each) =======================
-    // group g takes the column chunks c = g, g+2, ... of every tile with its own staging buffers, named barrier and
-    // TMA-store issuer: two epilogue warps per SM sub-partition
-    const int q = warp & 3;
-    const int grp = (warp - 4) >> 2;
-    const int row_in_tile = q * 32 + lane;
-    const bool issuer = (threadIdx.x == 128 + grp * 128);
-    uint8_t* sEg = sE + grp * (C::EPI_BUFS_G * EPI_BUF);
-    constexpr int EPI_BUFS_G = C::EPI_BUFS_G;
-    constexpr int CW = (EPI == EPI_F32) ? 32 : 64;             // columns per staged chunk (128 B wide)
-    constexpr int STORES = C::STORES;                           // staging buffers consumed per chunk
-    int ebuf = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const uint32_t swz = (row_in_tile & 7);
-    // fp8 operands: fold the per-tensor de-scales (device scalars written by the quantising producers) into alpha
+  } else {
+    // ======================= MMA + epilogue (warpgroups 1, 2: rows 64 * (wg - 1) .. of the tile) =======================
+    regs_alloc<232>();
+    const int cw = wg - 1;                       // which 64-row half of the tile
+    const int wq = (threadIdx.x >> 5) & 3;       // warp inside the warpgroup: 16 rows each
+    const int g = lane >> 2, t4 = lane & 3;
     float alpha = p.alpha;
     if (F8) alpha *= (p.sinv_a ? __ldg(p.sinv_a) : 1.0f) * (p.sinv_b ? __ldg(p.sinv_b) : 1.0f);
     const float q8_scale = (EPI == EPI_GELU_GRAD_Q8 && p.out_scale) ? __ldg(p.out_scale) : 1.0f;
     float q8_amax = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[128];
     for (int w = w0; w < num_work; w += wstride) {
-      const int tile = w % num_tiles;
+      const int tile = w % num_tiles, sp = w / num_tiles;
       const int m_blk = (p.m_fastest ? tile % tiles_mu : tile / p.tiles_n) * CL + crank;
       const int n_blk = p.m_fastest ? tile / tiles_mu : tile % p.tiles_n;
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      const long long row = (long long)m_blk * BM + row_in_tile;
-      const bool row_ok = row < p.M;
-#pragma unroll 1
-      for (int c = grp; c < BN / CW; c += 2) {
-        const int col0 = n_blk * BN + c * CW;
-        if (col0 >= p.N) break;  // whole chunk out of range (uniform)
-        // aux tile (residual / pre-activation) for this chunk: issue the global loads FIRST so their latency
-        // overlaps the TMEM read below
-        uint4 ax[8];
-        if (EPI == EPI_RESIDUAL || EPI == EPI_DGELU || EPI == EPI_MUL) {
-          const __nv_bfloat16* arow = p.aux + row * p.ld_aux + col0;
+      const int kb0 = sp * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint8_t* a_st = sA + stage * A_STAGE;
+        const uint8_t* b_st = sB + stage * B_STAGE;
+        // this warpgroup's 64 A rows: K-major -> 64 rows further; MN-major -> the cw-th 64-wide chunk (bf16 only)
+        const uint64_t ad = A_MN ? desc_sw128(a_st + cw * CHUNK, CHUNK) : desc_sw128(a_st + cw * 64 * ROW_BYTES, 16);
+        const uint64_t bd = B_MN ? desc_sw128(b_st, CHUNK) : desc_sw128(b_st, 16);
+        wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 8; ++j)
-            ax[j] = (row_ok && col0 + 8 * j < p.N) ? __ldg(reinterpret_cast<const uint4*>(arow + 8 * j)) : make_uint4(0, 0, 0, 0);
+        for (int k = 0; k < 4; ++k) {
+          // k-step inside the stage: 16 k-rows of 128 B (MN-major) or 32 bytes of K (K-major)
+          const uint64_t adk = desc_add(ad, A_MN ? k * 16 * ROW_BYTES : k * 32);
+          const uint64_t bdk = desc_add(bd, B_MN ? k * 16 * ROW_BYTES : k * 32);
+          const uint32_t accum = (kb > kb0 || k > 0) ? 1u : 0u;
+          if (F8) wgmma_f8_n256(acc, adk, bdk, accum, p.a_fmt, p.b_fmt);
+          else wgmma_bf16_ss_n256<A_MN, B_MN>(acc, adk, bdk, accum);
         }
-        float v[CW];
-        {
-          uint32_t r[32];
-          const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16) + acc * BN + c * CW;
-          tmem_ld_32x32(taddr, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * alpha;
-          if (CW == 64) {
-            tmem_ld_32x32(taddr + 32, r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[(CW == 64 ? 32 : 0) + j] = __uint_as_float(r[j]) * alpha;
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous stage's MMAs retired: release its shared memory
+        if (prev >= 0 && lane == 0) {
+          if (CL > 1) {
+            mbar_arrive_remote(&empty[prev], 0);
+            mbar_arrive_remote(&empty[prev], 1);
+          } else {
+            mbar_arrive(&empty[prev]);
           }
         }
-        if (EPI != EPI_F32 && p.bias != nullptr) {
-#pragma unroll
-          for (int j = 0; j < CW; j += 4) {
-            if (col0 + j < p.N) {
-              const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + j));
-              v[j] += b.x, v[j + 1] += b.y, v[j + 2] += b.z, v[j + 3] += b.w;
-            }
-          }
+        prev = stage;
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1;
         }
-        uint8_t* buf0 = sEg + ebuf * EPI_BUF;
-        uint8_t* buf1 = sEg + ((ebuf + 1) % EPI_BUFS_G) * EPI_BUF;
-        if (issuer) tma_wait_read<EPI_BUFS_G / STORES - 1>();
-        named_bar_sync(1 + grp, 128);
-        if (EPI == EPI_F32) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4 o = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-            *reinterpret_cast<float4*>(buf0 + row_in_tile * 128 + ((j ^ swz) << 4)) = o;
-          }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (prev >= 0 && lane == 0) {
+        if (CL > 1) {
+          mbar_arrive_remote(&empty[prev], 0);
+          mbar_arrive_remote(&empty[prev], 1);
         } else {
-          if (EPI == EPI_RESIDUAL || EPI == EPI_DGELU || EPI == EPI_MUL) {
+          mbar_arrive(&empty[prev]);
+        }
+      }
+      if (kb1 <= kb0) continue;
+      // ---------------------------------------------------------------- epilogue from registers
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              {
-                const uint4 a = ax[j];
-                const uint32_t w[4] = {a.x, a.y, a.z, a.w};
+      for (int h = 0; h < 2; ++h) {
+        const long long row = (long long)m_blk * BM + cw * 64 + wq * 16 + g + 8 * h;
+        if (row >= p.M) continue;
 #pragma unroll
-                for (int t = 0; t < 4; ++t) {
-                  const float2 f = unpack_bf16(w[t]);
-                  if (EPI == EPI_RESIDUAL) {
-                    v[8 * j + 2 * t] += f.x;
-                    v[8 * j + 2 * t + 1] += f.y;
-                  } else if (EPI == EPI_MUL) {
-                    v[8 * j + 2 * t] *= f.x;
-                    v[8 * j + 2 * t + 1] *= f.y;
-                  } else {
-                    v[8 * j + 2 * t] *= gelu_grad(f.x);
-                    v[8 * j + 2 * t + 1] *= gelu_grad(f.y);
-                  }
-                }
-              }
+        for (int j = 0; j < 32; ++j) {
+          const int col = n_blk * BN + 8 * j + 2 * t4;
+          if (col >= p.N) continue;   // N % 8 == 0: col + 1 < N as well
+          float v0 = acc[4 * j + 2 * h] * alpha, v1 = acc[4 * j + 2 * h + 1] * alpha;
+          if (EPI == EPI_F32) {
+            float* dst = reinterpret_cast<float*>(p.d) + row * p.ldd + col;
+            if (p.accumulate || p.splits > 1) {
+              red_add_f32x2(dst, v0, v1);
+            } else {
+              *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
             }
+            continue;
           }
-          if (EPI == EPI_GELU_GRAD) {
+          if (p.bias != nullptr) {
+            const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+            v0 += b.x, v1 += b.y;
+          }
+          if (EPI == EPI_RESIDUAL || EPI == EPI_DGELU || EPI == EPI_MUL) {
+            const float2 f = unpack_bf16(__ldg(reinterpret_cast<const uint32_t*>(p.aux + row * p.ld_aux + col)));
+            if (EPI == EPI_RESIDUAL) v0 += f.x, v1 += f.y;
+            else if (EPI == EPI_MUL) v0 *= f.x, v1 *= f.y;
+            else v0 *= gelu_grad(f.x), v1 *= gelu_grad(f.y);
+          }
+          __nv_bfloat16* drow = reinterpret_cast<__nv_bfloat16*>(p.d) + row * p.ldd + col;
+          if (EPI == EPI_GELU_DUAL) {
+            *reinterpret_cast<uint32_t*>(p.d2 + row * p.ldd2 + col) = pack_bf16(v0, v1);   // z (pre-activation)
+            v0 = gelu_exact(v0), v1 = gelu_exact(v1);
+          } else if (EPI == EPI_GELU_GRAD || EPI == EPI_GELU_GRAD_Q8) {
             // gelu and its derivative share the CDF / PDF evaluation; the derivative replaces the pre-activation as the
             // tensor saved for backward, so the dgrad epilogue is a plain multiply
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float d[8];
-#pragma unroll
-              for (int t = 0; t < 8; ++t) {
-                float c, pd;
-                gelu_cdf_pdf(v[8 * j + t], c, pd);
-                d[t] = fmaf(v[8 * j + t], pd, c);
-                v[8 * j + t] *= c;
-              }
-              uint4 o;
-              o.x = pack_bf16(d[0], d[1]), o.y = pack_bf16(d[2], d[3]), o.z = pack_bf16(d[4], d[5]), o.w = pack_bf16(d[6], d[7]);
-              *reinterpret_cast<uint4*>(buf1 + row_in_tile * 128 + ((j ^ swz) << 4)) = o;   // gelu'(z)
+            float c0, pd0, c1, pd1;
+            gelu_cdf_pdf(v0, c0, pd0);
+            gelu_cdf_pdf(v1, c1, pd1);
+            *reinterpret_cast<uint32_t*>(p.d2 + row * p.ldd2 + col) = pack_bf16(fmaf(v0, pd0, c0), fmaf(v1, pd1, c1));
+            v0 *= c0, v1 *= c1;
+            if (EPI == EPI_GELU_GRAD_Q8) {
+              q8_amax = fmaxf(q8_amax, fmaxf(fabsf(v0), fabsf(v1)));
+              *reinterpret_cast<uint16_t*>(p.d8 + row * p.ld_d8 + col) = pack_e4m3x2(v0 * q8_scale, v1 * q8_scale);
+              continue;
             }
           }
-          if (EPI == EPI_GELU_GRAD_Q8) {
-            // gelu'(z) -> v (staged + TMA-stored as bf16 below, through tmD2); gelu(z) -> E4M3 straight to global memory:
-            // each thread owns 64 consecutive bytes of one output row (two full 32-byte sectors)
-            uint32_t q[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              float a4[4];
-#pragma unroll
-              for (int t = 0; t < 4; ++t) {
-                float c, pd;
-                const float z = v[4 * j + t];
-                gelu_cdf_pdf(z, c, pd);
-                v[4 * j + t] = fmaf(z, pd, c);
-                a4[t] = z * c;
-                if (row_ok && col0 + 4 * j + t < p.N) q8_amax = fmaxf(q8_amax, fabsf(a4[t]));
-              }
-              q[j] = pack_e4m3x4(a4[0] * q8_scale, a4[1] * q8_scale, a4[2] * q8_scale, a4[3] * q8_scale);
-            }
-            if (row_ok) {
-              uint8_t* drow = p.d8 + row * p.ld_d8 + col0;
-#pragma unroll
-              for (int j = 0; j < 4; ++j)
-                if (col0 + 16 * j < p.N) *reinterpret_cast<uint4*>(drow + 16 * j) = make_uint4(q[4 * j], q[4 * j + 1], q[4 * j + 2], q[4 * j + 3]);
-            }
-          }
-          if (EPI == EPI_GELU_DUAL) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              uint4 o;
-              o.x = pack_bf16(v[8 * j], v[8 * j + 1]);
-              o.y = pack_bf16(v[8 * j + 2], v[8 * j + 3]);
-              o.z = pack_bf16(v[8 * j + 4], v[8 * j + 5]);
-              o.w = pack_bf16(v[8 * j + 6], v[8 * j + 7]);
-              *reinterpret_cast<uint4*>(buf1 + row_in_tile * 128 + ((j ^ swz) << 4)) = o;  // z (pre-activation)
-            }
-#pragma unroll
-            for (int j = 0; j < CW; ++j) v[j] = gelu_exact(v[j]);
-          }
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            uint4 o;
-            o.x = pack_bf16(v[8 * j], v[8 * j + 1]);
-            o.y = pack_bf16(v[8 * j + 2], v[8 * j + 3]);
-            o.z = pack_bf16(v[8 * j + 4], v[8 * j + 5]);
-            o.w = pack_bf16(v[8 * j + 6], v[8 * j + 7]);
-            *reinterpret_cast<uint4*>(buf0 + row_in_tile * 128 + ((j ^ swz) << 4)) = o;
-          }
+          *reinterpret_cast<uint32_t*>(drow) = pack_bf16(v0, v1);
         }
-        fence_proxy_async_smem();
-        named_bar_sync(1 + grp, 128);
-        if (issuer) {
-          if (EPI == EPI_F32 && (p.accumulate || p.splits > 1)) {
-            tma_reduce_add_2d(&tmD, buf0, col0, m_blk * BM);
-          } else if (EPI == EPI_GELU_GRAD_Q8) {
-            tma_store_2d(&tmD2, buf0, col0, m_blk * BM);
-          } else {
-            tma_store_2d(&tmD, buf0, col0, m_blk * BM);
-          }
-          if (EPI == EPI_GELU_DUAL || EPI == EPI_GELU_GRAD) tma_store_2d(&tmD2, buf1, col0, m_blk * BM);
-          tma_commit();
-        }
-        ebuf = (ebuf + STORES) % EPI_BUFS_G;
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (CL > 1 && crank != 0) mbar_arrive_remote(&tempty[acc], 0);
-        else mbar_arrive(&tempty[acc]);
-      }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
     }
-    if (issuer) tma_wait_all<0>();
     if (EPI == EPI_GELU_GRAD_Q8 && p.out_amax) {
       q8_amax = warp_max_f(q8_amax);
       if (lane == 0 && q8_amax > 0.f) atomic_max_pos_f32(p.out_amax, q8_amax);
     }
   }
+  if (CL > 1) cluster_sync_all();   // nobody leaves while the peer may still multicast into it or arrive on its barriers
+}
 
-  tc_fence_before();
-  __syncthreads();
-  if (CL > 1) cluster_sync_all();  // nobody leaves (or frees TMEM) while the pair's MMAs / remote arrives are in flight
-  if (warp == 2) {
-    if (CL > 1) tmem_dealloc_2sm<TMEM_COLS>(tmem_base);
-    else tmem_dealloc<TMEM_COLS>(tmem_base);
+// [R, C] bytes (row stride ld) -> [C, R] contiguous: makes an MN-major fp8 operand K-major for wgmma
+__global__ void __launch_bounds__(256) transpose_u8_kernel(const uint8_t* __restrict__ src, long long ld, uint8_t* __restrict__ dst, int R, int C) {
+  __shared__ uint8_t t[64][65];
+  const int r0 = blockIdx.y * 64, c0 = blockIdx.x * 64;
+  for (int i = threadIdx.x; i < 64 * 64; i += 256) {
+    const int r = i >> 6, c = i & 63;
+    t[r][c] = (r0 + r < R && c0 + c < C) ? src[(long long)(r0 + r) * ld + c0 + c] : 0;
   }
+  __syncthreads();
+  for (int i = threadIdx.x; i < 64 * 64; i += 256) {
+    const int c = i >> 6, r = i & 63;
+    if (r0 + r < R && c0 + c < C) dst[(long long)(c0 + c) * R + r0 + r] = t[r][c];
+  }
+}
+
+// Same for 64-aligned shapes and 16-byte aligned rows: 16-byte loads and stores, each thread gathers one 16-byte piece of an
+// output row from a column of the shared tile
+__global__ void __launch_bounds__(256) transpose_u8_v16_kernel(const uint8_t* __restrict__ src, long long ld, uint8_t* __restrict__ dst, int R) {
+  __shared__ __align__(16) uint8_t t[64][80];
+  const int r0 = blockIdx.y * 64, c0 = blockIdx.x * 64;
+  const int tr = threadIdx.x >> 2, tc = (threadIdx.x & 3) * 16;
+  *reinterpret_cast<uint4*>(&t[tr][tc]) = __ldg(reinterpret_cast<const uint4*>(src + (long long)(r0 + tr) * ld + c0 + tc));
+  __syncthreads();
+  uint32_t w[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int r = tc + 4 * q;
+    w[q] = uint32_t(t[r][tr]) | (uint32_t(t[r + 1][tr]) << 8) | (uint32_t(t[r + 2][tr]) << 16) | (uint32_t(t[r + 3][tr]) << 24);
+  }
+  *reinterpret_cast<uint4*>(dst + (long long)(c0 + tr) * R + r0 + tc) = make_uint4(w[0], w[1], w[2], w[3]);
 }
 
 // ------------------------------------------------------------------------------------------ host
@@ -503,19 +351,18 @@ CUtensorMap make_tmap_2d(const void* ptr, int elem_bytes, bool is_float32, uint6
 }
 
 template <int A_MN, int B_MN, int EPI, int CL, int F8>
-static void launch_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& td, const CUtensorMap& td2,
-                      const Params& p, int grid, cudaStream_t stream) {
+static void launch_cl(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, int grid, cudaStream_t stream) {
   auto kern = gemm_kernel<A_MN, B_MN, EPI, CL, F8>;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<EPI, CL>::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e != cudaSuccess) throw std::runtime_error(std::string("gemm smem attr: ") + cudaGetErrorString(e));
     configured = true;
   }
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = Cfg<EPI, CL>::SMEM_BYTES;
+  cfg.dynamicSmemBytes = SMEM_BYTES;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -524,51 +371,52 @@ static void launch_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CUtens
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, td, td2, p);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, p);
   if (e != cudaSuccess) throw std::runtime_error(std::string("gemm launch: ") + cudaGetErrorString(e));
 }
 
 template <int A_MN, int B_MN, int EPI, int F8>
-static void launch_inst(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& td, const CUtensorMap& td2,
-                        const Params& p, int grid, int cluster, cudaStream_t stream) {
-  if (cluster == 2) launch_cl<A_MN, B_MN, EPI, 2, F8>(ta, tb, td, td2, p, grid, stream);
-  else launch_cl<A_MN, B_MN, EPI, 1, F8>(ta, tb, td, td2, p, grid, stream);
+static void launch_inst(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, int grid, int cluster, cudaStream_t stream) {
+  if (cluster == 2) launch_cl<A_MN, B_MN, EPI, 2, F8>(ta, tb, p, grid, stream);
+  else launch_cl<A_MN, B_MN, EPI, 1, F8>(ta, tb, p, grid, stream);
 }
 
-// Operands are bf16 (kind::f16) or, with g.fp8, 8-bit floats (kind::f8f6f4: E4M3 / E5M2 chosen per operand, fp32 accumulate,
-// per-tensor de-scales applied in the epilogue). Everything else — pipeline, tile shape, epilogues — is shared.
+void transpose_u8(const void* src, long long ld, void* dst, int R, int C, cudaStream_t stream) {
+  const dim3 grid((C + 63) / 64, (R + 63) / 64);
+  if (R % 64 == 0 && C % 64 == 0 && ld % 16 == 0 && !(reinterpret_cast<uintptr_t>(src) & 15) && !(reinterpret_cast<uintptr_t>(dst) & 15))
+    transpose_u8_v16_kernel<<<grid, 256, 0, stream>>>((const uint8_t*)src, ld, (uint8_t*)dst, R);
+  else
+    transpose_u8_kernel<<<grid, 256, 0, stream>>>((const uint8_t*)src, ld, (uint8_t*)dst, R, C);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) throw std::runtime_error(std::string("transpose_u8 launch: ") + cudaGetErrorString(e));
+}
+
+// Operands are bf16 or, with g.fp8, 8-bit floats (E4M3 / E5M2 chosen per operand, fp32 accumulate, per-tensor de-scales
+// applied in the epilogue). Everything else — pipeline, tile shape, epilogues — is shared.
 void gemm_launch(const GemmArgs& g, cudaStream_t stream) {
   if (g.M <= 0 || g.N <= 0 || g.K <= 0) return;
   if (g.N % 8) throw std::runtime_error("photon_b200 gemm: N must be a multiple of 8");
+  if (g.fp8 && (g.a_mn || g.b_mn)) throw std::runtime_error("photon_b200 gemm: fp8 operands must be K-major (transpose_u8 first)");
   const bool f32 = g.epi == EPI_F32;
   const int eb = g.fp8 ? 1 : 2;                 // operand element bytes
   const int BKE = ROW_BYTES / eb;               // K elements per stage
   const int MNC = ROW_BYTES / eb;               // MN elements per 128-byte row of an MN-major tile
+  // 2-CTA clusters (B tile multicast to both) whenever there are >= 2 M tiles
+  const int cluster = (g.cluster > 0 ? g.cluster : ((g.M + BM - 1) / BM >= 2 ? 2 : 1));
   // A: K-major -> dims {K, M}, box {128 B of K, 128 rows};  MN-major -> dims {M, K}, box {128 B of M, BKE k-rows}
   CUtensorMap ta = g.a_mn ? make_tmap_2d(g.A, eb, false, g.M, g.K, g.lda * eb, MNC, BKE)
                           : make_tmap_2d(g.A, eb, false, g.K, g.M, g.lda * eb, BKE, BM);
-  // 2-CTA clusters (each CTA stages half of the B tile) whenever there are >= 2 M tiles
-  const int cluster = (g.cluster > 0 ? g.cluster : ((g.M + BM - 1) / BM >= 2 ? 2 : 1));
   CUtensorMap tb = g.b_mn ? make_tmap_2d(g.B, eb, false, g.N, g.K, g.ldb * eb, MNC, BKE)
                           : make_tmap_2d(g.B, eb, false, g.K, g.N, g.ldb * eb, BKE, BN / cluster);
   const bool two_out = g.epi == EPI_GELU_DUAL || g.epi == EPI_GELU_GRAD || g.epi == EPI_GELU_GRAD_Q8;
-  CUtensorMap td2{};
-  if (two_out) {
-    if (!g.D2) throw std::runtime_error("photon_b200 gemm: the two-output GELU epilogues need the second output");
-    td2 = make_tmap_2d(g.D2, 2, false, g.N, g.M, g.ldd2 * 2, 64, BM);
-  }
-  CUtensorMap td;
-  if (g.epi == EPI_GELU_GRAD_Q8) {
-    if (!g.fp8 || !g.D8 || (g.ldd8 % 16) || (reinterpret_cast<uintptr_t>(g.D8) & 15))
-      throw std::runtime_error("photon_b200 gemm: the fp8-output epilogue needs fp8 operands and a 16-byte aligned fp8 output");
-    td = td2;   // the primary output leaves by direct stores
-  } else {
-    td = f32 ? make_tmap_2d(g.D, 4, true, g.N, g.M, g.ldd * 4, 32, BM) : make_tmap_2d(g.D, 2, false, g.N, g.M, g.ldd * 2, 64, BM);
-  }
-  if (!two_out) td2 = td;
+  if (two_out && !g.D2) throw std::runtime_error("photon_b200 gemm: the two-output GELU epilogues need the second output");
+  if (g.epi == EPI_GELU_GRAD_Q8 && (!g.fp8 || !g.D8 || (g.ldd8 % 2) || (reinterpret_cast<uintptr_t>(g.D8) & 1)))
+    throw std::runtime_error("photon_b200 gemm: the fp8-output epilogue needs fp8 operands and a 2-byte aligned fp8 output with an even row stride");
   if ((g.epi == EPI_RESIDUAL || g.epi == EPI_DGELU || g.epi == EPI_MUL) && (!g.aux || (g.ld_aux % 8) || (reinterpret_cast<uintptr_t>(g.aux) & 15)))
     throw std::runtime_error("photon_b200 gemm: aux operand missing or not 16-byte aligned");
   if (g.bias && (reinterpret_cast<uintptr_t>(g.bias) & 15)) throw std::runtime_error("photon_b200 gemm: bias must be 16-byte aligned");
+  if (g.epi != EPI_GELU_GRAD_Q8 && ((reinterpret_cast<uintptr_t>(g.D) & 15) || (g.ldd % 8)))
+    throw std::runtime_error("photon_b200 gemm: output must be 16-byte aligned");
   Params p{};
   p.M = g.M, p.N = g.N, p.K = g.K;
   p.tiles_m = (g.M + BM - 1) / BM;
@@ -578,6 +426,8 @@ void gemm_launch(const GemmArgs& g, cudaStream_t stream) {
   p.bias = g.bias;
   p.aux = reinterpret_cast<const __nv_bfloat16*>(g.aux);
   p.ld_aux = g.ld_aux;
+  p.d = g.D, p.ldd = g.ldd;
+  p.d2 = reinterpret_cast<__nv_bfloat16*>(g.D2), p.ldd2 = g.ldd2;
   p.accumulate = g.accumulate;
   p.alpha = g.alpha;
   p.a_fmt = g.a_fmt, p.b_fmt = g.b_fmt, p.sinv_a = g.sinv_a, p.sinv_b = g.sinv_b;
@@ -593,7 +443,7 @@ void gemm_launch(const GemmArgs& g, cudaStream_t stream) {
   p.splits = 1;
   if (f32 && g.accumulate && tiles < sms && num_kb >= 16) {
     // few output tiles, long K (weight gradients): split K across CTAs, partials meet in the fp32
-    // gradient bucket through TMA reduce-add. Aim for ~2 waves, >= 8 k-blocks per split.
+    // gradient bucket through red.global.add. Aim for ~2 waves, >= 8 k-blocks per split.
     int s = (2 * sms + tiles / 2) / tiles;
     if (s > num_kb / 8) s = num_kb / 8;
     if (s < 1) s = 1;
@@ -610,7 +460,7 @@ void gemm_launch(const GemmArgs& g, cudaStream_t stream) {
 
 #define PB_CASE(AM, BMJ, E, F)                                              \
   if (g.a_mn == AM && g.b_mn == BMJ && g.epi == E && int(g.fp8) == F) {     \
-    launch_inst<AM, BMJ, E, F>(ta, tb, td, td2, p, grid, cluster, stream);  \
+    launch_inst<AM, BMJ, E, F>(ta, tb, p, grid, cluster, stream);           \
     return;                                                                 \
   }
   PB_CASE(0, 0, EPI_BF16, 0)
@@ -626,17 +476,13 @@ void gemm_launch(const GemmArgs& g, cudaStream_t stream) {
   PB_CASE(1, 1, EPI_BF16, 0)
   PB_CASE(1, 0, EPI_F32, 0)
   PB_CASE(1, 0, EPI_BF16, 0)
-  // fp8 operands: forward (K-major x K-major), dgrad (dY K-major x W MN-major), wgrad (both MN-major)
+  // fp8 operands (K-major; the bindings transpose MN-major ones): forward, dgrad and wgrad epilogues
   PB_CASE(0, 0, EPI_BF16, 1)
   PB_CASE(0, 0, EPI_RESIDUAL, 1)
   PB_CASE(0, 0, EPI_GELU_GRAD, 1)
   PB_CASE(0, 0, EPI_GELU_GRAD_Q8, 1)
   PB_CASE(0, 0, EPI_F32, 1)
-  PB_CASE(0, 1, EPI_BF16, 1)
-  PB_CASE(0, 1, EPI_MUL, 1)
-  PB_CASE(0, 1, EPI_F32, 1)
-  PB_CASE(1, 1, EPI_F32, 1)
-  PB_CASE(1, 1, EPI_BF16, 1)
+  PB_CASE(0, 0, EPI_MUL, 1)
 #undef PB_CASE
   throw std::runtime_error("photon_b200 gemm: unsupported (a_major, b_major, epilogue, operand type) combination");
 }

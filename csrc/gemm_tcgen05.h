@@ -1,4 +1,4 @@
-// Host API of the tcgen05 GEMM family (see gemm_tcgen05.cu).
+// Host API of the wgmma GEMM family (see gemm_tcgen05.cu).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -11,7 +11,7 @@ enum Epilogue : int {
   EPI_RESIDUAL = 1,   // D = bf16(acc*alpha + bias + aux)
   EPI_GELU_DUAL = 2,  // D2 = bf16(z = acc*alpha + bias);  D = bf16(gelu(z))
   EPI_DGELU = 3,      // D = bf16((acc*alpha + bias) * gelu'(aux))
-  EPI_F32 = 4,        // D (fp32) = acc*alpha   or  D += acc*alpha   (accumulate, TMA reduce-add)
+  EPI_F32 = 4,        // D (fp32) = acc*alpha   or  D += acc*alpha   (accumulate, red.global.add)
   EPI_GELU_GRAD = 5,  // z = acc*alpha + bias;  D = bf16(gelu(z));  D2 = bf16(gelu'(z))  — the backward then needs no erf/exp
   EPI_MUL = 6,        // D = bf16((acc*alpha + bias) * aux)
   EPI_GELU_GRAD_Q8 = 7,  // fp8 operands only: z = acc*alpha + bias;  D8 = e4m3(gelu(z) * *out_scale) (+ amax);  D2 = bf16(gelu'(z))
@@ -32,7 +32,7 @@ struct GemmArgs {
   float alpha = 1.0f;
   int num_sms = 0;
   int cluster = 0;   // 0 = auto (2-CTA clusters with B multicast when >= 2 M tiles), 1 or 2 to force
-  // ---- fp8 operands (tcgen05.mma kind::f8f6f4): A and B hold 1-byte elements, lda / ldb count elements (= bytes)
+  // ---- fp8 operands (wgmma e4m3 / e5m2, K-major only): A and B hold 1-byte elements, lda / ldb count elements (= bytes)
   int fp8 = 0;
   int a_fmt = 0, b_fmt = 0;           // 0 = E4M3, 1 = E5M2
   const float* sinv_a = nullptr;      // device scalars: 1 / quantisation scale of A and of B (multiplied into alpha)
@@ -45,8 +45,10 @@ struct GemmArgs {
 
 void gemm_launch(const GemmArgs& g, cudaStream_t stream);
 void gemm_bf16_launch(const GemmArgs& g, cudaStream_t stream);   // same entry (kept for callers that predate fp8)
+// [R, C] bytes (row stride ld) -> [C, R] contiguous: an MN-major fp8 operand made K-major
+void transpose_u8(const void* src, long long ld, void* dst, int R, int C, cudaStream_t stream);
 
-// ---- block-scaled MXFP8 (gemm_mxfp8.cu): E4M3 elements + one E8M0 scale per 32 K-elements of every row, scales applied in the tensor core
+// ---- block-scaled MXFP8 (gemm_mxfp8.cu): E4M3 elements + one E8M0 scale per 32 K-elements of every row, scales applied per 32-K group to the wgmma partial sums
 // x [R,K] bf16 -> q8 [R,K] E4M3, sf [K/128][rblk][512] scale atoms (rblk >= ceil(R/128); rows beyond R must be pre-zeroed)
 void mx_quantize(const void* x_bf16, long long ld, void* q8, void* sf, long long R, int K, int rblk, cudaStream_t st);
 // D[M,N] bf16 = (A.*SFA)[M,K] (B.*SFB)[N,K]^T (+ bias); sfa [K/128][ceil(M/128)][512], sfb [K/128][2*ceil(N/256)][512]

@@ -1,7 +1,7 @@
-// Thin inline-PTX wrappers for the Blackwell (sm_100a) features the kernels in this
-// directory are built on: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM
-// alloc / ld / commit), named barriers, cross-GPU memory-model primitives.
-// Hand-written for photon_b200 — no CUTLASS/CuTe dependency in product code.
+// Thin inline-PTX wrappers for the Hopper (sm_90a) features the kernels in this
+// directory are built on: mbarrier, TMA (cp.async.bulk.tensor), clusters, wgmma
+// descriptors (the MMA wrappers are in wgmma.cuh), named barriers, cross-GPU
+// memory-model primitives. Hand-written — no CUTLASS/CuTe dependency in product code.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -115,43 +115,7 @@ __device__ __forceinline__ void tma_wait_all() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// MMA completion -> mbarrier (implicitly fences before_thread_sync)
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// same, arriving on the barrier at this smem offset in every CTA of `cta_mask` (cluster multicast)
-__device__ __forceinline__ void tc_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-// ---- CTA-pair (cta_group::2) primitives: two SMs cooperate on one 256-row UMMA tile --------------------------
-// In a cluster launch the 32-bit shared address carries the CTA rank in bit 24; clearing it addresses the leader.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-// TMA load issued by EITHER CTA of the pair; the transaction bytes are credited to the LEADER's mbarrier
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
+// ---------------------------------------------------------------- clusters
 // arrive on the barrier at this smem offset in CTA `cta` of the cluster
 __device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
   asm volatile(
@@ -160,30 +124,6 @@ __device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) 
       "mbarrier.arrive.shared::cluster.b64 _, [remAddr32];\n\t}\n" ::"r"(smem_u32(bar)),
       "r"(cta)
       : "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst) {  // same warp id in both CTAs, same dst offset
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "n"(NCOLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[256 x K: 128 rows per CTA] * B[N x K: N/2 rows per CTA]; issued by the leader only
-__device__ __forceinline__ void tc_mma_f16_ss_2sm(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// completion of all prior cta_group::2 MMAs -> arrive on the barrier at this offset in every CTA of `cta_mask`
-__device__ __forceinline__ void tc_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
 }
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
@@ -194,162 +134,29 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// D[tmem] (+)= A[smem desc] * B[smem desc]; bf16/fp16 inputs, fp32 accumulate
-__device__ __forceinline__ void tc_mma_f16_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Same, with the descriptors given by their LOW words only: every SWIZZLE_128B descriptor this code base builds has the
-// same high word (SBO = 1024 B, version 1, layout 2), so the k-step / stage arithmetic is 32-bit and the issue sequence
-// around each UTCHMMA stays short.
-constexpr uint32_t kDescHiSw128 = (1024u >> 4) | (1u << 14) | (2u << 29);
-__device__ __forceinline__ uint32_t smem_desc_lo(uint32_t smem_addr, uint32_t lbo_bytes) {
-  return ((smem_addr & 0x3FFFFu) >> 4) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
-}
-__device__ __forceinline__ void tc_mma_f16_ss_lo(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(kDescHiSw128)
-      : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16_ss_2sm_lo(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(kDescHiSw128)
-      : "memory");
-}
-// fp8 operands (E4M3 / E5M2 picked per operand by the instruction descriptor), fp32 accumulate: 32 K-elements per instruction
-__device__ __forceinline__ void tc_mma_f8_ss_lo(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], da, db, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(kDescHiSw128)
-      : "memory");
-}
-__device__ __forceinline__ void tc_mma_f8_ss_2sm_lo(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], da, db, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(kDescHiSw128)
-      : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16_ts_lo(uint32_t d_tmem, uint32_t a_tmem, uint32_t b_lo, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 db;\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], db, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(kDescHiSw128)
-      : "memory");
-}
-// A operand from TMEM (e.g. softmax probabilities), B from smem
-__device__ __forceinline__ void tc_mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+// register budget of a warpgroup (producer warpgroups give registers to the MMA warpgroups)
+template <int R>
+__device__ __forceinline__ void regs_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void regs_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives lane (base_lane+i)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-// 32 lanes x 16 columns of 32-bit: thread i of the warp receives lane (base+i), columns [c, c+16)
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-
-// ---------------------------------------------------------------- UMMA descriptors
-// Shared-memory matrix descriptor (sm_100 "version 1"), 128-byte swizzle.
-//   K-major  tile [rows][64 bf16]: 8-row groups are 1024 B apart -> SBO = 1024, LBO unused.
-//   MN-major tile [k rows][64 bf16 of MN]: 8-k groups 1024 B apart (SBO), next 64-wide MN
-//   chunk `lbo_bytes` further (LBO).
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// ---------------------------------------------------------------- wgmma shared-memory descriptors (sm_90)
+// 128-byte swizzle (layout type 1 in bits [62,64)), tiles written by TMA with CU_TENSOR_MAP_SWIZZLE_128B and 1024-byte aligned.
+//   K-major  tile [rows][128 B of K]: 8-row groups 1024 B apart (SBO); LBO unused. A k-step adds its byte offset inside the
+//            128-byte row to the start address.
+//   MN-major tile [k rows][128 B of MN]: 8-k-row groups 1024 B apart (SBO), the next 128-byte-wide MN chunk `lbo_bytes`
+//            further (LBO); a k-step of 16 rows adds 2048 B.
+__device__ __forceinline__ uint64_t desc_sw128(const void* smem_ptr, uint32_t lbo_bytes) {
+  const uint32_t a = smem_u32(smem_ptr);
   uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);            // [0,14)  start address >> 4
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;       // [16,30) leading byte offset >> 4
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;       // [32,46) stride byte offset >> 4
-  d |= static_cast<uint64_t>(1) << 46;                               // [46,48) descriptor version = 1 (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;                               // [61,64) layout = SWIZZLE_128B
+  d |= static_cast<uint64_t>((a & 0x3FFFF) >> 4);               // [0,14)  start address >> 4
+  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;  // [16,30) leading byte offset >> 4
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;                  // [32,46) stride byte offset >> 4
+  d |= static_cast<uint64_t>(1) << 62;                          // [62,64) SWIZZLE_128B
   return d;
 }
-// Instruction descriptor for kind::f16 (A/B bf16, D fp32). major: 0 = K-major, 1 = MN-major.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4)                      // D format  = F32
-         | (1u << 7)                    // A format  = BF16
-         | (1u << 10)                   // B format  = BF16
-         | (uint32_t(a_mn_major) << 15) // A major
-         | (uint32_t(b_mn_major) << 16) // B major
-         | (uint32_t(N >> 3) << 17)     // N / 8
-         | (uint32_t(M >> 4) << 24);    // M / 16
-}
-
-// Instruction descriptor for kind::f8f6f4 (A/B 8-bit floats, D fp32). fmt: 0 = E4M3, 1 = E5M2. MN-major operands are legal for
-// the 8-bit formats (not for the 4/6-bit ones).
-__host__ __device__ constexpr uint32_t make_idesc_f8(int M, int N, int a_mn_major, int b_mn_major, int a_fmt, int b_fmt) {
-  return (1u << 4)                      // D format  = F32
-         | (uint32_t(a_fmt) << 7)       // A format
-         | (uint32_t(b_fmt) << 10)      // B format
-         | (uint32_t(a_mn_major) << 15) // A major
-         | (uint32_t(b_mn_major) << 16) // B major
-         | (uint32_t(N >> 3) << 17)     // N / 8
-         | (uint32_t(M >> 4) << 24);    // M / 16
-}
+// byte offset added to a descriptor's start-address field
+__device__ __forceinline__ uint64_t desc_add(uint64_t d, uint32_t bytes) { return d + (bytes >> 4); }
 
 // ---------------------------------------------------------------- fp8 packing (saturating, round-to-nearest-even)
 __device__ __forceinline__ uint32_t pack_e4m3x4(float a, float b, float c, float d) {
@@ -364,28 +171,10 @@ __device__ __forceinline__ uint32_t pack_e5m2x4(float a, float b, float c, float
   asm("cvt.rn.satfinite.e5m2x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(d), "f"(c));
   return uint32_t(lo) | (uint32_t(hi) << 16);
 }
-// Packed fp32 pairs (sm_100: FFMA2 / FADD2 issue once for two lanes of work — the FMA pipe does the same flops, the scheduler spends
-// half the issue slots; the operands are 64-bit register pairs)
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  unsigned long long ra, rb, rc, rd;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rc) : "f"(c.x), "f"(c.y));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-  float2 d;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-  return d;
+// two consecutive fp32 (8-byte aligned) added in global memory by one vector reduction
+__device__ __forceinline__ void red_add_f32x2(float* p, float a, float b) {
+  asm volatile("red.relaxed.gpu.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-  unsigned long long ra, rb, rd;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-  float2 d;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-  return d;
-}
-
 __device__ __forceinline__ float warp_max_f(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffff, v, o));

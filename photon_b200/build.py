@@ -1,9 +1,9 @@
-"""In-tree build of the sm_100a extension ``photon_b200/_C*.so``.
+"""In-tree build of the sm_90a extension ``photon_b200/_C*.so``.
 
 Plain ``nvcc`` / ``g++`` invocations (parallel, mtime-incremental) so that the
-exact arch flags are under our control: ``-gencode arch=compute_100a,code=sm_100a
--lineinfo`` (tcgen05/TMA need the arch-specific ``a`` target).  The product is
-kept in-tree so the GPU box sees it and the driver can record it as loaded.
+exact arch flags are under our control: ``-gencode arch=compute_90a,code=sm_90a
+-lineinfo`` (wgmma / setmaxnreg need the arch-specific ``a`` target).  The product
+is kept in-tree so the package imports straight from a checkout.
 """
 from __future__ import annotations
 
@@ -21,7 +21,7 @@ EXT_NAME = "_C"
 
 CU_SOURCES = ["gemm_tcgen05.cu", "gemm_mxfp8.cu", "attention_tcgen05.cu", "fused_ops.cu", "fp8_ops.cu", "comm.cu"]
 CPP_SOURCES = ["bindings.cpp"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "--use_fast_math", "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 
 
@@ -66,7 +66,7 @@ def build(force: bool = False, verbose: bool = True) -> Path:
         if force or _newer(src, dst, headers):
             jobs.append((["g++", "-O2", "-std=c++17", "-fPIC", "-w", *defs, *incs, "-c", str(src), "-o", str(dst)], None))
     if verbose and jobs:
-        print(f"[photon_b200.build] compiling {len(jobs)} translation unit(s) for sm_100a ...", flush=True)
+        print(f"[photon_b200.build] compiling {len(jobs)} translation unit(s) for sm_90a ...", flush=True)
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 2)) as ex:
         list(ex.map(lambda j: _run(*j), jobs))
     out = ext_path()

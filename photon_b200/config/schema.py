@@ -1,9 +1,9 @@
 """Typed schema for the resolved config tree.
 
 Same key surface as the reference's ``BaseConfig`` (ref:
-photon/conf/base_schema.py:11-392) plus two B200-native additions:
+photon/conf/base_schema.py:11-392) plus two H100-native additions:
 ``photon.comm_stack.nvl`` (fused NVLink kernels for the round hot paths) and
-the optional ``kernels`` section (which hand-written sm_100a ops are on).
+the optional ``kernels`` section (which hand-written sm_90a ops are on).
 Validation is strict on the federation/photon nodes and permissive on
 ``llm_config`` / ``dataset`` (free-form in the reference too, ref:
 base_schema.py:336-342).
@@ -26,7 +26,7 @@ class CommStack(_Strict):
     s3: bool = False
     shm: bool = True
     ray: bool = False
-    nvl: bool = False  # B200-native: in-kernel NVLink P2P / multicast path
+    nvl: bool = False  # H100-native: in-kernel NVLink P2P / multicast path
 
     @model_validator(mode="after")
     def _one_hot(self) -> "CommStack":
@@ -158,7 +158,7 @@ class FL(_Strict):
     aggregate_momenta: bool = False
     use_noise_scale_metric: bool = False
     noise_scale_beta: float = 0.99
-    # B200-native additions (absent keys default to reference behaviour)
+    # H100-native additions (absent keys default to reference behaviour)
     reference_sign_compat: bool = False  # FedAdam/FedYogi ascent quirk, SURVEY §2.4
     fault_injection: dict[str, Any] | None = None  # {"round": r, "cid": k, "kind": "drop"}
 
@@ -232,11 +232,11 @@ class Wandb(_Strict):
 
 
 class Kernels(_Strict):
-    """Which hand-written sm_100a kernels the engine uses (B200-native knob).
+    """Which hand-written sm_90a kernels the engine uses (H100-native knob).
     ``auto`` = on when a CUDA device is present, plain PyTorch on CPU."""
 
-    gemm: str = "auto"        # tcgen05/TMEM/TMA GEMM family
-    attention: str = "auto"   # tcgen05 flash attention
+    gemm: str = "auto"        # wgmma/TMA GEMM family
+    attention: str = "auto"   # wgmma flash attention
     norm: str = "auto"        # fused residual+LayerNorm
     loss: str = "auto"        # fused cross-entropy
     optimizer: str = "auto"   # fused flat-buffer ADOPT / DecoupledAdamW

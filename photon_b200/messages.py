@@ -2,7 +2,7 @@
 
 The reference moves these as Flower ``RecordSet``s over gRPC with every
 non-scalar field stringified (ref: photon/server/server_util.py:205-302,
-photon/client_app.py:182-211; SURVEY Appendix A).  The B200 engine keeps the
+photon/client_app.py:182-211; SURVEY Appendix A).  The H100 engine keeps the
 same *schema* (so logs, semantics and tests line up) but as plain dataclasses
 passed through in-process / torch.distributed object channels — there is no
 serialisation of tensors on either hot path: ``parameters`` is a handle (flat

@@ -1,15 +1,15 @@
-"""B200Engine — the MPT training step on hand-written sm_100a kernels.
+"""B200Engine (name kept for compatibility) — the MPT training step on hand-written sm_90a kernels.
 
 No autograd, no per-op dispatcher: forward and backward are an explicit
 schedule of our own kernels over preallocated bf16 activations, flat fp32
 master parameters/gradients and a flat bf16 compute shadow
 (SURVEY §2.5 (a) K1–K15 → one engine):
 
-* every linear layer = ``csrc/gemm_tcgen05.cu`` (TMA → tcgen05.mma → TMEM →
-  fused epilogue): bias, bias+residual, bias+GELU (pre-activation and
+* every linear layer = ``csrc/gemm_tcgen05.cu`` (TMA → wgmma → register
+  accumulators → fused epilogue): bias, bias+residual, bias+GELU (pre-activation and
   activation written by the same epilogue), dgrad with the stored weight
   consumed MN-major (no transposes), dGELU fused into the dgrad epilogue, wgrad
-  with both operands MN-major accumulating in fp32 by TMA reduce-add straight
+  with both operands MN-major accumulating in fp32 by red.global.add straight
   into the flat gradient bucket that the DDP all-reduce / optimizer consume;
 * LM head + cross-entropy chunked over tokens so the ``[T, 50368]`` logits are
   never materialised (``[chunk, V]`` scratch that stays L2/HBM friendly);
@@ -52,7 +52,7 @@ class B200Engine:
     def __init__(self, cfg: MPTConfig, device: torch.device | str = "cuda", precision: str = "amp_bf16",
                  kernels: dict[str, Any] | None = None, seed: int | None = 17, frozen_layers: list[str] | None = None,
                  unfrozen_layers: list[str] | None = None, unigram_log_probs: torch.Tensor | None = None,
-                 lm_head_chunk: int = 18944, grads_storage: torch.Tensor | None = None,
+                 lm_head_chunk: int = 16896, grads_storage: torch.Tensor | None = None,
                  activation_checkpointing: bool = False, params_storage: torch.Tensor | None = None,
                  shadow_storage: torch.Tensor | None = None, zero3: Any = None) -> None:
         """``zero3``: a :class:`photon_b200.parallel.zero3.NvlZero3Comm` — full parameter sharding: this rank keeps 1/world of the
@@ -61,7 +61,7 @@ class B200Engine:
         self.cfg = cfg
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError("B200Engine needs a CUDA (sm_100a) device")
+            raise RuntimeError("B200Engine needs a CUDA (sm_90a) device")
         if precision not in ("amp_bf16", "amp_fp8"):
             raise NotImplementedError(f"B200Engine computes in bf16 (got precision={precision}); use kernels.*=torch for fp32/fp16")
         if frozen_layers or unfrozen_layers:
@@ -73,7 +73,7 @@ class B200Engine:
             raise NotImplementedError("full parameter sharding runs in amp_bf16 (the fp8 weight copies are quantised from a resident bf16 plane)")
         kernels = dict(kernels or {})
         # amp_fp8 (ref: scripts/centralised_training.sh:91, Composer amp_fp8 -> TransformerEngine): the four GEMMs of every block
-        # and their dgrad / wgrad run on tcgen05.mma kind::f8f6f4 (E4M3 activations / weights, E5M2 gradients, per-tensor
+        # and their dgrad / wgrad run on fp8 wgmma (E4M3 activations / weights, E5M2 gradients, per-tensor
         # scaling, fp32 accumulation); LayerNorm, attention, residuals, LM head, loss and optimizer stay bf16 / fp32
         self.fp8 = precision == "amp_fp8"
         self.attn_mode = "torch" if kernels.get("attention", "auto") == "torch" else "b200"
@@ -83,9 +83,9 @@ class B200Engine:
         self.use_graph = bool(kernels.get("cuda_graph", True)) and zero3 is None
         self._graphs: dict[tuple, Any] = {}
         if self.attn_mode == "b200" and cfg.d_head not in (64, 128):
-            # the tcgen05 attention kernels cover d_head 64 and 128 (every shipped MPT config); anything else uses the
+            # the wgmma attention kernels cover d_head 64 and 128 (every shipped MPT config); anything else uses the
             # library attention for BOTH directions (explicit + logged; GEMM/LN/CE/optimizer stay on our kernels)
-            print(f"[engine] d_head={cfg.d_head}: attention falls back to SDPA (tcgen05 kernels cover d_head 64 / 128)", flush=True)
+            print(f"[engine] d_head={cfg.d_head}: attention falls back to SDPA (wgmma kernels cover d_head 64 / 128)", flush=True)
             self.attn_mode = "torch"
         self.model = MPTForCausalLM(cfg, device=self.device, seed=seed)
         self.frozen = apply_freeze(self.model, frozen_layers, unfrozen_layers)

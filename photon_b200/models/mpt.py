@@ -5,7 +5,7 @@ and math follow what the reference trains through llm-foundry
 (ref: photon/conf/llm_config/mpt-125m.yaml:18-28; names relied on at
 photon/utils.py:572,591,602-637; SURVEY Appendix C). The B200 hot path lives in
 :mod:`photon_b200.models.engine`, which runs the same parameters through
-hand-written sm_100a kernels and is tested against this module.
+hand-written sm_90a kernels and is tested against this module.
 
 Block: ``x = x + attn(norm_1(x)); x = x + ffn(norm_2(x))``; ``ffn =
 down(gelu_exact(up(x)))``; LM head tied to ``wte``; loss = CE over

@@ -12,7 +12,7 @@
   (the reference retries forever, SURVEY §5.3);
 * ``refresh_workers`` recycles the pool every ``photon.refresh_period`` rounds.
 
-This is the host (shm) topology kept for parity and CPU runs; on a B200 box the SPMD
+This is the host (shm) topology kept for parity and CPU runs; on a H100 box the SPMD
 :class:`photon_b200.federation.FederationRuntime` is the primary path.
 """
 from __future__ import annotations

@@ -1,9 +1,8 @@
-"""Python face of the hand-written sm_100a kernels (``photon_b200._C``).
+"""Python face of the hand-written sm_90a kernels (``photon_b200._C``).
 
 Every function here launches OUR kernels; nothing silently falls back to a
 PyTorch op.  If the extension is missing on a machine that has a CUDA device
-the import error is raised loudly (the driver records which ``.so`` files the
-GPU tests actually loaded).  On CPU-only machines the extension still imports
+the import error is raised loudly.  On CPU-only machines the extension still imports
 (it is cross-compiled) but these wrappers are never called.
 """
 from __future__ import annotations
@@ -24,7 +23,7 @@ def ext() -> Any:
             from photon_b200 import _C  # type: ignore[attr-defined]
         except ImportError as e:  # pragma: no cover - depends on the box
             raise ImportError(
-                "photon_b200._C (sm_100a kernels) is not built. Run `python -m photon_b200.build` "
+                "photon_b200._C (sm_90a kernels) is not built. Run `python -m photon_b200.build` "
                 "(or __graft_entry__.build()) — refusing to fall back to PyTorch ops on the GPU path.") from e
         _EXT = _C
     return _EXT
@@ -53,14 +52,14 @@ def add_launch_count(n: int) -> None:
 
 # --------------------------------------------------------------------------------- GEMM
 EPI_BF16, EPI_RESIDUAL, EPI_GELU_DUAL, EPI_DGELU, EPI_F32, EPI_GELU_GRAD, EPI_MUL, EPI_GELU_GRAD_Q8 = 0, 1, 2, 3, 4, 5, 6, 7
-E4M3, E5M2 = 0, 1          # operand formats of the kind::f8f6f4 GEMMs
+E4M3, E5M2 = 0, 1          # operand formats of the fp8 wgmma GEMMs
 FP8_MAX = (448.0, 57344.0)
 
 
 def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False,
          epi: int = EPI_BF16, bias: torch.Tensor | None = None, aux: torch.Tensor | None = None,
          out2: torch.Tensor | None = None, accumulate: bool = False, alpha: float = 1.0, cluster: int = 0) -> torch.Tensor:
-    """``out[M,N] = epilogue(alpha * A @ B^T)`` on tcgen05 tensor cores.
+    """``out[M,N] = epilogue(alpha * A @ B^T)`` on wgmma tensor cores.
 
     ``a``: ``[M,K]`` (K-major) or ``[K,M]`` when ``a_mn``; ``b``: ``[N,K]`` or ``[K,N]`` when ``b_mn``."""
     ext().gemm(a, b, out, int(a_mn), int(b_mn), int(epi), bias, aux, out2, bool(accumulate), float(alpha), int(cluster))
@@ -107,7 +106,7 @@ def gemm_fp8(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, meta: torch.Te
              accumulate: bool = False, alpha: float = 1.0, cluster: int = 0, out8: torch.Tensor | None = None,
              role_out: int = -1) -> torch.Tensor:
     """``out = epilogue(alpha / (scale[role_a] * scale[role_b]) * A8 @ B8^T)`` — 1-byte operands (E4M3 / E5M2 per operand) on
-    ``tcgen05.mma kind::f8f6f4``, fp32 accumulation. ``meta`` = float32 ``[3, n_roles]`` (scale, 1/scale, amax) on the device;
+    fp8 ``wgmma`` (MN-major operands are transposed to K-major first), fp32 accumulation. ``meta`` = float32 ``[3, n_roles]`` (scale, 1/scale, amax) on the device;
     the de-scales are read by the kernel, so nothing here touches the host. ``EPI_GELU_GRAD_Q8`` writes ``out8`` (E4M3,
     scaled by ``scale[role_out]``, amax recorded) and ``out2`` = gelu'; ``out`` is then unused (pass ``out2``)."""
     ext().gemm_fp8(a, b, out, int(a_mn), int(b_mn), int(epi), int(a_fmt), int(b_fmt), meta, int(role_a), int(role_b), bias, aux, out2,
@@ -117,15 +116,15 @@ def gemm_fp8(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, meta: torch.Te
 
 def mx_quantize(x: torch.Tensor, row_blocks: int = 0) -> tuple[torch.Tensor, torch.Tensor]:
     """bf16 ``[R,K]`` → (E4M3 ``[R,K]`` uint8, E8M0 scale atoms ``[K/128, row_blocks, 512]`` uint8): OCP MXFP8, one power-of-two scale
-    per 32 consecutive K elements of a row, stored in the layout ``tcgen05.mma ... block_scale`` reads from TMEM."""
+    per 32 consecutive K elements of a row, stored as 512-byte atoms per 128 rows x 128 K that the GEMM loads with one bulk copy."""
     q, sf = ext().mx_quantize(x, int(row_blocks))
     return q, sf
 
 
 def gemm_mxfp8(a8: torch.Tensor, b8: torch.Tensor, out: torch.Tensor, sfa: torch.Tensor, sfb: torch.Tensor,
                bias: torch.Tensor | None = None) -> torch.Tensor:
-    """``out[M,N] = (A ⊙ SFA) @ (B ⊙ SFB)^T (+ bias)`` with the block scales applied inside the tensor core
-    (``tcgen05.mma kind::mxf8f6f4.block_scale``). ``sfb`` needs ``2·ceil(N/256)`` row blocks (``mx_quantize(w, 2 * ceil(N/256))``)."""
+    """``out[M,N] = (A ⊙ SFA) @ (B ⊙ SFB)^T (+ bias)`` with the block scales applied to the fp32 wgmma partial sum
+    of every 32-element K group. ``sfb`` needs ``2·ceil(N/256)`` row blocks (``mx_quantize(w, 2 * ceil(N/256))``)."""
     ext().gemm_mxfp8(a8, b8, out, sfa, sfb, bias)
     return out
 

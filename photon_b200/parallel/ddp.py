@@ -156,8 +156,9 @@ def wants_sharded_step(llm_cfg: Any) -> bool:
 def wants_full_sharding(cfg: Any, n_params: int, device: Any = None) -> bool:
     """``kernels.param_sharding``: ``zero3`` / ``zero1`` force a scheme; ``auto`` (default) shards parameters and gradients too
     (ZeRO-3, :mod:`photon_b200.parallel.zero3`) when ``fsdp_config.sharding_strategy`` is FULL_SHARD AND the replicated training
-    state (18 B/param) would take more than 40 % of the GPU — MPT-7B on 180 GB, not MPT-125M..3B, for which the fused ZeRO-1 step
-    (one kernel, CUDA-graphed microbatches) is faster and memory is not a concern."""
+    state (18 B/param) would take more than 40 % of the GPU — on an 80 GB H100 that is MPT-3B and MPT-7B, not MPT-125M / 1B, for
+    which the fused ZeRO-1 step (one kernel, CUDA-graphed microbatches) is faster and memory is not a concern. Without a CUDA
+    device the capacity of an 80 GB H100 is assumed."""
     llm = cfg["llm_config"]
     mode = str((cfg.get("kernels") or {}).get("param_sharding", "auto") or "auto").lower()
     if mode in ("zero3", "full", "full_shard"):
@@ -165,7 +166,7 @@ def wants_full_sharding(cfg: Any, n_params: int, device: Any = None) -> bool:
     fsdp = (llm or {}).get("fsdp_config") or None
     if mode != "auto" or not fsdp or str(dict(fsdp).get("sharding_strategy", "FULL_SHARD")).upper() != "FULL_SHARD":
         return False
-    cap = 180 * 2**30
+    cap = 80 * 2**30
     try:
         import torch as _t
 

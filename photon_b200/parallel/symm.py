@@ -120,8 +120,9 @@ class SymmArena:
 
     def mc_ptr(self, name: str) -> int:
         """Multicast address of a plane, or 0 = use the P2P loops: no NVLS mapping, or fewer than ``PB_NVLS_MIN_WORLD``
-        (default 4) GPUs — with 2 GPUs one peer read per element beats the switch round trip (0.96 vs 1.9 ms for the
-        125M-parameter round), from 4 GPUs on the N-fold P2P traffic loses."""
+        (default 4) GPUs: with 2 GPUs the P2P loops move one peer read per element, from 4 GPUs on their traffic grows N-fold
+        while the in-switch reduction's stays constant. Where the two cross over on a given system is not measured here; the
+        variable moves the threshold."""
         if not self.mc_base or self.world_size < int(os.environ.get("PB_NVLS_MIN_WORLD", "4")):
             return 0
         return self.mc_base + self.offsets[name][0]

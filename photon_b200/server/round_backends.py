@@ -2,7 +2,7 @@
 model reaches the clients — the four ``photon.comm_stack`` options.
 
 =========  ================================================================================
-``nvl``    PRODUCT PATH. One fused sm_100a kernel per GPU over the symmetric NVLink arena
+``nvl``    PRODUCT PATH. One fused sm_90a kernel per GPU over the symmetric NVLink arena
            (:class:`photon_b200.parallel.fed_round.NvlFedRound`): weighted reduce + server
            optimizer on the GPU's shard + broadcast with bf16 cast. No NCCL, no host.
 ``ray``    Collective baseline: weighted local sums → ``torch.distributed.all_reduce`` (NCCL on

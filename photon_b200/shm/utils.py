@@ -4,7 +4,7 @@ Role of ref photon/shm/utils.py (:138-651): model parameters travel between the
 node manager, its workers and the server as ONE flat segment described by
 ``ModelParametersMetadata`` (per-tensor byte bounds, shapes, dtypes); scalars
 (n_samples int64, eval loss float64) and pickled dicts (configs, metrics) get
-their own tiny segments.  On the B200 path this is the *fallback / baseline*
+their own tiny segments.  On the H100 path this is the *fallback / baseline*
 transport (``photon.comm_stack.shm``) — the product path is the NVLink arena —
 but it is also what the CPU plumbing tests and the multi-process node manager use.
 

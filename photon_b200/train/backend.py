@@ -6,7 +6,7 @@ attention, ATen LN/GELU/CE under ``torch.autocast`` — what the reference gets
 from Composer + llm-foundry, ref: photon/clients/trainer_utils.py:1615-1719).
 
 ``photon_b200.models.engine.B200Engine`` implements the same protocol with the
-hand-written sm_100a kernels and an explicit (autograd-free) backward; the
+hand-written sm_90a kernels and an explicit (autograd-free) backward; the
 Trainer does not care which one it drives.
 
 Protocol
@@ -144,14 +144,14 @@ class TorchBackend:
 
 def build_backend(model_cfg: MPTConfig, device: torch.device, precision: str, kernels: dict[str, Any] | None = None,
                   **kw: Any) -> Any:
-    """Pick the compute backend. On a CUDA device the B200 engine is THE path (and fails
+    """Pick the compute backend. On a CUDA device the sm_90a engine (``B200Engine``) is THE path (and fails
     loudly if its extension is missing); ``kernels.gemm: torch`` etc. selects the stock
     PyTorch baseline explicitly; CPU always uses stock PyTorch."""
     kernels = dict(kernels or {})
     modes = [kernels.get(k, "auto") for k in ("gemm", "attention", "norm", "loss", "optimizer")]
     want_engine = device.type == "cuda" and not all(m == "torch" for m in modes)
     if any(m == "b200" for m in modes) and device.type != "cuda":
-        raise RuntimeError("kernels.*=b200 requires a CUDA (sm_100a) device")
+        raise RuntimeError("kernels.*=b200 requires a CUDA (sm_90a) device")
     if want_engine:
         unsupported = []
         if precision not in ("amp_bf16", "amp_fp8"):
@@ -159,7 +159,7 @@ def build_backend(model_cfg: MPTConfig, device: torch.device, precision: str, ke
         if kw.get("frozen_layers") or kw.get("unfrozen_layers"):
             unsupported.append("frozen/unfrozen layers")
         if unsupported:
-            print(f"[backend] {', '.join(unsupported)} not covered by the sm_100a engine -> stock PyTorch backend "
+            print(f"[backend] {', '.join(unsupported)} not covered by the sm_90a engine -> stock PyTorch backend "
                   "(explicit, logged; set kernels.*=torch to silence)", flush=True)
             kw.pop("zero3", None)
             return TorchBackend(model_cfg, device=device, precision=precision, **kw)
@@ -167,5 +167,5 @@ def build_backend(model_cfg: MPTConfig, device: torch.device, precision: str, ke
 
         return B200Engine(model_cfg, device=device, precision=precision, kernels=kernels, **kw)
     if kw.pop("zero3", None) is not None:
-        raise RuntimeError("full parameter sharding (NvlZero3Comm) needs the sm_100a engine on a CUDA device")
+        raise RuntimeError("full parameter sharding (NvlZero3Comm) needs the sm_90a engine on a CUDA device")
     return TorchBackend(model_cfg, device=device, precision=precision, **kw)

@@ -6,12 +6,12 @@ ref: scripts/centralised_training.sh:91). The recipe is TE's "delayed scaling":
 * forward GEMM operands (activations, weights) are cast to **E4M3**, gradients flowing backward to **E5M2**;
 * every tensor role of every linear layer keeps an **amax history**; the scale used at step *t* comes from the history up to
   *t−1* (``scale = fp8_max / (amax · 2^margin)``), so no extra pass over the tensor is needed before the cast;
-* products are exact, accumulation is fp32 (what ``tcgen05.mma kind::f8f6f4`` does), the result is de-scaled by
+* products are exact, accumulation is fp32 (what fp8 ``wgmma`` does), the result is de-scaled by
   ``1 / (scale_a · scale_b)`` in the epilogue; LayerNorm, softmax, residuals, the LM head and the optimizer stay in
   bf16 / fp32.
 
 This module implements exactly that as a quantise → de-quantise emulation around ``F.linear`` (runs anywhere, CPU included),
-which makes ``amp_fp8`` a real reduced-precision mode of the stock-PyTorch backend and is the oracle a tcgen05 fp8 GEMM
+which makes ``amp_fp8`` a real reduced-precision mode of the stock-PyTorch backend and is the oracle a wgmma fp8 GEMM
 epilogue has to match. The hand-written engine still computes ``amp_fp8`` runs in bf16 (it says so when it starts).
 """
 from __future__ import annotations

@@ -15,7 +15,8 @@ mpt-125m.yaml:85-91; SURVEY §2.5 (b) N2).  Every rank of the client keeps the t
 moment planes for its contiguous slice of the flat index space only (8 of the 16
 optimizer bytes/param divided by the group size), steps that slice, and the
 updated fp32 master + bf16 compute copy are all-gathered slice by slice over
-NCCL/NVLink.  Parameters themselves stay replicated: ≤7B fits a 180 GB B200.
+NCCL/NVLink.  Parameters themselves stay replicated (models whose replicated state does not fit use
+full parameter sharding instead, :func:`photon_b200.parallel.ddp.wants_full_sharding`).
 """
 from __future__ import annotations
 

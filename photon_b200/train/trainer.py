@@ -17,7 +17,7 @@ photon/centralised_train.py:151-153).  Semantics kept:
 * checkpoints ``ep{E}-ba{B}-rank{R}.pt`` + ``latest-rank{R}.pt`` with
   ``save_num_checkpoints_to_keep`` and glob ``load_ignore_keys``.
 
-B200-first differences: one flat fp32 parameter/gradient/moment buffer, H2D
+H100-first differences: one flat fp32 parameter/gradient/moment buffer, H2D
 copies on a side stream from pinned memory, device-side loss/clip scalars (no
 per-step host sync besides the configurable metric read-back).
 """
@@ -485,7 +485,7 @@ class Trainer:
 
     def _fp8_state(self) -> dict[str, Any] | None:
         """amax histories / scales of an ``amp_fp8`` run (the delayed-scaling recipe resumes with the scales it stopped with)."""
-        if hasattr(self.state.backend, "fp8_state_dict"):      # the sm_100a engine keeps its scales on the device
+        if hasattr(self.state.backend, "fp8_state_dict"):      # the sm_90a engine keeps its scales on the device
             return self.state.backend.fp8_state_dict()
         if not getattr(self.state.backend, "fp8_layers", None):
             return None

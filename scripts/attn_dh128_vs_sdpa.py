@@ -1,4 +1,4 @@
-"""d_head = 128 attention (MPT-1B geometry): our tcgen05 forward / backward vs torch SDPA (library) on the same tensors."""
+"""d_head = 128 attention (MPT-1B geometry): our wgmma forward / backward vs torch SDPA (library) on the same tensors."""
 import math
 import sys
 

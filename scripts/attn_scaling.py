@@ -1,7 +1,7 @@
-"""Fit attention-forward time = CTAs/148 * (F + n_kv * t): fixed per-CTA cost F vs per-KV-tile cost t.
+"""Fit attention-forward time = CTAs/SMs * (F + n_kv * t): fixed per-CTA cost F vs per-KV-tile cost t.
 
 Non-causal runs with the same number of CTAs (b*H*S/128 fixed) but different n_kv = S/128 separate the two.
-Run on the GPU box:  python scripts/attn_scaling.py
+Run on a GPU:  python scripts/attn_scaling.py
 """
 import json
 import sys
@@ -28,6 +28,8 @@ def timed(fn, iters=10):
 
 
 def main():
+    global SMS
+    SMS = torch.cuda.get_device_properties(0).multi_processor_count
     H, dh = 12, 64
     rows = []
     for causal in (False, True):
@@ -39,7 +41,7 @@ def main():
             ms = timed(lambda: ops.attention_fwd(qkv, out, lse, H, dh ** -0.5, causal))
             ctas = b * H * S // 128
             n_kv = (S // 128 + 1) / 2 if causal else S // 128
-            us_per_cta = ms * 1e3 * 148 / ctas
+            us_per_cta = ms * 1e3 * SMS / ctas
             rows.append(dict(causal=causal, S=S, b=b, ms=ms, ctas=ctas, avg_kv_tiles=n_kv, us_per_cta=us_per_cta))
             print(rows[-1], flush=True)
     # backward: same fit (one CTA per (b, h, kv tile) walking the query tiles)
@@ -57,7 +59,7 @@ def main():
             ms = timed(lambda: ops.attention_bwd(qkv, out, dout, lse, dqkv, delta, H, dh ** -0.5, causal))
             ctas = b * H * S // 128
             n_q = (S // 128 + 1) / 2 if causal else S // 128
-            brow.append(dict(bwd=True, causal=causal, S=S, ms=ms, avg_q_tiles=n_q, us_per_cta=ms * 1e3 * 148 / ctas))
+            brow.append(dict(bwd=True, causal=causal, S=S, ms=ms, avg_q_tiles=n_q, us_per_cta=ms * 1e3 * SMS / ctas))
             print(brow[-1], flush=True)
     bn = [r for r in brow if not r["causal"]]
     tb = (bn[-1]["us_per_cta"] - bn[0]["us_per_cta"]) / (bn[-1]["avg_q_tiles"] - bn[0]["avg_q_tiles"])

@@ -1,6 +1,6 @@
-"""Our tcgen05 attention forward / backward vs the library kernels on the same tensors, at both flagship geometries:
+"""Our wgmma attention forward / backward vs the library kernels on the same tensors, at both flagship geometries:
 (b32, H12, S2048, d64) = MPT-125M and (b8, H16, S2048, d128) = MPT-1B. Libraries: torch SDPA restricted to each backend
-(cuDNN, flash) and flash-attn 2.8 (the package the reference calls, here its sm_100 build). CUDA-event timed, L2 flushed."""
+(cuDNN, flash) and flash-attn 2.8 (the package the reference calls, here its build for the installed GPU). CUDA-event timed, L2 flushed."""
 import json
 import math
 import sys

@@ -1,4 +1,4 @@
-"""Kernel microbenchmarks on one B200: our tcgen05 GEMM vs cuBLAS (torch.matmul) on the MPT shapes,
+"""Kernel microbenchmarks on one GPU: our wgmma GEMM vs cuBLAS (torch.matmul) on the MPT shapes,
 bandwidth of the fused memory-bound kernels. CUDA-event timed, L2 flushed between iterations."""
 import json
 import sys
@@ -42,10 +42,10 @@ def main():
               ("qkv fwd", T, 2304, 768, 0, 0), ("out fwd", T, 768, 768, 0, 0), ("up fwd", T, 3072, 768, 0, 0),
               ("down fwd", T, 768, 3072, 0, 0), ("up dgrad", T, 768, 3072, 0, 1), ("up wgrad", 3072, 768, T, 1, 1),
               ("lmhead fwd", 8192, 50368, 768, 0, 0), ("lmhead dgrad", 8192, 768, 50368, 0, 1), ("lmhead wgrad", 50368, 768, 8192, 1, 1),
-              # the shapes the engine ACTUALLY issues for the head: chunks of 18944 rows = 148 M-tiles, so the three N-tiles of the
+              # the shapes the engine ACTUALLY issues for the head: chunks of 16896 rows = 132 M-tiles, so the three N-tiles of the
               # dgrad are exactly three full waves (the 8192-row rows above fill 1.3 waves and pay for the tail)
-              ("lmhead fwd (engine chunk)", 18944, 50368, 768, 0, 0), ("lmhead dgrad (engine chunk)", 18944, 768, 50368, 0, 1),
-              ("lmhead wgrad (engine chunk)", 50368, 768, 18944, 1, 1),
+              ("lmhead fwd (engine chunk)", 16896, 50368, 768, 0, 0), ("lmhead dgrad (engine chunk)", 16896, 768, 50368, 0, 1),
+              ("lmhead wgrad (engine chunk)", 50368, 768, 16896, 1, 1),
               ("square 8192", 8192, 8192, 8192, 0, 0)]
     for name, M, N, K, amn, bmn in shapes:
         a = torch.randn((K, M) if amn else (M, K), device=dev).to(torch.bfloat16)
@@ -61,7 +61,7 @@ def main():
         else:
             cub = timeit(lambda: torch.matmul(A, Bt))
         fl = 2.0 * M * N * K
-        # same shape on kind::f8f6f4 (E4M3 x E4M3 forward, E5M2 x E4M3 backward; operands pre-quantised, de-scale in the epilogue)
+        # same shape on fp8 wgmma (E4M3 x E4M3 forward, E5M2 x E4M3 backward; operands pre-quantised, de-scale in the epilogue)
         a8 = (a.float().clamp(-400, 400)).to(torch.float8_e5m2 if (amn or bmn) else torch.float8_e4m3fn).view(torch.uint8)
         b8 = (b.float().clamp(-400, 400)).to(torch.float8_e4m3fn).view(torch.uint8)
         meta = torch.ones(3, 2, device=dev)

@@ -48,7 +48,7 @@ def run(kernels, batches, steps, precision="amp_bf16", lr=6e-4):
 
 
 def fp8_parity():
-    """amp_fp8 engine (tcgen05 kind::f8f6f4 GEMMs) vs the bf16 engine: 60 steps from the same weights on the same data, at a
+    """amp_fp8 engine (fp8 wgmma GEMMs) vs the bf16 engine: 60 steps from the same weights on the same data, at a
     learning rate high enough for the loss to move (3e-3): the two curves must fall together."""
     steps = 60
     batches = make_batches(steps, 16, 2048, 50368, seed=5)

@@ -1,6 +1,6 @@
 #!/usr/bin/env bash
 # MPT-125M federated example: 8 clients, local batch 32, 128 local steps/round, ADOPT + cosine, FedAvg
-# (ref: scripts/fed_125m_example.sh:36-103). On an 8xB200 box every GPU hosts one client; the round's
+# (ref: scripts/fed_125m_example.sh:36-103). On an 8-GPU box every GPU hosts one client; the round's
 # reduce + server optimizer + broadcast is one fused NVLink kernel (photon.comm_stack.nvl).
 LOCAL_BATCH_SIZE=32; LOCAL_STEPS=128; N_CLIENTS=8
 TOTAL_STEPS=$((5120 * 256 / LOCAL_BATCH_SIZE)); WARMUP_STEPS=$((100 * 256 / LOCAL_BATCH_SIZE)); N_ROUNDS=$((TOTAL_STEPS / LOCAL_STEPS))

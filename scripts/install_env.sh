@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# Build the sm_100a extension in-tree (the only "install" step; no network needed).
+# Build the sm_90a extension in-tree (the only "install" step; no network needed).
 # ref counterpart: scripts/install_env.sh (poetry + flash-attn build) — nothing of that is required here.
 set -euo pipefail
 cd "$(dirname "${BASH_SOURCE[0]}")/.."

@@ -1,9 +1,9 @@
-// Does the packed-bf16 exponential double the exp rate? Issue rates per SM sub-partition on sm_100a of
+// Does the packed-bf16 exponential double the exp rate? Issue rates per SM sub-partition on sm_90a of
 //   mode 0: ex2.approx.ftz.f32                (baseline, 1 exp per lane per instruction)
 //   mode 1: ex2.approx.ftz.bf16x2             (2 exps per lane per instruction — if the MUFU takes it at the same rate)
-//   mode 2: cvt.rn.bf16x2.f32 + ex2.bf16x2    (the softmax sequence: pack two scores, one packed exp -> P pair ready for TMEM)
+//   mode 2: cvt.rn.bf16x2.f32 + ex2.bf16x2    (the softmax sequence: pack two scores, one packed exp -> P pair ready for the MMA)
 //   mode 3: Cody-Waite + degree-3 polynomial exp2 on the FMA pipe (no MUFU)
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 scripts/microbench/ex2_packed.cu -o /tmp/ex2_packed && /tmp/ex2_packed
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 scripts/microbench/ex2_packed.cu -o /tmp/ex2_packed && /tmp/ex2_packed
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>

@@ -1,5 +1,5 @@
-// Issue rates of MUFU.EX2 and F2FP.BF16 (pack) per SM sub-partition on sm_100a.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 scripts/microbench/xu_rate.cu -o /tmp/xu_rate && /tmp/xu_rate
+// Issue rates of MUFU.EX2 and F2FP.BF16 (pack) per SM sub-partition on sm_90a.
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 scripts/microbench/xu_rate.cu -o /tmp/xu_rate && /tmp/xu_rate
 #include <cstdint>
 #include <cstdio>
 #include <cuda_bf16.h>

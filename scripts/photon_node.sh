@@ -8,7 +8,7 @@ set -euo pipefail
 SERVER=${1:?usage: photon_node.sh SERVER_HOST:PORT}
 cd "$(dirname "${BASH_SOURCE[0]}")/.."
 # SPMD=1: the whole box joins as ONE node that runs the SPMD runtime inside (one process per GPU, fused NVLink aggregation of the
-#         box's clients, one pre-aggregated model per round towards the server) — the shape for multi-box federations of B200 boxes
+#         box's clients, one pre-aggregated model per round towards the server) — the shape for multi-box federations of multi-GPU boxes
 if [ -n "${SPMD:-}" ]; then
   N=${N_GPUS:-$(python -c "import torch; print(max(1, torch.cuda.device_count()))")}
   exec python -m photon_b200.launch --nproc "$N" --master-port "${BOX_MASTER_PORT:-29600}" -m photon_b200.node -- --server "$SERVER" --spmd ${FLEET_TLS_CA:+--tls-ca "$FLEET_TLS_CA"}

@@ -7,7 +7,7 @@ import subprocess
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parents[1]
-PAT = re.compile(r"Compiling entry function '(\S+)' for 'sm_100a'.*?\n(?:.*?\n)??\s*(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads\n"
+PAT = re.compile(r"Compiling entry function '(\S+)' for 'sm_90a'.*?\n(?:.*?\n)??\s*(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads\n"
                  r".*?Used (\d+) registers(?:, used (\d+) barriers)?(?:, (\d+) bytes smem)?", re.S)
 
 
@@ -20,7 +20,7 @@ def main() -> None:
                          int(m.group(7) or 0)))
     names = [r[1] for r in rows]
     dem = subprocess.run(["c++filt"], input="\n".join(names), capture_output=True, text=True).stdout.splitlines() if names else []
-    out = ["# ptxas -v summary of the sm_100a build (scripts/ptxas_summary.py): registers/thread, stack frame, spill stores/loads (bytes), static smem",
+    out = ["# ptxas -v summary of the sm_90a build (scripts/ptxas_summary.py): registers/thread, stack frame, spill stores/loads (bytes), static smem",
            "# (dynamic shared memory is requested at launch: see the *Cfg::SMEM constants in csrc/)", ""]
     for (unit, _raw, regs, stack, st, ld, smem), name in zip(rows, dem):
         short = name.replace("pb::(anonymous namespace)::", "").replace("(anonymous namespace)::", "").replace("void ", "")

@@ -9,7 +9,7 @@ os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real CUDA (B200) device")
+    config.addinivalue_line("markers", "gpu: needs a real CUDA (H100) device")
 
 
 def pytest_collection_modifyitems(config, items):

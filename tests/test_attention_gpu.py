@@ -1,4 +1,4 @@
-"""tcgen05 flash attention (fwd + bwd) vs an fp32 PyTorch reference of the same op."""
+"""wgmma flash attention (fwd + bwd) vs an fp32 PyTorch reference of the same op."""
 import math
 
 import pytest

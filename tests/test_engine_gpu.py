@@ -128,7 +128,7 @@ def test_engine_cuda_graph_replay_matches_eager():
 
 
 def test_engine_d_head_128_runs_on_own_attention():
-    """MPT-1B/3B/7B geometry (d_head = 128): forward and backward attention stay on the tcgen05 kernels."""
+    """MPT-1B/3B/7B geometry (d_head = 128): forward and backward attention stay on the wgmma kernels."""
     from photon_b200.models.engine import B200Engine
     from photon_b200.models.mpt import MPTConfig
     from photon_b200.train.backend import TorchBackend
@@ -182,7 +182,7 @@ def test_engine_positional_variants_match_torch(variant):
 
 
 def test_engine_sequence_length_not_multiple_of_128_uses_library_attention():
-    """The tcgen05 attention kernels need S % 128 == 0; any other length runs attention through SDPA inside the same engine
+    """The wgmma attention kernels need S % 128 == 0; any other length runs attention through SDPA inside the same engine
     step (everything else stays on our kernels) and still matches the PyTorch model."""
     from photon_b200.models.engine import B200Engine
     from photon_b200.models.mpt import MPTConfig

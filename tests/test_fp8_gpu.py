@@ -1,4 +1,4 @@
-"""fp8 (tcgen05 kind::f8f6f4) path: GEMMs, quantising producers and the amp_fp8 engine vs PyTorch fp32 references.
+"""fp8 (wgmma e4m3 / e5m2) path: GEMMs, quantising producers and the amp_fp8 engine vs PyTorch fp32 references.
 
 The oracle is the recipe of ``photon_b200/train/fp8.py``: operands are the fp8 values (E4M3 forward, E5M2 gradients) times
 per-tensor scales, products exact, accumulation fp32, de-scale in the epilogue."""
@@ -292,7 +292,7 @@ def _mx_dequant(q, sf, R):
 
 @pytest.mark.parametrize("M,N,K", [(128, 256, 128), (640, 776, 1152), (2048, 2304, 768)])
 def test_gemm_mxfp8_block_scaled(M, N, K):
-    """OCP MXFP8 (one E8M0 scale per 32 K-elements of every row of A and B, applied inside tcgen05.mma ... block_scale):
+    """OCP MXFP8 (one E8M0 scale per 32 K-elements of every row of A and B, applied to the fp32 wgmma partial sum of each K group):
     quantiser and GEMM against the de-quantise-then-multiply oracle; rows of wildly different magnitude keep their precision."""
     from photon_b200 import ops
 

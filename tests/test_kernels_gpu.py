@@ -1,4 +1,4 @@
-"""Numerics of every hand-written sm_100a kernel vs a plain PyTorch fp32 reference of the same op."""
+"""Numerics of every hand-written sm_90a kernel vs a plain PyTorch fp32 reference of the same op."""
 import math
 
 import pytest

@@ -55,6 +55,8 @@ def test_full_sharding_policy():
 
     assert wants_full_sharding(cfg(), 6_650_000_000)                  # MPT-7B: 120 GB of replicated state
     assert not wants_full_sharding(cfg(), 125_000_000)                # MPT-125M keeps the fused ZeRO-1 step
+    assert not wants_full_sharding(cfg(), 1_320_000_000)              # MPT-1B: 22 GB, fits beside its activations on 80 GB
+    assert wants_full_sharding(cfg(), 2_650_000_000)                  # MPT-3B: 44 GB, more than 40 % of an 80 GB H100
     assert not wants_full_sharding(cfg("SHARD_GRAD_OP"), 6_650_000_000)
     assert not wants_full_sharding(cfg(fsdp=False), 6_650_000_000)
     assert wants_full_sharding(cfg(mode="zero3", fsdp=False), 125_000_000)
@@ -149,8 +151,8 @@ def test_sharded_trainer_steps_and_checkpoints_like_the_plain_one(tmp_path):
     def rel(x, y):
         return ((x - y).norm() / y.norm()).item()
 
-    # noise floor (profiles/zero3_noise.txt): two PLAIN runs end 1-3e-5 apart after 3 steps and 1.5-2e-4 after 5 (atomically
-    # accumulated gradients, amplified by Adam); the sharded run sits at 5.5e-5 / 1.8-2.1e-4 from a plain one
+    # noise floor: gradients are accumulated with atomics, so two PLAIN runs already differ in the last bits, and Adam amplifies
+    # that over the steps; the sharded run must stay within that band of a plain one
     assert rel(z3.state.flat.full_params(), plain.state.flat.params) < 2e-4
     la, lb = plain.loggers[0].data["loss/train/total"], z3.loggers[0].data["loss/train/total"]
     assert len(la) == len(lb) and all(abs(x[1] - y[1]) < 1e-3 for x, y in zip(la, lb)), (la, lb)
