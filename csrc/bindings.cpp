@@ -18,6 +18,7 @@
 #include "fused_ops.h"
 #include "gemm_tcgen05.h"
 #include "attention_tcgen05.h"
+#include "decode.h"
 
 namespace py = pybind11;
 using torch::Tensor;
@@ -309,6 +310,139 @@ void rope(Tensor& qkv, const Tensor& cos_t, const Tensor& sin_t, int n_heads, bo
   TORCH_CHECK(cos_t.is_contiguous() && sin_t.is_contiguous() && cos_t.size(0) >= S && cos_t.size(1) == dh / 2, "cos/sin must be [>=S, dh/2]");
   pb::rope_launch(qkv.data_ptr(), cos_t.data_ptr<float>(), sin_t.data_ptr<float>(), (long long)qkv.size(0) * S, S, n_heads, dh, inverse,
                   stream_of(qkv));
+  g_launches += 1;
+}
+
+// ---------------------------------------------------------------------------------- decoding
+inline void check_i32(const Tensor& t, const char* name) {
+  check_cuda(t, name);
+  TORCH_CHECK(t.scalar_type() == at::kInt && t.is_contiguous(), name, " must be contiguous int32");
+}
+inline void check_aligned16(const Tensor& t, const char* name) {
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(t.data_ptr()) & 15) == 0 && (t.dim() < 2 || t.stride(0) % 8 == 0), name,
+              " must be 16-byte aligned with a row stride that is a multiple of 8 elements");
+}
+// y[M,N] = epilogue(x[M,K] w[N,K]^T), 1 <= M <= 64
+void skinny_gemm(const Tensor& x, const Tensor& w, Tensor& y, const c10::optional<Tensor>& bias, const c10::optional<Tensor>& residual,
+                 int epi) {
+  check_bf16(x, "x");
+  check_bf16(w, "w");
+  check_bf16(y, "y");
+  TORCH_CHECK(x.dim() == 2 && w.dim() == 2 && y.dim() == 2, "skinny_gemm operands must be 2-D");
+  TORCH_CHECK(x.stride(1) == 1 && w.stride(1) == 1 && y.stride(1) == 1, "skinny_gemm operands must have unit inner stride");
+  TORCH_CHECK(x.size(1) == w.size(1), "skinny_gemm: K mismatch between x and w");
+  TORCH_CHECK(y.size(0) == x.size(0) && y.size(1) == w.size(0), "skinny_gemm: output must be [M, N]");
+  TORCH_CHECK(x.size(0) >= 1 && x.size(0) <= 64, "skinny_gemm: 1 <= M <= 64 rows");
+  TORCH_CHECK(x.size(1) % 8 == 0, "skinny_gemm: K must be a multiple of 8");
+  check_aligned16(x, "x");
+  check_aligned16(w, "w");
+  TORCH_CHECK(epi >= pb::SKINNY_PLAIN && epi <= pb::SKINNY_GELU, "skinny_gemm: unknown epilogue");
+  c10::cuda::CUDAGuard guard(x.device());
+  pb::SkinnyArgs a;
+  a.X = x.data_ptr(), a.W = w.data_ptr(), a.Y = y.data_ptr();
+  a.ldx = x.stride(0), a.ldw = w.stride(0), a.ldy = y.stride(0);
+  a.M = int(x.size(0)), a.N = int(w.size(0)), a.K = int(x.size(1));
+  a.epi = epi;
+  if (bias.has_value()) {
+    check_f32(*bias, "bias");
+    TORCH_CHECK(bias->numel() == a.N && bias->is_contiguous(), "bias must be contiguous with N elements");
+    a.bias = bias->data_ptr<float>();
+  }
+  if (epi == pb::SKINNY_RESIDUAL) {
+    TORCH_CHECK(residual.has_value(), "the residual epilogue needs the residual");
+    check_bf16(*residual, "residual");
+    TORCH_CHECK(residual->dim() == 2 && residual->size(0) == a.M && residual->size(1) == a.N && residual->stride(1) == 1,
+                "residual must be [M, N]");
+    a.R = residual->data_ptr(), a.ldr = residual->stride(0);
+  }
+  a.num_sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+  const int splits = pb::skinny_gemm_splits(a.M, a.N, a.K, a.num_sms);
+  Tensor part;
+  if (splits > 1) part = torch::empty({(long long)splits * a.M * a.N}, x.options().dtype(at::kFloat));
+  pb::skinny_gemm_launch(a, splits > 1 ? part.data_ptr<float>() : nullptr, stream_of(x));
+  g_launches += splits > 1 ? 2 : 1;
+}
+// kc / vc: one layer of the cache, [B_max, H, S_max, dh]; q: rows of [B, >= H*dh] (the q third of the fused qkv)
+void decode_attention(const Tensor& q, const Tensor& kc, const Tensor& vc, const Tensor& pos, Tensor& out, int n_heads, double scale,
+                      const c10::optional<Tensor>& alibi_slopes) {
+  check_bf16(q, "q");
+  check_bf16(kc, "k_cache");
+  check_bf16(vc, "v_cache");
+  check_bf16(out, "out");
+  check_i32(pos, "pos");
+  TORCH_CHECK(kc.dim() == 4 && kc.is_contiguous() && vc.sizes() == kc.sizes() && vc.is_contiguous(), "k/v cache must be contiguous [B_max, H, S_max, dh]");
+  const int B = int(q.size(0)), H = int(kc.size(1)), S = int(kc.size(2)), dh = int(kc.size(3));
+  TORCH_CHECK(H == n_heads && (dh == 64 || dh == 128), "decode_attention: cache heads must equal n_heads and d_head be 64 or 128");
+  TORCH_CHECK(B <= kc.size(0) && pos.numel() >= B, "decode_attention: batch larger than the cache or the position vector");
+  TORCH_CHECK(q.dim() == 2 && q.stride(1) == 1 && q.size(1) >= H * dh, "q must be [B, >= H*dh] with unit inner stride");
+  TORCH_CHECK(out.dim() == 2 && out.size(0) == B && out.size(1) == H * dh && out.stride(1) == 1, "out must be [B, H*dh]");
+  if (alibi_slopes.has_value()) {
+    check_f32(*alibi_slopes, "alibi_slopes");
+    TORCH_CHECK(alibi_slopes->numel() == n_heads, "alibi_slopes must have n_heads elements");
+  }
+  c10::cuda::CUDAGuard guard(q.device());
+  const int splits = pb::decode_attention_splits(S);
+  Tensor po = torch::empty({(long long)B * H * splits * dh}, q.options().dtype(at::kFloat));
+  Tensor pml = torch::empty({(long long)B * H * splits * 2}, q.options().dtype(at::kFloat));
+  pb::decode_attention_launch(q.data_ptr(), q.stride(0), kc.data_ptr(), vc.data_ptr(), pos.data_ptr<int>(), out.data_ptr(), out.stride(0),
+                              po.data_ptr<float>(), pml.data_ptr<float>(), B, H, dh, S, float(scale),
+                              alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr, stream_of(q));
+  g_launches += 2;
+}
+void decode_append(Tensor& qkv, const Tensor& pos, Tensor& kc, Tensor& vc, const c10::optional<Tensor>& cos_t,
+                   const c10::optional<Tensor>& sin_t, int n_heads) {
+  check_bf16(qkv, "qkv");
+  check_bf16(kc, "k_cache");
+  check_bf16(vc, "v_cache");
+  check_i32(pos, "pos");
+  TORCH_CHECK(kc.dim() == 4 && kc.is_contiguous() && vc.sizes() == kc.sizes() && vc.is_contiguous(), "k/v cache must be contiguous [B_max, H, S_max, dh]");
+  const int B = int(qkv.size(0)), H = int(kc.size(1)), S = int(kc.size(2)), dh = int(kc.size(3));
+  TORCH_CHECK(H == n_heads && qkv.dim() == 2 && qkv.size(1) == 3 * H * dh && qkv.stride(1) == 1, "qkv must be [B, 3*H*dh]");
+  check_aligned16(qkv, "qkv");
+  TORCH_CHECK(B <= kc.size(0) && pos.numel() >= B, "decode_append: batch larger than the cache or the position vector");
+  TORCH_CHECK(cos_t.has_value() == sin_t.has_value(), "decode_append: pass both RoPE tables or neither");
+  if (cos_t.has_value()) {
+    check_f32(*cos_t, "cos");
+    check_f32(*sin_t, "sin");
+    TORCH_CHECK(cos_t->is_contiguous() && sin_t->is_contiguous() && cos_t->size(0) >= S && cos_t->size(1) == dh / 2,
+                "cos/sin must be [>= S_max, dh/2]");
+  }
+  c10::cuda::CUDAGuard guard(qkv.device());
+  pb::decode_append_launch(qkv.data_ptr(), qkv.stride(0), pos.data_ptr<int>(), kc.data_ptr(), vc.data_ptr(),
+                           cos_t.has_value() ? cos_t->data_ptr<float>() : nullptr, sin_t.has_value() ? sin_t->data_ptr<float>() : nullptr,
+                           B, H, dh, S, stream_of(qkv));
+  g_launches += 1;
+}
+void embed_pos(const Tensor& ids, const Tensor& pos, const Tensor& wte, const c10::optional<Tensor>& wpe, Tensor& out) {
+  check_i32(ids, "ids");
+  check_i32(pos, "pos");
+  check_bf16(wte, "wte");
+  check_bf16(out, "out");
+  const int B = int(out.size(0)), d = int(wte.size(1));
+  TORCH_CHECK(out.dim() == 2 && out.size(1) == d && out.is_contiguous() && d % 8 == 0, "out must be contiguous [B, d], d % 8 == 0");
+  TORCH_CHECK(ids.numel() >= B && pos.numel() >= B, "ids / pos shorter than the batch");
+  if (wpe.has_value()) {
+    check_bf16(*wpe, "wpe");
+    TORCH_CHECK(wpe->size(1) == d && wpe->is_contiguous(), "wpe must be contiguous [S, d]");
+  }
+  c10::cuda::CUDAGuard guard(ids.device());
+  pb::embed_pos_launch(ids.data_ptr<int>(), pos.data_ptr<int>(), wte.data_ptr(), opt_ptr(wpe), out.data_ptr(), B, d, int(wte.size(0)),
+                       stream_of(ids));
+  g_launches += 1;
+}
+void argmax_advance(const Tensor& logits, Tensor& ids, c10::optional<Tensor> pos) {
+  check_bf16(logits, "logits");
+  check_i32(ids, "ids");
+  TORCH_CHECK(logits.dim() == 2 && logits.stride(1) == 1, "logits must be [B, V] with unit inner stride");
+  const int B = int(logits.size(0));
+  TORCH_CHECK(ids.numel() >= B, "ids shorter than the batch");
+  if (pos.has_value()) {
+    check_i32(*pos, "pos");
+    TORCH_CHECK(pos->numel() >= B, "pos shorter than the batch");
+  }
+  c10::cuda::CUDAGuard guard(logits.device());
+  pb::argmax_advance_launch(logits.data_ptr(), logits.stride(0), B, int(logits.size(1)), ids.data_ptr<int>(),
+                            pos.has_value() ? pos->data_ptr<int>() : nullptr, stream_of(logits));
   g_launches += 1;
 }
 
@@ -621,6 +755,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("n_heads"), py::arg("scale"), py::arg("causal"), py::arg("alibi_slopes") = py::none());
   m.def("rope", &rope);
   m.def("embed_fwd", &embed_fwd);
+  m.def("skinny_gemm", &skinny_gemm, py::arg("x"), py::arg("w"), py::arg("y"), py::arg("bias") = py::none(), py::arg("residual") = py::none(),
+        py::arg("epi") = 0);
+  m.def("decode_attention", &decode_attention, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("pos"), py::arg("out"),
+        py::arg("n_heads"), py::arg("scale"), py::arg("alibi_slopes") = py::none());
+  m.def("decode_append", &decode_append, py::arg("qkv"), py::arg("pos"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cos") = py::none(),
+        py::arg("sin") = py::none(), py::arg("n_heads") = 1);
+  m.def("embed_pos", &embed_pos, py::arg("ids"), py::arg("pos"), py::arg("wte"), py::arg("wpe"), py::arg("out"));
+  m.def("argmax_advance", &argmax_advance, py::arg("logits"), py::arg("ids"), py::arg("pos") = py::none());
   m.def("embed_bwd", &embed_bwd);
   m.def("layernorm_fwd", &layernorm_fwd);
   m.def("layernorm_bwd", &layernorm_bwd);
@@ -669,4 +811,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.attr("EPI_GELU_GRAD") = int(pb::EPI_GELU_GRAD);
   m.attr("EPI_MUL") = int(pb::EPI_MUL);
   m.attr("EPI_GELU_GRAD_Q8") = int(pb::EPI_GELU_GRAD_Q8);
+  m.attr("SKINNY_PLAIN") = int(pb::SKINNY_PLAIN);
+  m.attr("SKINNY_RESIDUAL") = int(pb::SKINNY_RESIDUAL);
+  m.attr("SKINNY_GELU") = int(pb::SKINNY_GELU);
 }

@@ -1,0 +1,501 @@
+// Kernels of the KV-cached greedy decoder for sm_90a (layouts and contracts in decode.h).
+//
+//   * skinny GEMM  Y[M,N] = X[M,K] W[N,K]^T for M <= 64 rows: a decode step is bound by streaming the weights, so the
+//     weight rows fill the wgmma M side (m64) and the few activation rows are the N side (n8 / n16 / n32 / n64, "swap AB").
+//     One producer thread streams 64 x 64 weight tiles and the matching activation tile by TMA through a 6-stage mbarrier
+//     ring; one warpgroup issues the wgmmas. Every CTA owns 64 output columns and one K range; when the column tiles alone
+//     cannot fill the GPU, K is split and the fp32 partials are summed in split order by a second kernel (no float atomics,
+//     so the result does not depend on scheduling).
+//   * decode attention: one query per (sequence, head) against the cache, split over 256-key chunks (flash-decoding); the
+//     chunk results (unnormalised o, running max, sum) are combined in chunk order.
+//   * append (RoPE at each row's own position + cache write), embedding at per-row positions, argmax + position advance.
+#include <cuda.h>
+#include <cuda_bf16.h>
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <stdexcept>
+#include <string>
+
+#include "decode.h"
+#include "gemm_tcgen05.h"
+#include "ptx.cuh"
+#include "wgmma.cuh"
+
+namespace pb {
+
+namespace {
+
+#define PB_DECODE_CHECK(name)                                                                            \
+  do {                                                                                                   \
+    cudaError_t e__ = cudaGetLastError();                                                                \
+    if (e__ != cudaSuccess) throw std::runtime_error(std::string(name " launch: ") + cudaGetErrorString(e__)); \
+  } while (0)
+
+constexpr float LOG2E = 1.4426950408889634f;
+
+// ------------------------------------------------------------------------------------------- skinny GEMM
+constexpr int SK_BN = 64;                  // weight rows (output columns) per CTA = wgmma M
+constexpr int SK_BK = 64;                  // K elements per stage: 128 bytes per row, one 128B-swizzle atom row
+constexpr int SK_STAGES = 6;
+constexpr int SK_W_STAGE = SK_BN * 128;    // 8 KiB
+constexpr int SK_THREADS = 160;            // warps 0-3: MMA + epilogue (one warpgroup); warp 4: TMA producer
+
+template <int NB>
+constexpr int sk_smem_bytes() { return SK_STAGES * (SK_W_STAGE + NB * 128) + 2 * SK_STAGES * 8 + 1024; }
+
+struct SkParams {
+  const float* bias;
+  const __nv_bfloat16* R;
+  long long ldr;
+  __nv_bfloat16* Y;
+  long long ldy;
+  float* part;          // [splits, M, N] fp32 when splits > 1
+  int M, N, K, kb_per_split, splits;
+};
+
+template <int EPI>
+__device__ __forceinline__ float sk_finish(float v, const SkParams& p, int m, int n) {
+  if (p.bias) v += __ldg(p.bias + n);
+  if (EPI == SKINNY_RESIDUAL) v += __bfloat162float(p.R[(long long)m * p.ldr + n]);
+  if (EPI == SKINNY_GELU) v = gelu_exact(v);
+  return v;
+}
+
+template <int NB>
+__device__ __forceinline__ void sk_mma(float (&acc)[NB / 2], uint64_t wd, uint64_t xd, uint32_t accum) {
+  if constexpr (NB == 8) wgmma_bf16_ss_n8<0, 0>(acc, wd, xd, accum);
+  else if constexpr (NB == 16) wgmma_bf16_ss_n16<0, 0>(acc, wd, xd, accum);
+  else if constexpr (NB == 32) wgmma_bf16_ss_n32<0, 0>(acc, wd, xd, accum);
+  else wgmma_bf16_ss_n64<0, 0>(acc, wd, xd, accum);
+}
+
+template <int NB, int EPI>
+__global__ void __launch_bounds__(SK_THREADS)
+skinny_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const SkParams p) {
+  constexpr int X_STAGE = NB * 128;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sW = smem;
+  uint8_t* sX = sW + SK_STAGES * SK_W_STAGE;
+  uint64_t* full = reinterpret_cast<uint64_t*>(sX + SK_STAGES * X_STAGE);
+  uint64_t* empty = full + SK_STAGES;
+
+  const int n_blk = blockIdx.x, sp = blockIdx.y;
+  const int num_kb = (p.K + SK_BK - 1) / SK_BK;
+  const int kb0 = sp * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < SK_STAGES; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 4);   // one arrival per MMA warp
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (threadIdx.x >= 128) {
+    // ------------------------------------------------------------ TMA producer (one thread)
+    if (threadIdx.x == 128) {
+      prefetch_tmap(&tmW);
+      prefetch_tmap(&tmX);
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&empty[stage], phase ^ 1);
+        mbar_expect_tx(&full[stage], SK_W_STAGE + X_STAGE);
+        tma_load_2d(sW + stage * SK_W_STAGE, &tmW, &full[stage], kb * SK_BK, n_blk * SK_BN);
+        tma_load_2d(sX + stage * X_STAGE, &tmX, &full[stage], kb * SK_BK, 0);   // rows >= M arrive as zeros
+        if (++stage == SK_STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------- MMA warpgroup: D[64 weight rows, NB activation rows]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float acc[NB / 2];
+#pragma unroll
+  for (int i = 0; i < NB / 2; ++i) acc[i] = 0.f;
+  int stage = 0, prev = -1;
+  uint32_t phase = 0;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(&full[stage], phase);
+    const uint64_t wd = desc_sw128(sW + stage * SK_W_STAGE, 16);
+    const uint64_t xd = desc_sw128(sX + stage * X_STAGE, 16);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) sk_mma<NB>(acc, desc_add(wd, k * 32), desc_add(xd, k * 32), (kb > kb0 || k > 0) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();   // the previous stage's MMAs retired: release its shared memory
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+    prev = stage;
+    if (++stage == SK_STAGES) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc);
+  // accumulator (m64nNB): acc[4j + e] = weight row 16*warp + lane/4 + 8*(e/2), activation row 8j + 2*(lane%4) + e%2
+#pragma unroll
+  for (int j = 0; j < NB / 8; ++j) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int n = n_blk * SK_BN + warp * 16 + (lane >> 2) + 8 * (e >> 1);
+      const int m = 8 * j + 2 * (lane & 3) + (e & 1);
+      if (m >= p.M || n >= p.N) continue;
+      const float v = acc[4 * j + e];
+      if (p.splits > 1) p.part[((long long)sp * p.M + m) * p.N + n] = v;
+      else p.Y[(long long)m * p.ldy + n] = __float2bfloat16_rn(sk_finish<EPI>(v, p, m, n));
+    }
+  }
+}
+
+// the split partials of one output element, summed in split order, then the epilogue
+template <int EPI>
+__global__ void __launch_bounds__(256) skinny_reduce_kernel(const SkParams p) {
+  const long long total = (long long)p.M * p.N, plane = total;
+  for (long long i = blockIdx.x * 256LL + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const int m = int(i / p.N), n = int(i % p.N);
+    float v = 0.f;
+    for (int s = 0; s < p.splits; ++s) v += p.part[s * plane + i];
+    p.Y[(long long)m * p.ldy + n] = __float2bfloat16_rn(sk_finish<EPI>(v, p, m, n));
+  }
+}
+
+template <int NB, int EPI>
+void skinny_launch_inst(const CUtensorMap& tw, const CUtensorMap& tx, const SkParams& p, int tiles, cudaStream_t st) {
+  auto kern = skinny_gemm_kernel<NB, EPI>;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, sk_smem_bytes<NB>());
+    if (e != cudaSuccess) throw std::runtime_error(std::string("skinny gemm smem attr: ") + cudaGetErrorString(e));
+    configured = true;
+  }
+  kern<<<dim3(tiles, p.splits), SK_THREADS, sk_smem_bytes<NB>(), st>>>(tw, tx, p);
+  PB_DECODE_CHECK("skinny gemm");
+  if (p.splits > 1) {
+    const long long total = (long long)p.M * p.N;
+    const int blocks = int(std::min<long long>((total + 255) / 256, 132 * 8));
+    skinny_reduce_kernel<EPI><<<blocks, 256, 0, st>>>(p);
+    PB_DECODE_CHECK("skinny gemm split reduce");
+  }
+}
+
+template <int EPI>
+void skinny_launch_nb(const CUtensorMap& tw, const SkinnyArgs& a, const SkParams& p, int tiles, cudaStream_t st) {
+  const int nb = a.M <= 8 ? 8 : a.M <= 16 ? 16 : a.M <= 32 ? 32 : 64;
+  // activation tile: all M rows (box of nb rows; rows past M are filled with zeros by the TMA unit)
+  const CUtensorMap tx = make_tmap_2d(a.X, 2, false, a.K, a.M, a.ldx * 2, SK_BK, nb);
+  if (nb == 8) skinny_launch_inst<8, EPI>(tw, tx, p, tiles, st);
+  else if (nb == 16) skinny_launch_inst<16, EPI>(tw, tx, p, tiles, st);
+  else if (nb == 32) skinny_launch_inst<32, EPI>(tw, tx, p, tiles, st);
+  else skinny_launch_inst<64, EPI>(tw, tx, p, tiles, st);
+}
+
+// ------------------------------------------------------------------------------------------- decode attention
+constexpr int DA_CHUNK = 256;   // keys per CTA
+constexpr int DA_THREADS = 128;
+
+__device__ __forceinline__ float da_warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffff, v, o);
+  return v;
+}
+
+template <int DH, bool ALIBI>
+__global__ void __launch_bounds__(DA_THREADS)
+decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __nv_bfloat16* __restrict__ kc,
+                   const __nv_bfloat16* __restrict__ vc, const int* __restrict__ pos, float* __restrict__ po, float* __restrict__ pml,
+                   int H, int s_max, int n_split, float sc, const float* __restrict__ slopes) {
+  __shared__ float qs[DH];
+  __shared__ float ps[DA_CHUNK];
+  __shared__ float red[2][4];
+  __shared__ float os[4][DH];
+  const int s = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int len = pos[b] + 1;
+  const int j0 = s * DA_CHUNK, j1 = min(len, j0 + DA_CHUNK);
+  if (j0 >= j1) return;   // chunk past the sequence: the combine kernel reads only the chunks below pos[b] + 1
+  const long long slot = (long long)(b * H + h) * n_split + s;
+  for (int i = tid; i < DH; i += DA_THREADS) qs[i] = __bfloat162float(q[b * ldq + h * DH + i]) * sc;
+  __syncthreads();
+  const long long head = (long long)(b * H + h) * s_max * DH;
+  const float slope2 = ALIBI ? slopes[h] * LOG2E : 0.f;
+  // scores (log2 domain): one key per thread and pass, 16-byte loads of the key row, q broadcast from shared memory
+  float mx = -INFINITY;
+  for (int jj = tid; jj < DA_CHUNK; jj += DA_THREADS) {
+    const int j = j0 + jj;
+    float x = -INFINITY;
+    if (j < j1) {
+      const uint4* kr = reinterpret_cast<const uint4*>(kc + head + (long long)j * DH);
+      float acc = 0.f;
+#pragma unroll
+      for (int c = 0; c < DH / 8; ++c) {
+        const uint4 u = kr[c];
+        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+          const float2 f = unpack_bf16(w[t]);
+          acc = fmaf(qs[c * 8 + 2 * t], f.x, acc);
+          acc = fmaf(qs[c * 8 + 2 * t + 1], f.y, acc);
+        }
+      }
+      x = acc;
+      if (ALIBI) x = fmaf(slope2, float(j - (len - 1)), x);   // slope * (key - query)
+    }
+    ps[jj] = x;
+    mx = fmaxf(mx, x);
+  }
+  mx = warp_max_f(mx);
+  if (lane == 0) red[0][warp] = mx;
+  __syncthreads();
+  const float m = fmaxf(fmaxf(red[0][0], red[0][1]), fmaxf(red[0][2], red[0][3]));
+  float l = 0.f;
+  for (int jj = tid; jj < DA_CHUNK; jj += DA_THREADS) {
+    const float pv = (j0 + jj < j1) ? exp2f(ps[jj] - m) : 0.f;
+    ps[jj] = pv;
+    l += pv;
+  }
+  l = da_warp_sum(l);
+  if (lane == 0) red[1][warp] = l;
+  __syncthreads();
+  // P.V: warp w takes keys w, w+4, ...; each lane owns DH/32 consecutive output dims (coalesced value rows)
+  constexpr int PER = DH / 32;
+  float o[PER];
+#pragma unroll
+  for (int i = 0; i < PER; ++i) o[i] = 0.f;
+  for (int jj = warp; jj < j1 - j0; jj += 4) {
+    const float pv = ps[jj];
+    const __nv_bfloat16* vr = vc + head + (long long)(j0 + jj) * DH + lane * PER;
+    if constexpr (PER == 2) {
+      const float2 f = unpack_bf16(*reinterpret_cast<const uint32_t*>(vr));
+      o[0] = fmaf(pv, f.x, o[0]), o[1] = fmaf(pv, f.y, o[1]);
+    } else {
+      const uint2 u = *reinterpret_cast<const uint2*>(vr);
+      const float2 f0 = unpack_bf16(u.x), f1 = unpack_bf16(u.y);
+      o[0] = fmaf(pv, f0.x, o[0]), o[1] = fmaf(pv, f0.y, o[1]), o[2] = fmaf(pv, f1.x, o[2]), o[3] = fmaf(pv, f1.y, o[3]);
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < PER; ++i) os[warp][lane * PER + i] = o[i];
+  __syncthreads();
+  for (int i = tid; i < DH; i += DA_THREADS) po[slot * DH + i] = ((os[0][i] + os[1][i]) + os[2][i]) + os[3][i];
+  if (tid == 0) {
+    pml[2 * slot] = m;
+    pml[2 * slot + 1] = ((red[1][0] + red[1][1]) + red[1][2]) + red[1][3];
+  }
+}
+
+template <int DH>
+__global__ void __launch_bounds__(DH) decode_combine_kernel(const float* __restrict__ po, const float* __restrict__ pml,
+                                                            const int* __restrict__ pos, __nv_bfloat16* __restrict__ out, long long ldo,
+                                                            int H, int n_split) {
+  const int h = blockIdx.x, b = blockIdx.y, t = threadIdx.x;
+  const int used = (pos[b] + 1 + DA_CHUNK - 1) / DA_CHUNK;
+  const long long slot0 = (long long)(b * H + h) * n_split;
+  float M = -INFINITY;
+  for (int s = 0; s < used; ++s) M = fmaxf(M, pml[2 * (slot0 + s)]);
+  float L = 0.f, o = 0.f;
+  for (int s = 0; s < used; ++s) {
+    const float w = exp2f(pml[2 * (slot0 + s)] - M);
+    L = fmaf(w, pml[2 * (slot0 + s) + 1], L);
+    o = fmaf(w, po[(slot0 + s) * DH + t], o);
+  }
+  out[b * ldo + h * DH + t] = __float2bfloat16_rn(o / L);
+}
+
+// ------------------------------------------------------------------------------------------- append / embed / argmax
+__global__ void __launch_bounds__(128) decode_append_kernel(__nv_bfloat16* __restrict__ qkv, long long ld, const int* __restrict__ pos,
+                                                            __nv_bfloat16* __restrict__ kc, __nv_bfloat16* __restrict__ vc,
+                                                            const float* __restrict__ cosT, const float* __restrict__ sinT, int H,
+                                                            int dh, int s_max) {
+  const int b = blockIdx.x, p = pos[b];
+  const int d = H * dh, half = dh / 2, groups = half / 8, vec = dh / 8;
+  __nv_bfloat16* row = qkv + b * ld;
+  const long long cache_row = ((long long)b * H) * s_max + p;   // + h * s_max: row of head h
+  if (cosT != nullptr) {
+    // rotate-half RoPE at position p, the arithmetic of rope_kernel: q in place, k straight into the cache
+    for (int i = threadIdx.x; i < 2 * H * groups; i += blockDim.x) {
+      const int g = i % groups, h = (i / groups) % H, which = i / (groups * H);
+      __nv_bfloat16* src = row + which * d + h * dh + g * 8;
+      const uint4 a = *reinterpret_cast<const uint4*>(src);
+      const uint4 bb = *reinterpret_cast<const uint4*>(src + half);
+      const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {bb.x, bb.y, bb.z, bb.w};
+      uint32_t oa[4], ob[4];
+      const float* c = cosT + (long long)p * half + g * 8;
+      const float* sn = sinT + (long long)p * half + g * 8;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float2 x1 = unpack_bf16(aw[k]), x2 = unpack_bf16(bw[k]);
+        const float c0 = c[2 * k], c1 = c[2 * k + 1], s0 = sn[2 * k], s1 = sn[2 * k + 1];
+        oa[k] = pack_bf16(x1.x * c0 - x2.x * s0, x1.y * c1 - x2.y * s1);
+        ob[k] = pack_bf16(x2.x * c0 + x1.x * s0, x2.y * c1 + x1.y * s1);
+      }
+      __nv_bfloat16* dst = which == 0 ? src : kc + (cache_row + (long long)h * s_max) * dh + g * 8;
+      *reinterpret_cast<uint4*>(dst) = make_uint4(oa[0], oa[1], oa[2], oa[3]);
+      *reinterpret_cast<uint4*>(dst + half) = make_uint4(ob[0], ob[1], ob[2], ob[3]);
+    }
+  } else {
+    for (int i = threadIdx.x; i < H * vec; i += blockDim.x) {
+      const int h = i / vec, c = i % vec;
+      *reinterpret_cast<uint4*>(kc + (cache_row + (long long)h * s_max) * dh + c * 8) =
+          *reinterpret_cast<const uint4*>(row + d + h * dh + c * 8);
+    }
+  }
+  for (int i = threadIdx.x; i < H * vec; i += blockDim.x) {
+    const int h = i / vec, c = i % vec;
+    *reinterpret_cast<uint4*>(vc + (cache_row + (long long)h * s_max) * dh + c * 8) =
+        *reinterpret_cast<const uint4*>(row + 2 * d + h * dh + c * 8);
+  }
+}
+
+__global__ void __launch_bounds__(128) embed_pos_kernel(const int* __restrict__ ids, const int* __restrict__ pos,
+                                                        const __nv_bfloat16* __restrict__ wte, const __nv_bfloat16* __restrict__ wpe,
+                                                        __nv_bfloat16* __restrict__ out, int d, int V) {
+  const int b = blockIdx.x;
+  int id = ids[b];
+  id = id < 0 ? 0 : (id >= V ? V - 1 : id);
+  const uint4* a = reinterpret_cast<const uint4*>(wte + (long long)id * d);
+  const uint4* e = wpe ? reinterpret_cast<const uint4*>(wpe + (long long)pos[b] * d) : nullptr;
+  uint4* o = reinterpret_cast<uint4*>(out + (long long)b * d);
+  for (int i = threadIdx.x; i < d / 8; i += blockDim.x) {
+    uint4 u = a[i];
+    if (e) {
+      const uint4 w = e[i];
+      const uint32_t x[4] = {u.x, u.y, u.z, u.w}, y[4] = {w.x, w.y, w.z, w.w};
+      uint32_t r[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float2 f = unpack_bf16(x[k]), g = unpack_bf16(y[k]);
+        r[k] = pack_bf16(f.x + g.x, f.y + g.y);
+      }
+      u = make_uint4(r[0], r[1], r[2], r[3]);
+    }
+    o[i] = u;
+  }
+}
+
+__device__ __forceinline__ void argmax_pick(float& best, int& idx, float ob, int oi) {
+  if (ob > best || (ob == best && oi < idx)) best = ob, idx = oi;
+}
+
+__global__ void __launch_bounds__(1024) argmax_advance_kernel(const __nv_bfloat16* __restrict__ logits, long long ldl, int V,
+                                                              int* __restrict__ ids, int* __restrict__ pos) {
+  __shared__ float sb[32];
+  __shared__ int si[32];
+  const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  float best = -INFINITY;
+  int idx = 0x7fffffff;
+  for (int v = threadIdx.x; v < V; v += blockDim.x) {
+    const float x = __bfloat162float(logits[b * ldl + v]);
+    if (x > best) best = x, idx = v;   // ascending v: the first maximum of this thread's slice
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) argmax_pick(best, idx, __shfl_xor_sync(0xffffffff, best, o), __shfl_xor_sync(0xffffffff, idx, o));
+  if (lane == 0) sb[warp] = best, si[warp] = idx;
+  __syncthreads();
+  if (warp == 0) {
+    const int nw = blockDim.x >> 5;
+    best = lane < nw ? sb[lane] : -INFINITY;
+    idx = lane < nw ? si[lane] : 0x7fffffff;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) argmax_pick(best, idx, __shfl_xor_sync(0xffffffff, best, o), __shfl_xor_sync(0xffffffff, idx, o));
+    if (lane == 0) {
+      ids[b] = idx == 0x7fffffff ? 0 : idx;
+      if (pos) pos[b] += 1;
+    }
+  }
+}
+
+}  // namespace
+
+// ------------------------------------------------------------------------------------------- host
+int skinny_gemm_splits(int M, int N, int K, int num_sms) {
+  (void)M;
+  const int tiles = (N + SK_BN - 1) / SK_BN;
+  const int num_kb = (K + SK_BK - 1) / SK_BK;
+  // aim for two resident CTAs per SM, keep >= 2 k-blocks per split
+  int s = (2 * num_sms + tiles - 1) / tiles;
+  const int max_s = num_kb / 2 > 1 ? num_kb / 2 : 1;
+  if (s > max_s) s = max_s;
+  if (s < 1) s = 1;
+  const int per = (num_kb + s - 1) / s;
+  return (num_kb + per - 1) / per;   // no empty tail split
+}
+
+void skinny_gemm_launch(const SkinnyArgs& a, float* partials, cudaStream_t st) {
+  if (a.M < 1 || a.M > 64) throw std::runtime_error("photon_b200 skinny gemm: 1 <= M <= 64");
+  if (a.N < 1 || a.K < 1 || a.K % 8) throw std::runtime_error("photon_b200 skinny gemm: K must be a positive multiple of 8");
+  const int splits = skinny_gemm_splits(a.M, a.N, a.K, a.num_sms);
+  if (splits > 1 && !partials) throw std::runtime_error("photon_b200 skinny gemm: split-K needs the fp32 partial buffer");
+  SkParams p{};
+  p.bias = a.bias;
+  p.R = reinterpret_cast<const __nv_bfloat16*>(a.R), p.ldr = a.ldr;
+  p.Y = reinterpret_cast<__nv_bfloat16*>(a.Y), p.ldy = a.ldy;
+  p.part = partials;
+  p.M = a.M, p.N = a.N, p.K = a.K, p.splits = splits;
+  const int num_kb = (a.K + SK_BK - 1) / SK_BK;
+  p.kb_per_split = (num_kb + splits - 1) / splits;
+  const int tiles = (a.N + SK_BN - 1) / SK_BN;
+  const CUtensorMap tw = make_tmap_2d(a.W, 2, false, a.K, a.N, a.ldw * 2, SK_BK, SK_BN);
+  if (a.epi == SKINNY_PLAIN) skinny_launch_nb<SKINNY_PLAIN>(tw, a, p, tiles, st);
+  else if (a.epi == SKINNY_RESIDUAL) skinny_launch_nb<SKINNY_RESIDUAL>(tw, a, p, tiles, st);
+  else if (a.epi == SKINNY_GELU) skinny_launch_nb<SKINNY_GELU>(tw, a, p, tiles, st);
+  else throw std::runtime_error("photon_b200 skinny gemm: unknown epilogue");
+}
+
+int decode_attention_splits(int s_max) { return (s_max + DA_CHUNK - 1) / DA_CHUNK; }
+
+void decode_attention_launch(const void* q, long long ldq, const void* kc, const void* vc, const int* pos, void* out, long long ldo,
+                             float* partial_o, float* partial_ml, int B, int H, int dh, int s_max, float scale, const float* alibi_slopes,
+                             cudaStream_t st) {
+  if (B < 1) return;
+  const int n_split = decode_attention_splits(s_max);
+  const dim3 grid(n_split, H, B);
+  const auto* qq = (const __nv_bfloat16*)q;
+  const auto* kk = (const __nv_bfloat16*)kc;
+  const auto* vv = (const __nv_bfloat16*)vc;
+  const float sc = scale * LOG2E;
+#define PB_DA(D, A)                                                                                                         \
+  {                                                                                                                         \
+    decode_attn_kernel<D, A><<<grid, DA_THREADS, 0, st>>>(qq, ldq, kk, vv, pos, partial_o, partial_ml, H, s_max, n_split, sc, \
+                                                         alibi_slopes);                                                     \
+    PB_DECODE_CHECK("decode attention");                                                                                    \
+    decode_combine_kernel<D><<<dim3(H, B), D, 0, st>>>(partial_o, partial_ml, pos, (__nv_bfloat16*)out, ldo, H, n_split);   \
+    PB_DECODE_CHECK("decode attention combine");                                                                            \
+    return;                                                                                                                 \
+  }
+  if (dh == 64 && !alibi_slopes) PB_DA(64, false)
+  if (dh == 64) PB_DA(64, true)
+  if (dh == 128 && !alibi_slopes) PB_DA(128, false)
+  if (dh == 128) PB_DA(128, true)
+#undef PB_DA
+  throw std::runtime_error("photon_b200 decode attention: d_head must be 64 or 128");
+}
+
+void decode_append_launch(void* qkv, long long ldqkv, const int* pos, void* kc, void* vc, const float* cosT, const float* sinT, int B,
+                          int H, int dh, int s_max, cudaStream_t st) {
+  if (B < 1) return;
+  if (dh % 16) throw std::runtime_error("photon_b200 decode append: d_head must be a multiple of 16");
+  decode_append_kernel<<<B, 128, 0, st>>>((__nv_bfloat16*)qkv, ldqkv, pos, (__nv_bfloat16*)kc, (__nv_bfloat16*)vc, cosT, sinT, H, dh,
+                                          s_max);
+  PB_DECODE_CHECK("decode append");
+}
+
+void embed_pos_launch(const int* ids, const int* pos, const void* wte, const void* wpe, void* out, int B, int d, int V, cudaStream_t st) {
+  if (B < 1) return;
+  embed_pos_kernel<<<B, 128, 0, st>>>(ids, pos, (const __nv_bfloat16*)wte, (const __nv_bfloat16*)wpe, (__nv_bfloat16*)out, d, V);
+  PB_DECODE_CHECK("embed_pos");
+}
+
+void argmax_advance_launch(const void* logits, long long ldl, int B, int V, int* ids, int* pos, cudaStream_t st) {
+  if (B < 1) return;
+  argmax_advance_kernel<<<B, 1024, 0, st>>>((const __nv_bfloat16*)logits, ldl, V, ids, pos);
+  PB_DECODE_CHECK("argmax");
+}
+
+}  // namespace pb

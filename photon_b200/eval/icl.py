@@ -9,10 +9,12 @@ self-contained implementation of the two task types that dominate those tables:
 * ``multiple_choice``     — pick the choice with the highest length-normalised log-likelihood;
   ``schema`` tasks are scored the same way with the context varying instead of the continuation.
 
-* ``generation_task_with_answers`` — greedy decoding (one ``logits_fn`` call per new token, no KV cache: this is an
-  evaluation utility, not a serving path) until ``max_new_tokens`` or an ``early_stopping_criteria`` string; exact match
-  against any of the ``answer`` / ``aliases`` after llm-foundry's normalisation (lower-case, punctuation and articles
-  stripped) unless ``do_normalization: false``; with a ``cot_delimiter`` only the text after it counts.
+* ``generation_task_with_answers`` — greedy decoding until ``max_new_tokens`` or an ``early_stopping_criteria`` string; exact
+  match against any of the ``answer`` / ``aliases`` after llm-foundry's normalisation (lower-case, punctuation and articles
+  stripped) unless ``do_normalization: false``; with a ``cot_delimiter`` only the text after it counts. With a ``decoder``
+  (a KV-cached batched decoder such as :meth:`B200Engine.decoder`) the rows are decoded in batches of the task's
+  ``batch_size``; rows whose prompt plus ``max_new_tokens`` exceeds the decoder's cache, and every row when there is no
+  decoder, recompute the last ``max_seq_len`` tokens with ``logits_fn`` for every new token (a sliding window, batch of one).
 
 Datasets are jsonl files resolved against ``icl_tasks_config.root_dir`` (there is no network, so missing files yield
 ``skipped``).
@@ -53,11 +55,40 @@ def _rows(path: Path) -> list[dict[str, Any]]:
     return [json.loads(l) for l in path.read_text().splitlines() if l.strip()]
 
 
-class ICLEvaluator:
-    """``logits_fn(ids [B,S] LongTensor) -> [B,S,V]`` abstracts the model (torch backend or engine)."""
+class _RecomputeDecoder:
+    """Greedy decoding without a cache: every new token runs ``logits_fn`` on the last ``max_seq_len`` tokens (batch of one).
+    Same protocol as the cached decoders: ``start(prompts, max_new_tokens)`` returns the first new token of each prompt,
+    ``step()`` the next one."""
 
-    def __init__(self, logits_fn: Callable[[torch.Tensor], torch.Tensor], tokenizer: Any, max_seq_len: int, root_dir: str | None = None) -> None:
+    max_batch = 1
+
+    def __init__(self, logits_fn: Callable[[torch.Tensor], torch.Tensor], max_seq_len: int) -> None:
+        self.logits_fn, self.max_seq_len = logits_fn, max_seq_len
+        self.ids: list[int] = []
+
+    def _next(self) -> list[int]:
+        window = self.ids[-self.max_seq_len:]
+        nxt = int(self.logits_fn(torch.tensor([window], dtype=torch.long))[0, -1].float().argmax())
+        self.ids.append(nxt)
+        return [nxt]
+
+    def start(self, prompts: list[list[int]], max_new_tokens: int) -> list[int]:
+        (self.ids,) = [list(p) for p in prompts]
+        return self._next()
+
+    def step(self) -> list[int]:
+        return self._next()
+
+
+class ICLEvaluator:
+    """``logits_fn(ids [B,S] LongTensor) -> [B,S,V]`` abstracts the model (torch backend or engine); ``decoder`` (optional) is
+    a batched KV-cached greedy decoder with ``max_batch``, ``max_seq_len``, ``start(prompts, max_new_tokens)`` and ``step()``
+    that generation tasks use for every row that fits its cache."""
+
+    def __init__(self, logits_fn: Callable[[torch.Tensor], torch.Tensor], tokenizer: Any, max_seq_len: int, root_dir: str | None = None,
+                 decoder: Any = None) -> None:
         self.logits_fn, self.tok, self.max_seq_len, self.root = logits_fn, tokenizer, int(max_seq_len), Path(root_dir or ".")
+        self.decoder = decoder
 
     def _enc(self, text: str) -> list[int]:
         if hasattr(self.tok, "encode") and not hasattr(self.tok, "__call__"):
@@ -86,20 +117,48 @@ class ICLEvaluator:
 
     @torch.no_grad()
     def _generate(self, ctx: list[int], max_new_tokens: int, stops: list[str]) -> str:
-        """Greedy continuation of ``ctx`` as text, cut at the first stop string."""
-        ids, new = list(ctx), []
+        """Greedy continuation of ``ctx`` as text, cut at the first stop string (sliding window, no cache)."""
+        return self._generate_batch(_RecomputeDecoder(self.logits_fn, self.max_seq_len), [ctx], max_new_tokens, stops)[0]
+
+    def _generate_batch(self, dec: Any, ctxs: list[list[int]], max_new_tokens: int, stops: list[str]) -> list[str]:
+        """Greedy continuations of a batch of prompts with ``dec``. Per row: EOS ends the row and is not emitted; after each
+        token the decoded text is checked against the stop strings and cut at the first one."""
         eos = getattr(self.tok, "eos_token_id", None)
-        for _ in range(max_new_tokens):
-            window = ids[-self.max_seq_len:]
-            nxt = int(self.logits_fn(torch.tensor([window], dtype=torch.long))[0, -1].float().argmax())
-            if eos is not None and nxt == eos:
+        new: list[list[int]] = [[] for _ in ctxs]
+        texts: list[str | None] = [None] * len(ctxs)
+        if max_new_tokens <= 0:
+            return [self.tok.decode([]) for _ in ctxs]
+        toks = dec.start(ctxs, max_new_tokens)
+        for t in range(max_new_tokens):
+            for i, nxt in enumerate(toks):
+                if texts[i] is not None:
+                    continue
+                if eos is not None and nxt == eos:
+                    texts[i] = self.tok.decode(new[i])
+                    continue
+                new[i].append(nxt)
+                text = self.tok.decode(new[i])
+                hit = [text.index(s) for s in stops if s and s in text]
+                if hit:
+                    texts[i] = text[: min(hit)]
+            if t == max_new_tokens - 1 or all(x is not None for x in texts):
                 break
-            ids.append(nxt), new.append(nxt)
-            text = self.tok.decode(new)
-            hit = [text.index(s) for s in stops if s and s in text]
-            if hit:
-                return text[: min(hit)]
-        return self.tok.decode(new)
+            toks = dec.step()
+        return [x if x is not None else self.tok.decode(n) for x, n in zip(texts, new)]
+
+    @torch.no_grad()
+    def _generate_rows(self, ctxs: list[list[int]], max_new_tokens: int, stops: list[str], batch_size: int) -> list[str]:
+        """Every row that fits the decoder's cache in batches of ``batch_size``; the others one by one on the sliding window."""
+        out: list[str | None] = [None] * len(ctxs)
+        dec = self.decoder
+        if dec is not None:
+            fits = [i for i, c in enumerate(ctxs) if 1 <= len(c) and len(c) + max_new_tokens <= dec.max_seq_len]
+            n = max(1, min(int(batch_size), dec.max_batch))
+            for lo in range(0, len(fits), n):
+                idx = fits[lo: lo + n]
+                for i, text in zip(idx, self._generate_batch(dec, [ctxs[i] for i in idx], max_new_tokens, stops)):
+                    out[i] = text
+        return [x if x is not None else self._generate(c, max_new_tokens, stops) for x, c in zip(out, ctxs)]
 
     def evaluate_task(self, task: dict[str, Any]) -> dict[str, float | str]:
         t = expand_task(task)
@@ -115,11 +174,15 @@ class ICLEvaluator:
         out: dict[str, float | str] = {}
         for k in t["num_fewshot"]:
             correct = 0
+            texts: list[str] = []
+            if kind == "generation_task_with_answers":
+                ctxs = [self._enc(self._fewshot_prefix(rows, i, k, t) + t["question_prelimiter"] + r["context"]
+                                  + t["continuation_delimiter"].rstrip()) for i, r in enumerate(rows)]
+                texts = self._generate_rows(ctxs, int(t["max_new_tokens"]), list(t["early_stopping_criteria"] or []), int(t["batch_size"]))
             for i, r in enumerate(rows):
                 prefix = self._fewshot_prefix(rows, i, k, t)
                 if kind == "generation_task_with_answers":
-                    ctx = self._enc(prefix + t["question_prelimiter"] + r["context"] + t["continuation_delimiter"].rstrip())
-                    text = self._generate(ctx, int(t["max_new_tokens"]), list(t["early_stopping_criteria"] or []))
+                    text = texts[i]
                     if t["cot_delimiter"] and t["cot_delimiter"] in text:
                         text = text.split(t["cot_delimiter"])[-1]
                     golds = [str(r["answer"])] + [str(a) for a in r.get("aliases", [])]
@@ -188,11 +251,13 @@ class EvalGauntlet:
         return out
 
 
-def run_icl_suite(logits_fn: Callable[[torch.Tensor], torch.Tensor], tokenizer: Any, cfg: Any, max_seq_len: int) -> dict[str, Any]:
-    """Evaluate every task of ``cfg.icl_tasks_config`` and fold through ``cfg.eval_gauntlet_config``."""
+def run_icl_suite(logits_fn: Callable[[torch.Tensor], torch.Tensor], tokenizer: Any, cfg: Any, max_seq_len: int,
+                  decoder: Any = None) -> dict[str, Any]:
+    """Evaluate every task of ``cfg.icl_tasks_config`` and fold through ``cfg.eval_gauntlet_config``; generation tasks decode with
+    ``decoder`` when one is given (see :class:`ICLEvaluator`)."""
     icl = cfg.get("icl_tasks_config") or {}
     tasks = icl.get("icl_tasks") or []
-    ev = ICLEvaluator(logits_fn, tokenizer, max_seq_len, icl.get("root_dir"))
+    ev = ICLEvaluator(logits_fn, tokenizer, max_seq_len, icl.get("root_dir"), decoder=decoder)
     metrics: dict[str, Any] = {}
     for t in tasks:
         metrics.update({k: v for k, v in ev.evaluate_task(dict(t)).items() if not (k == "status")})

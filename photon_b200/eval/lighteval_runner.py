@@ -60,8 +60,8 @@ def to_icl_task(entry: dict[str, Any]) -> dict[str, Any] | None:
 
 
 def run_task_list(tasks_file: str | Path, logits_fn: Callable[[torch.Tensor], torch.Tensor], tokenizer: Any, max_seq_len: int,
-                  data_root: str | Path) -> dict[str, Any]:
-    ev = ICLEvaluator(logits_fn, tokenizer, max_seq_len, str(data_root))
+                  data_root: str | Path, decoder: Any = None) -> dict[str, Any]:
+    ev = ICLEvaluator(logits_fn, tokenizer, max_seq_len, str(data_root), decoder=decoder)
     results: dict[str, Any] = {}
     for entry in parse_task_list(tasks_file):
         key = f"{entry['suite']}|{entry['task']}|{entry['num_fewshot']}"
@@ -98,18 +98,30 @@ def main() -> None:
     dev = torch.device("cuda" if torch.cuda.is_available() else "cpu")
     if dev.type == "cpu" and mcfg.attn_impl == "flash":
         mcfg.attn_impl = "torch"
-    model = MPTForCausalLM(mcfg, device=dev, seed=17)
-    if a.checkpoint:
-        flat = FlatParams(model, device=dev, with_grad=False)
-        flat.load_ndarrays(load_model_parameters_from_file(a.checkpoint)[: len(flat.names)])
-    model.eval()
+    decoder = None
+    if dev.type == "cuda":
+        # the engine scores with the same torch-module forward (``engine.logits``) and generates with its KV-cached decoder
+        from photon_b200.models.engine import B200Engine
 
-    @torch.no_grad()
-    def logits_fn(ids: torch.Tensor) -> torch.Tensor:
-        with torch.autocast(dev.type, dtype=torch.bfloat16, enabled=dev.type == "cuda"):
+        engine = B200Engine(mcfg, device=dev, seed=17)
+        if a.checkpoint:
+            engine.flat.load_ndarrays(load_model_parameters_from_file(a.checkpoint)[: len(engine.flat.names)])
+            engine.params_updated()
+        engine.train_mode(False)
+        logits_fn = engine.logits
+        decoder = engine.decoder(64)
+    else:
+        model = MPTForCausalLM(mcfg, device=dev, seed=17)
+        if a.checkpoint:
+            flat = FlatParams(model, device=dev, with_grad=False)
+            flat.load_ndarrays(load_model_parameters_from_file(a.checkpoint)[: len(flat.names)])
+        model.eval()
+
+        @torch.no_grad()
+        def logits_fn(ids: torch.Tensor) -> torch.Tensor:
             return model(ids.to(dev))
 
-    res = run_task_list(a.tasks, logits_fn, build_tokenizer(a.tokenizer), mcfg.max_seq_len, a.data_root)
+    res = run_task_list(a.tasks, logits_fn, build_tokenizer(a.tokenizer), mcfg.max_seq_len, a.data_root, decoder=decoder)
     text = json.dumps(res, indent=1)
     if a.out:
         Path(a.out).write_text(text)

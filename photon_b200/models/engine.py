@@ -541,6 +541,17 @@ class B200Engine:
         with torch.autocast("cuda", dtype=torch.bfloat16):
             return self.model(ids.to(self.device))
 
+    def decoder(self, max_batch: int) -> Any:
+        """A KV-cached greedy decoder (:class:`photon_b200.models.decode.KVDecoder`) over this engine's bf16 weights for batches of
+        up to ``max_batch`` sequences, or None where it does not apply: full parameter sharding, a d_head the wgmma attention
+        kernels do not cover, or a ``max_seq_len`` that is not a multiple of the 128-row prefill tiles. It owns its cache and
+        buffers; the training workspace and captured training graphs are left alone."""
+        if self.zero3 is not None or self.cfg.d_head not in (64, 128) or self.cfg.max_seq_len % 128:
+            return None
+        from photon_b200.models.decode import KVDecoder
+
+        return KVDecoder(self, max_batch, use_graph=self.use_graph)
+
     def train_mode(self, on: bool = True) -> None:
         if self.model is not None:
             self.model.train(on)

@@ -264,3 +264,45 @@ def rope_(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_heads: int,
     transposed rotation (what the gradients of q and k need)."""
     ext().rope(qkv, cos, sin, int(n_heads), bool(inverse))
     return qkv
+
+
+# ---------------------------------------------------------------------------- decoding
+SKINNY_PLAIN, SKINNY_RESIDUAL, SKINNY_GELU = 0, 1, 2
+
+
+def skinny_gemm(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor, bias: torch.Tensor | None = None,
+                residual: torch.Tensor | None = None, gelu: bool = False) -> torch.Tensor:
+    """``out[M,N] = x[M,K] @ w[N,K]^T (+ bias) (+ residual | then exact GELU)`` for 1 <= M <= 64 rows (decode steps): the weight
+    rows stream through the GPU once, K is split when the 64-column tiles cannot fill it, and split partials are summed in a
+    fixed order, so the result is bitwise reproducible."""
+    epi = SKINNY_GELU if gelu else (SKINNY_RESIDUAL if residual is not None else SKINNY_PLAIN)
+    ext().skinny_gemm(x, w, out, bias, residual, epi)
+    return out
+
+
+def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, pos: torch.Tensor, out: torch.Tensor, n_heads: int,
+                     scale: float, alibi_slopes: torch.Tensor | None = None) -> torch.Tensor:
+    """One query row per sequence (``q`` [B, >= H*dh]) against one layer of the cache (``k_cache`` / ``v_cache``
+    [B_max, H, S_max, dh]) over keys ``0..pos[b]`` (int32 on the device); ``out`` [B, H*dh]."""
+    ext().decode_attention(q, k_cache, v_cache, pos, out, int(n_heads), float(scale), alibi_slopes)
+    return out
+
+
+def decode_append(qkv: torch.Tensor, pos: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor,
+                  rope: tuple[torch.Tensor, torch.Tensor] | None, n_heads: int) -> None:
+    """Rotate q / k of every row of the fused ``qkv`` [B, 3d] at position ``pos[b]`` (``rope`` = the ``rope_`` tables, or None)
+    and write k / v into the cache at ``pos[b]``."""
+    cos, sin = rope if rope is not None else (None, None)
+    ext().decode_append(qkv, pos, k_cache, v_cache, cos, sin, int(n_heads))
+
+
+def embed_pos(ids: torch.Tensor, pos: torch.Tensor, wte: torch.Tensor, wpe: torch.Tensor | None, out: torch.Tensor) -> torch.Tensor:
+    """``out[b] = wte[ids[b]] + wpe[pos[b]]`` with int32 ``ids`` / ``pos`` on the device."""
+    ext().embed_pos(ids, pos, wte, wpe, out)
+    return out
+
+
+def argmax_advance(logits: torch.Tensor, ids: torch.Tensor, pos: torch.Tensor | None = None) -> torch.Tensor:
+    """``ids[b] = argmax(logits[b])`` (lowest index on ties) and ``pos[b] += 1`` when ``pos`` is given."""
+    ext().argmax_advance(logits, ids, pos)
+    return ids

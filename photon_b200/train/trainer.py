@@ -153,7 +153,7 @@ class Trainer:
         self.fit_start_batch, self.fit_end_batch = 0, None
         self.closed = False
         self.last_batch_stats: dict[str, float] = {}
-        self.icl_suite: Any = None              # callable(logits_fn) -> metrics; set by get_trainer_object from icl_tasks_config
+        self.icl_suite: Any = None              # callable(logits_fn, decoder=None) -> metrics; set by get_trainer_object from icl_tasks_config
         self.last_icl_metrics: dict[str, float] = {}
 
         seq = self.model_cfg.max_seq_len
@@ -430,7 +430,7 @@ class Trainer:
         vals = st.eval_metric_values
         self.log({f"metrics/{k}": v for k, v in vals.items()})
         if self.icl_suite is not None:   # llm-foundry's ICL evaluators + EvalGauntlet run as part of every trainer.eval()
-            icl = {k: v for k, v in self.icl_suite(st.backend.logits).items() if isinstance(v, (int, float))} if self.rank == 0 else {}
+            icl = {k: v for k, v in self._run_icl_suite(st.backend).items() if isinstance(v, (int, float))} if self.rank == 0 else {}
             self.last_icl_metrics = icl
             if self.world_size > 1 and dist.is_initialized():
                 # the suite runs on rank 0 only and can take minutes: the others wait HERE, on the host, instead of inside the next
@@ -441,6 +441,18 @@ class Trainer:
         self._emit("eval_end")
         self._flush_logs()
         return vals
+
+    def _run_icl_suite(self, backend: Any) -> dict[str, Any]:
+        """The ICL suite on ``backend``; generation tasks decode with the backend's KV-cached decoder when it has one (the
+        cache is sized by the largest task batch and freed afterwards)."""
+        make = getattr(backend, "decoder", None)
+        decoder = make(64) if make is not None else None
+        if decoder is None:
+            return self.icl_suite(backend.logits)
+        try:
+            return self.icl_suite(backend.logits, decoder=decoder)
+        finally:
+            decoder.close()
 
     def _eval_batch_stats(self, ids: torch.Tensor) -> dict[str, float]:
         """Sum-type statistics of one eval batch, computed in ``device_eval_microbatch_size`` slices (``auto`` halves the
