@@ -390,7 +390,7 @@ void decode_attention(const Tensor& q, const Tensor& kc, const Tensor& vc, const
   g_launches += 2;
 }
 void decode_append(Tensor& qkv, const Tensor& pos, Tensor& kc, Tensor& vc, const c10::optional<Tensor>& cos_t,
-                   const c10::optional<Tensor>& sin_t, int n_heads) {
+                   const c10::optional<Tensor>& sin_t, int n_heads, const c10::optional<Tensor>& slot) {
   check_bf16(qkv, "qkv");
   check_bf16(kc, "k_cache");
   check_bf16(vc, "v_cache");
@@ -399,7 +399,13 @@ void decode_append(Tensor& qkv, const Tensor& pos, Tensor& kc, Tensor& vc, const
   const int B = int(qkv.size(0)), H = int(kc.size(1)), S = int(kc.size(2)), dh = int(kc.size(3));
   TORCH_CHECK(H == n_heads && qkv.dim() == 2 && qkv.size(1) == 3 * H * dh && qkv.stride(1) == 1, "qkv must be [B, 3*H*dh]");
   check_aligned16(qkv, "qkv");
-  TORCH_CHECK(B <= kc.size(0) && pos.numel() >= B, "decode_append: batch larger than the cache or the position vector");
+  TORCH_CHECK(pos.numel() >= B, "decode_append: position vector shorter than the batch");
+  if (slot.has_value()) {
+    check_i32(*slot, "slot");
+    TORCH_CHECK(slot->numel() >= B, "decode_append: slot vector shorter than the batch");
+  } else {
+    TORCH_CHECK(B <= kc.size(0), "decode_append: batch larger than the cache");
+  }
   TORCH_CHECK(cos_t.has_value() == sin_t.has_value(), "decode_append: pass both RoPE tables or neither");
   if (cos_t.has_value()) {
     check_f32(*cos_t, "cos");
@@ -410,7 +416,33 @@ void decode_append(Tensor& qkv, const Tensor& pos, Tensor& kc, Tensor& vc, const
   c10::cuda::CUDAGuard guard(qkv.device());
   pb::decode_append_launch(qkv.data_ptr(), qkv.stride(0), pos.data_ptr<int>(), kc.data_ptr(), vc.data_ptr(),
                            cos_t.has_value() ? cos_t->data_ptr<float>() : nullptr, sin_t.has_value() ? sin_t->data_ptr<float>() : nullptr,
-                           B, H, dh, S, stream_of(qkv));
+                           B, H, dh, S, slot.has_value() ? slot->data_ptr<int>() : nullptr, stream_of(qkv));
+  g_launches += 1;
+}
+// query rows of qkv [N, 3*H*dh] in tiles (int32 [T, 4]: slot, first_row, n_rows <= 64, first_pos) against one cache layer
+void cache_attention(const Tensor& qkv, const Tensor& kc, const Tensor& vc, const Tensor& tiles, Tensor& out, int n_heads, double scale,
+                     const c10::optional<Tensor>& alibi_slopes) {
+  check_bf16(qkv, "qkv");
+  check_bf16(kc, "k_cache");
+  check_bf16(vc, "v_cache");
+  check_bf16(out, "out");
+  check_i32(tiles, "tiles");
+  TORCH_CHECK(kc.dim() == 4 && kc.is_contiguous() && vc.sizes() == kc.sizes() && vc.is_contiguous(), "k/v cache must be contiguous [B_max, H, S_max, dh]");
+  const int Bm = int(kc.size(0)), H = int(kc.size(1)), S = int(kc.size(2)), dh = int(kc.size(3));
+  TORCH_CHECK(H == n_heads && (dh == 64 || dh == 128), "cache_attention: cache heads must equal n_heads and d_head be 64 or 128");
+  TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == 3 * H * dh && qkv.stride(1) == 1, "qkv must be [N, 3*H*dh] with unit inner stride");
+  check_aligned16(qkv, "qkv");
+  TORCH_CHECK(out.dim() == 2 && out.size(0) == qkv.size(0) && out.size(1) == H * dh && out.stride(1) == 1, "out must be [N, H*dh]");
+  check_aligned16(out, "out");
+  TORCH_CHECK(tiles.dim() == 2 && tiles.size(1) == 4, "tiles must be int32 [T, 4] (slot, first_row, n_rows, first_pos)");
+  if (alibi_slopes.has_value()) {
+    check_f32(*alibi_slopes, "alibi_slopes");
+    TORCH_CHECK(alibi_slopes->numel() == n_heads, "alibi_slopes must have n_heads elements");
+  }
+  c10::cuda::CUDAGuard guard(qkv.device());
+  pb::cache_attention_launch(qkv.data_ptr(), qkv.stride(0), qkv.size(0), kc.data_ptr(), vc.data_ptr(), tiles.data_ptr<int>(),
+                             int(tiles.size(0)), out.data_ptr(), out.stride(0), Bm, H, dh, S, float(scale),
+                             alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr, stream_of(qkv));
   g_launches += 1;
 }
 void embed_pos(const Tensor& ids, const Tensor& pos, const Tensor& wte, const c10::optional<Tensor>& wpe, Tensor& out) {
@@ -760,7 +792,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("decode_attention", &decode_attention, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("pos"), py::arg("out"),
         py::arg("n_heads"), py::arg("scale"), py::arg("alibi_slopes") = py::none());
   m.def("decode_append", &decode_append, py::arg("qkv"), py::arg("pos"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cos") = py::none(),
-        py::arg("sin") = py::none(), py::arg("n_heads") = 1);
+        py::arg("sin") = py::none(), py::arg("n_heads") = 1, py::arg("slot") = py::none());
+  m.def("cache_attention", &cache_attention, py::arg("qkv"), py::arg("k_cache"), py::arg("v_cache"), py::arg("tiles"), py::arg("out"),
+        py::arg("n_heads"), py::arg("scale"), py::arg("alibi_slopes") = py::none());
   m.def("embed_pos", &embed_pos, py::arg("ids"), py::arg("pos"), py::arg("wte"), py::arg("wpe"), py::arg("out"));
   m.def("argmax_advance", &argmax_advance, py::arg("logits"), py::arg("ids"), py::arg("pos") = py::none());
   m.def("embed_bwd", &embed_bwd);

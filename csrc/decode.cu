@@ -8,7 +8,10 @@
 //     so the result does not depend on scheduling).
 //   * decode attention: one query per (sequence, head) against the cache, split over 256-key chunks (flash-decoding); the
 //     chunk results (unnormalised o, running max, sum) are combined in chunk order.
-//   * append (RoPE at each row's own position + cache write), embedding at per-row positions, argmax + position advance.
+//   * cache attention (scoring): tiles of up to 64 consecutive query rows of one cache slot against the slot's keys on wgmma,
+//     with the causal mask at each row's own position.
+//   * append (RoPE at each row's own position + cache write into the row's slot), embedding at per-row positions, argmax +
+//     position advance.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -308,15 +311,191 @@ __global__ void __launch_bounds__(DH) decode_combine_kernel(const float* __restr
   out[b * ldo + h * DH + t] = __float2bfloat16_rn(o / L);
 }
 
+// ------------------------------------------------------------------------------------------- cache attention
+// One CTA = one (tile, head): up to 64 query rows of one cache slot, at consecutive positions, against that slot's keys.
+// Warps 0-3 (one warpgroup) own the 64 rows: S = Q K^T on wgmma (both operands in shared memory, K-major), online softmax in
+// registers (log2 domain), O += P V with P as the register A operand and V read MN-major as the cache stores it. Warp 4 is
+// the TMA producer: Q once from the fused qkv, then 128-key K / V tiles through a 2-stage ring from the cache viewed as
+// [B_max * H * S_max, dh] rows. Every row is reduced by one thread quad in a fixed order: no atomics, bitwise repeatable.
+constexpr int CA_BQ = 64, CA_BKV = 128;
+constexpr int CA_THREADS = 160;
+
+template <int DH>
+struct CaCfg {
+  static constexpr int CH = DH / 64;                // 64-column (128-byte) swizzle chunks per row
+  static constexpr int Q_BYTES = CA_BQ * 128 * CH;  // [64 x DH] bf16: CH chunks of 8 KiB
+  static constexpr int KV_BYTES = CA_BKV * 128 * CH;  // [128 x DH] bf16: CH chunks of 16 KiB
+  static constexpr int SMEM = Q_BYTES + 4 * KV_BYTES + 9 * 8 + 1024;   // Q, K[2], V[2], barriers, 1 KiB alignment slack
+  static_assert(SMEM <= 232448, "smem budget");
+};
+
+template <int DH, bool ALIBI>
+__global__ void __launch_bounds__(CA_THREADS)
+cache_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                  const int4* __restrict__ tiles, __nv_bfloat16* __restrict__ out, long long ldo, long long n_q, int H, int s_max, float sc,
+                  const float* __restrict__ slopes) {
+  using C = CaCfg<DH>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sQ = smem;
+  uint8_t* sK = sQ + C::Q_BYTES;        // [2]
+  uint8_t* sV = sK + 2 * C::KV_BYTES;   // [2]
+  uint64_t* q_full = reinterpret_cast<uint64_t*>(sV + 2 * C::KV_BYTES);
+  uint64_t* k_full = q_full + 1;        // [2]
+  uint64_t* k_empty = q_full + 3;       // [2]
+  uint64_t* v_full = q_full + 5;        // [2]
+  uint64_t* v_empty = q_full + 7;       // [2]
+
+  const int4 tile = tiles[blockIdx.x];  // (slot, first_row, n_rows, first_pos)
+  const int h = blockIdx.y;
+  const int n_kv = (tile.w + tile.z - 1) / CA_BKV + 1;   // key tiles up to the last row's position
+  if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(&k_full[s], 1);
+      mbar_init(&k_empty[s], 4);   // one arrival per MMA warp
+      mbar_init(&v_full[s], 1);
+      mbar_init(&v_empty[s], 4);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (threadIdx.x >= 128) {
+    // ------------------------------------------------------------ TMA producer (one thread)
+    if (threadIdx.x == 128) {
+      prefetch_tmap(&tmQ);
+      prefetch_tmap(&tmK);
+      prefetch_tmap(&tmV);
+      const int kv_row0 = (tile.x * H + h) * s_max;
+      mbar_expect_tx(q_full, C::Q_BYTES);   // rows past the last qkv row arrive as zeros
+#pragma unroll
+      for (int c = 0; c < C::CH; ++c) tma_load_2d(sQ + c * 8192, &tmQ, q_full, h * DH + c * 64, tile.y);
+      for (int j = 0; j < n_kv; ++j) {
+        const int st = j & 1;
+        const uint32_t ph = ((j >> 1) & 1) ^ 1;
+        mbar_wait(&k_empty[st], ph);
+        mbar_expect_tx(&k_full[st], C::KV_BYTES);
+#pragma unroll
+        for (int c = 0; c < C::CH; ++c) tma_load_2d(sK + st * C::KV_BYTES + c * 16384, &tmK, &k_full[st], c * 64, kv_row0 + j * CA_BKV);
+        mbar_wait(&v_empty[st], ph);
+        mbar_expect_tx(&v_full[st], C::KV_BYTES);
+#pragma unroll
+        for (int c = 0; c < C::CH; ++c) tma_load_2d(sV + st * C::KV_BYTES + c * 16384, &tmV, &v_full[st], c * 64, kv_row0 + j * CA_BKV);
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------- MMA warpgroup: 64 query rows x 128 keys per step
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int t4 = lane & 3;
+  const int r0 = warp * 16 + (lane >> 2);   // this thread's tile rows r0, r0 + 8 (accumulator layout of m64nN)
+  const float slope2 = ALIBI ? slopes[h] * LOG2E : 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float o[DH / 2];
+#pragma unroll
+  for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
+  float s[64];
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < n_kv; ++j) {
+    const int st = j & 1;
+    const uint32_t ph = (j >> 1) & 1;
+    mbar_wait(&k_full[st], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < DH / 16; ++kk) {
+      const int c = kk >> 2, off = (kk & 3) * 32;
+      wgmma_bf16_ss_n128<0, 0>(s, desc_add(desc_sw128(sQ + c * 8192, 16), off),
+                               desc_add(desc_sw128(sK + st * C::KV_BYTES + c * 16384, 16), off), kk > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&k_empty[st]);
+    // row r (position first_pos + r) sees keys 0 .. first_pos + r; key 0 is always visible, so m is finite after tile 0
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int j8 = 0; j8 < 16; ++j8) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int hh = e >> 1;
+        const int key = j * CA_BKV + 8 * j8 + 2 * t4 + (e & 1);
+        const int qpos = tile.w + r0 + 8 * hh;
+        float x = s[4 * j8 + e] * sc;
+        if (ALIBI) x = fmaf(slope2, float(key - qpos), x);
+        if (key > qpos) x = -INFINITY;
+        s[4 * j8 + e] = x;
+        mx[hh] = fmaxf(mx[hh], x);
+      }
+    }
+    float alpha[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffff, mx[hh], 1));
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffff, mx[hh], 2));
+      const float m_new = fmaxf(m[hh], mx[hh]);
+      alpha[hh] = exp2f(m[hh] - m_new);
+      m[hh] = m_new;
+      l[hh] *= alpha[hh];
+    }
+    // P in bf16 as the A fragments of the 8 k-steps of P V (accumulator columns 16k .. 16k+15 = k-step k)
+    uint32_t pa[8][4];
+#pragma unroll
+    for (int kc = 0; kc < 8; ++kc) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const float p0 = exp2f(s[8 * kc + 2 * q] - m[q & 1]);
+        const float p1 = exp2f(s[8 * kc + 2 * q + 1] - m[q & 1]);
+        l[q & 1] += p0 + p1;
+        pa[kc][q] = pack_bf16(p0, p1);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < DH / 8; ++i) {
+      o[4 * i] *= alpha[0], o[4 * i + 1] *= alpha[0];
+      o[4 * i + 2] *= alpha[1], o[4 * i + 3] *= alpha[1];
+    }
+    mbar_wait(&v_full[st], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int kc = 0; kc < 8; ++kc) {
+      const uint64_t vd = desc_add(desc_sw128(sV + st * C::KV_BYTES, 16384), kc * 2048);
+      if constexpr (DH == 64) wgmma_bf16_rs_n64<1>(o, pa[kc], vd, 1u);
+      else wgmma_bf16_rs_n128<1>(o, pa[kc], vd, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&v_empty[st]);
+  }
+  // only the rows of the tile are written
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int r = r0 + 8 * hh;
+    l[hh] += __shfl_xor_sync(0xffffffff, l[hh], 1);
+    l[hh] += __shfl_xor_sync(0xffffffff, l[hh], 2);
+    if (r >= tile.z || tile.y + r >= n_q) continue;
+    const float inv_l = 1.0f / l[hh];
+    __nv_bfloat16* orow = out + (long long)(tile.y + r) * ldo + h * DH;
+#pragma unroll
+    for (int i = 0; i < DH / 8; ++i)
+      *reinterpret_cast<uint32_t*>(orow + 8 * i + 2 * t4) = pack_bf16(o[4 * i + 2 * hh] * inv_l, o[4 * i + 2 * hh + 1] * inv_l);
+  }
+}
+
 // ------------------------------------------------------------------------------------------- append / embed / argmax
 __global__ void __launch_bounds__(128) decode_append_kernel(__nv_bfloat16* __restrict__ qkv, long long ld, const int* __restrict__ pos,
-                                                            __nv_bfloat16* __restrict__ kc, __nv_bfloat16* __restrict__ vc,
-                                                            const float* __restrict__ cosT, const float* __restrict__ sinT, int H,
-                                                            int dh, int s_max) {
+                                                            const int* __restrict__ slot, __nv_bfloat16* __restrict__ kc,
+                                                            __nv_bfloat16* __restrict__ vc, const float* __restrict__ cosT,
+                                                            const float* __restrict__ sinT, int H, int dh, int s_max) {
   const int b = blockIdx.x, p = pos[b];
+  const int sb = slot ? slot[b] : b;   // the cache slot this row writes
   const int d = H * dh, half = dh / 2, groups = half / 8, vec = dh / 8;
   __nv_bfloat16* row = qkv + b * ld;
-  const long long cache_row = ((long long)b * H) * s_max + p;   // + h * s_max: row of head h
+  const long long cache_row = ((long long)sb * H) * s_max + p;   // + h * s_max: row of head h
   if (cosT != nullptr) {
     // rotate-half RoPE at position p, the arithmetic of rope_kernel: q in place, k straight into the cache
     for (int i = threadIdx.x; i < 2 * H * groups; i += blockDim.x) {
@@ -478,12 +657,45 @@ void decode_attention_launch(const void* q, long long ldq, const void* kc, const
 }
 
 void decode_append_launch(void* qkv, long long ldqkv, const int* pos, void* kc, void* vc, const float* cosT, const float* sinT, int B,
-                          int H, int dh, int s_max, cudaStream_t st) {
+                          int H, int dh, int s_max, const int* slot, cudaStream_t st) {
   if (B < 1) return;
   if (dh % 16) throw std::runtime_error("photon_b200 decode append: d_head must be a multiple of 16");
-  decode_append_kernel<<<B, 128, 0, st>>>((__nv_bfloat16*)qkv, ldqkv, pos, (__nv_bfloat16*)kc, (__nv_bfloat16*)vc, cosT, sinT, H, dh,
-                                          s_max);
+  decode_append_kernel<<<B, 128, 0, st>>>((__nv_bfloat16*)qkv, ldqkv, pos, slot, (__nv_bfloat16*)kc, (__nv_bfloat16*)vc, cosT, sinT, H,
+                                          dh, s_max);
   PB_DECODE_CHECK("decode append");
+}
+
+void cache_attention_launch(const void* qkv, long long ldq, long long n_q, const void* kc, const void* vc, const int* tiles, int n_tiles,
+                            void* out, long long ldo, int B_max, int H, int dh, int s_max, float scale, const float* alibi_slopes,
+                            cudaStream_t st) {
+  if (n_tiles < 1 || n_q < 1) return;
+  const long long kv_rows = (long long)B_max * H * s_max;
+  if (kv_rows >= (1LL << 31)) throw std::runtime_error("photon_b200 cache attention: the cache has more than 2^31 rows per layer");
+  const CUtensorMap tq = make_tmap_2d(qkv, 2, false, uint64_t(3) * H * dh, uint64_t(n_q), uint64_t(ldq) * 2, 64, CA_BQ);
+  const CUtensorMap tk = make_tmap_2d(kc, 2, false, dh, kv_rows, uint64_t(dh) * 2, 64, CA_BKV);
+  const CUtensorMap tv = make_tmap_2d(vc, 2, false, dh, kv_rows, uint64_t(dh) * 2, 64, CA_BKV);
+  const dim3 grid(n_tiles, H);
+  const auto* tt = reinterpret_cast<const int4*>(tiles);
+  const float sc = scale * LOG2E;
+#define PB_CA(D, A)                                                                                                              \
+  {                                                                                                                              \
+    auto kern = cache_attn_kernel<D, A>;                                                                                         \
+    static bool configured = false;                                                                                              \
+    if (!configured) {                                                                                                           \
+      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, CaCfg<D>::SMEM);                   \
+      if (e != cudaSuccess) throw std::runtime_error(std::string("cache attention smem attr: ") + cudaGetErrorString(e));       \
+      configured = true;                                                                                                         \
+    }                                                                                                                            \
+    kern<<<grid, CA_THREADS, CaCfg<D>::SMEM, st>>>(tq, tk, tv, tt, (__nv_bfloat16*)out, ldo, n_q, H, s_max, sc, alibi_slopes);  \
+    PB_DECODE_CHECK("cache attention");                                                                                          \
+    return;                                                                                                                      \
+  }
+  if (dh == 64 && !alibi_slopes) PB_CA(64, false)
+  if (dh == 64) PB_CA(64, true)
+  if (dh == 128 && !alibi_slopes) PB_CA(128, false)
+  if (dh == 128) PB_CA(128, true)
+#undef PB_CA
+  throw std::runtime_error("photon_b200 cache attention: d_head must be 64 or 128");
 }
 
 void embed_pos_launch(const int* ids, const int* pos, const void* wte, const void* wpe, void* out, int B, int d, int V, cudaStream_t st) {

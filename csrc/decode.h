@@ -47,9 +47,19 @@ void decode_attention_launch(const void* q, long long ldq, const void* kc, const
                              cudaStream_t st);
 
 // For each row b of the fused qkv [B, 3*H*dh]: rotate q and k (rotate-half tables cos / sin [>= s_max, dh/2], nullptr = no RoPE)
-// at position pos[b] (q in place), and write k, v into the cache at position pos[b].
+// at position pos[b] (q in place), and write k, v into the cache at position pos[b] of slot slot[b] (slot == nullptr: slot b).
 void decode_append_launch(void* qkv, long long ldqkv, const int* pos, void* kc, void* vc, const float* cosT, const float* sinT, int B,
-                          int H, int dh, int s_max, cudaStream_t st);
+                          int H, int dh, int s_max, const int* slot, cudaStream_t st);
+
+// Several query rows per cache slot (log-likelihood scoring). tiles: int32 [n_tiles, 4] on the device, each
+// (slot, first_row, n_rows <= 64, first_pos): query rows first_row .. first_row + n_rows - 1 of qkv [n_q, 3*H*dh] (q third, after
+// RoPE) sit at positions first_pos + i of that slot, and row i attends to keys 0 .. first_pos + i of the slot:
+//   out[first_row + i, h*dh:(h+1)*dh] = softmax(q k^T * scale + alibi) v.
+// Rows outside every tile are not written. The keys of all tile rows must already be in the cache (decode_append first).
+// qkv and out rows must be 16-byte aligned (TMA); d_head 64 or 128.
+void cache_attention_launch(const void* qkv, long long ldq, long long n_q, const void* kc, const void* vc, const int* tiles, int n_tiles,
+                            void* out, long long ldo, int B_max, int H, int dh, int s_max, float scale, const float* alibi_slopes,
+                            cudaStream_t st);
 
 // h[b,:] = wte[ids[b],:] + wpe[pos[b],:] (wpe may be nullptr)
 void embed_pos_launch(const int* ids, const int* pos, const void* wte, const void* wpe, void* out, int B, int d, int V, cudaStream_t st);

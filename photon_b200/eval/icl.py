@@ -16,6 +16,12 @@ self-contained implementation of the two task types that dominate those tables:
   ``batch_size``; rows whose prompt plus ``max_new_tokens`` exceeds the decoder's cache, and every row when there is no
   decoder, recompute the last ``max_seq_len`` tokens with ``logits_fn`` for every new token (a sliding window, batch of one).
 
+The scoring tasks (the first two kinds and ``schema``) decide each row on the log-likelihood of (context, continuation) pairs,
+left-truncated to ``max_seq_len``. When the ``decoder`` also has ``score(pairs)`` (:meth:`KVDecoder.score`), the pairs go to it
+in batches of whole rows (at most the task's ``batch_size`` rows and ``decoder.max_batch`` pairs): each distinct context is
+prefilled once and shared by its choices. Rows with more pairs than ``max_batch``, pairs with nothing to score, and every
+pair when there is no such decoder, run ``logits_fn`` on one pair at a time.
+
 Datasets are jsonl files resolved against ``icl_tasks_config.root_dir`` (there is no network, so missing files yield
 ``skipped``).
 """
@@ -103,17 +109,69 @@ class ICLEvaluator:
             parts.append(f"{t['question_prelimiter']}{r.get('context', r.get('query', ''))}{t['continuation_delimiter']}{cont}")
         return t["prompt_string"] + t["example_delimiter"].join(parts) + (t["example_delimiter"] if parts else "")
 
-    @torch.no_grad()
-    def _continuation_stats(self, ctx: list[int], cont: list[int]) -> tuple[float, bool]:
-        """(sum log p(cont | ctx), greedy-exact-match) with left truncation to ``max_seq_len``."""
+    def _truncate(self, ctx: list[int], cont: list[int]) -> tuple[list[int], list[int]]:
+        """The (context, scored tokens) of a pair after left truncation: ``ctx + cont`` keeps its last ``max_seq_len`` tokens,
+        of which the last ``min(len(cont), kept - 1)`` are scored (at least one context token stays)."""
         ids = (ctx + cont)[-self.max_seq_len:]
         n = min(len(cont), len(ids) - 1)
+        return ids[: len(ids) - n], ids[len(ids) - n:]
+
+    @torch.no_grad()
+    def _continuation_stats(self, ctx: list[int], cont: list[int]) -> tuple[float, bool]:
+        """(sum log p(cont | ctx), greedy-exact-match) with left truncation to ``max_seq_len`` (see ``_truncate``)."""
+        head, tail = self._truncate(ctx, cont)
+        ids, n = head + tail, len(tail)
         x = torch.tensor([ids], dtype=torch.long)
         logp = torch.log_softmax(self.logits_fn(x)[0].float(), dim=-1)
         pos = torch.arange(len(ids) - n - 1, len(ids) - 1)
-        tgt = torch.tensor(ids[-n:])
+        tgt = torch.tensor(tail, dtype=torch.long)
         lp = logp[pos].cpu()
         return float(lp[torch.arange(n), tgt].sum()), bool((lp.argmax(-1) == tgt).all())
+
+    def _question_pairs(self, kind: str, prefix: str, r: dict[str, Any], t: dict[str, Any]) -> list[tuple[list[int], list[int]]]:
+        """The (context, continuation) token pairs one row of a scoring task is decided on, in choice order."""
+        if kind == "language_modeling":
+            ctx = self._enc(prefix + t["question_prelimiter"] + r["context"] + t["continuation_delimiter"].rstrip())
+            return [(ctx, self._enc(" " + r["continuation"].lstrip()))]
+        if kind == "multiple_choice":
+            ctx = self._enc(prefix + t["question_prelimiter"] + r["query"] + t["continuation_delimiter"].rstrip())
+            return [(ctx, self._enc(" " + ch.lstrip())) for ch in r["choices"]]
+        cont = self._enc(" " + r["continuation"].lstrip())   # schema: the context options vary, the continuation is shared
+        return [(self._enc(prefix + opt), cont) for opt in r["context_options"]]
+
+    @torch.no_grad()
+    def _score_questions(self, questions: list[list[tuple[list[int], list[int]]]], batch_size: int) -> list[list[tuple[float, bool]]]:
+        """``_continuation_stats`` of every pair of every question. With a decoder that has ``score``, the truncated pairs go to
+        it in batches of whole questions: at most ``batch_size`` questions and ``decoder.max_batch`` pairs per call. A question
+        with more pairs than that, and a pair with nothing to score or that does not fit the decoder's cache, take
+        ``logits_fn`` one pair at a time."""
+        out: list[list[tuple[float, bool] | None]] = [[None] * len(q) for q in questions]
+        dec = self.decoder
+        if dec is not None and callable(getattr(dec, "score", None)):
+            cap, per = int(dec.max_batch), max(1, int(batch_size))
+            batch: list[tuple[int, int, list[int], list[int]]] = []   # (question, pair, context, scored)
+            n_q = 0
+
+            def flush() -> None:
+                for (qi, pi, _, _), st in zip(batch, dec.score([(c, s) for _, _, c, s in batch])):
+                    out[qi][pi] = st
+
+            for qi, q in enumerate(questions):
+                if len(q) > cap:
+                    continue
+                items = [(qi, pi, *self._truncate(ctx, cont)) for pi, (ctx, cont) in enumerate(q)]
+                items = [it for it in items if it[2] and it[3] and len(it[2]) + len(it[3]) <= dec.max_seq_len]
+                if not items:
+                    continue
+                if batch and (n_q == per or len(batch) + len(items) > cap):
+                    flush()
+                    batch, n_q = [], 0
+                batch += items
+                n_q += 1
+            if batch:
+                flush()
+        return [[st if st is not None else self._continuation_stats(ctx, cont) for st, (ctx, cont) in zip(row, q)]
+                for row, q in zip(out, questions)]
 
     @torch.no_grad()
     def _generate(self, ctx: list[int], max_new_tokens: int, stops: list[str]) -> str:
@@ -175,12 +233,15 @@ class ICLEvaluator:
         for k in t["num_fewshot"]:
             correct = 0
             texts: list[str] = []
+            stats: list[list[tuple[float, bool]]] = []
             if kind == "generation_task_with_answers":
                 ctxs = [self._enc(self._fewshot_prefix(rows, i, k, t) + t["question_prelimiter"] + r["context"]
                                   + t["continuation_delimiter"].rstrip()) for i, r in enumerate(rows)]
                 texts = self._generate_rows(ctxs, int(t["max_new_tokens"]), list(t["early_stopping_criteria"] or []), int(t["batch_size"]))
+            else:
+                questions = [self._question_pairs(kind, self._fewshot_prefix(rows, i, k, t), r, t) for i, r in enumerate(rows)]
+                stats = self._score_questions(questions, int(t["batch_size"]))
             for i, r in enumerate(rows):
-                prefix = self._fewshot_prefix(rows, i, k, t)
                 if kind == "generation_task_with_answers":
                     text = texts[i]
                     if t["cot_delimiter"] and t["cot_delimiter"] in text:
@@ -189,20 +250,9 @@ class ICLEvaluator:
                     norm = _normalize_answer if t["do_normalization"] else (lambda x: x.strip())
                     correct += int(any(norm(text).startswith(norm(g)) for g in golds if norm(g)))
                 elif kind == "language_modeling":
-                    ctx = self._enc(prefix + t["question_prelimiter"] + r["context"] + t["continuation_delimiter"].rstrip())
-                    _, em = self._continuation_stats(ctx, self._enc(" " + r["continuation"].lstrip()))
-                    correct += int(em)
-                else:
-                    scores = []
-                    if kind == "multiple_choice":
-                        ctx = self._enc(prefix + t["question_prelimiter"] + r["query"] + t["continuation_delimiter"].rstrip())
-                        for ch in r["choices"]:
-                            cont = self._enc(" " + ch.lstrip())
-                            scores.append(self._continuation_stats(ctx, cont)[0] / max(1, len(cont)))
-                    else:  # schema: the context options vary, the continuation is shared
-                        cont = self._enc(" " + r["continuation"].lstrip())
-                        for opt in r["context_options"]:
-                            scores.append(self._continuation_stats(self._enc(prefix + opt), cont)[0] / max(1, len(cont)))
+                    correct += int(stats[i][0][1])
+                else:   # multiple_choice / schema: the highest length-normalised log-likelihood
+                    scores = [lp / max(1, len(cont)) for (lp, _), (_, cont) in zip(stats[i], questions[i])]
                     correct += int(int(torch.tensor(scores).argmax()) == int(r["gold"]))
             out[f"{t['label']}/{k}-shot/accuracy"] = correct / max(1, len(rows))
             out[f"{t['label']}/{k}-shot/n_samples"] = float(len(rows))

@@ -100,7 +100,8 @@ def main() -> None:
         mcfg.attn_impl = "torch"
     decoder = None
     if dev.type == "cuda":
-        # the engine scores with the same torch-module forward (``engine.logits``) and generates with its KV-cached decoder
+        # the engine scores and generates with its KV-cached decoder; ``engine.logits`` (the torch-module forward) serves the
+        # pairs the decoder does not take
         from photon_b200.models.engine import B200Engine
 
         engine = B200Engine(mcfg, device=dev, seed=17)

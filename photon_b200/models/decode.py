@@ -15,6 +15,11 @@ buffers, and the host reads back one int32 per sequence. The GEMMs of a step use
 Cache layout: bf16 ``[L, 2, B, H, max_seq_len, d_head]`` (k = index 0, v = 1), see ``csrc/decode.h``. It is allocated for the
 largest batch the decoder has been asked to run (at most ``max_batch``). The weights are the engine's bf16 compute shadow,
 also under ``amp_fp8``; the decoder never touches the training workspace or its captured graphs.
+
+The same cache serves log-likelihood scoring (:meth:`KVDecoder.score`, the multiple-choice, schema and language-modelling ICL
+tasks): each distinct context is prefilled once and its k / v copied into one slot per (context, continuation) pair; the
+continuation tokens of every pair then run through the blocks together, several rows per slot, with cache attention (a
+wgmma kernel over the slot's keys, causal at each row's own position) in place of decode attention.
 """
 from __future__ import annotations
 
@@ -53,19 +58,26 @@ class KVDecoder:
         if b <= self._cap:
             return
         c, dev = self.cfg, self.dev
-        bf = lambda *s: torch.empty(*s, dtype=torch.bfloat16, device=dev)  # noqa: E731
-        f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
         self._graphs.clear()   # graphs point into the old buffers
         self.cache = None
         self.cache = torch.zeros(c.n_layers, 2, b, c.n_heads, self.max_seq_len, c.d_head, dtype=torch.bfloat16, device=dev)
-        d, dff = c.d_model, c.expansion_ratio * c.d_model
         self.tok = torch.zeros(b, dtype=torch.int32, device=dev)
         self.pos = torch.zeros(b, dtype=torch.int32, device=dev)
-        self.buf = {"h": bf(b, d), "ln": bf(b, d), "m": f32(b), "r": f32(b), "qkv": bf(b, 3 * d), "attn": bf(b, d), "hmid": bf(b, d),
-                    "u": bf(b, dff), "z": bf(b, dff), "logits": bf(b, c.vocab_size)}
-        if c.qk_ln:
-            self.buf.update(qk_pre=bf(b, d), qk_tmp=bf(b, d))
+        self.buf = self._row_buffers(b)
+        self.buf["logits"] = torch.empty(b, c.vocab_size, dtype=torch.bfloat16, device=dev)
         self._cap = b
+
+    def _row_buffers(self, n: int, h: torch.Tensor | None = None) -> dict[str, torch.Tensor]:
+        """Activations of ``n`` rows through the blocks (``h``: the residual stream, allocated when None)."""
+        c, dev = self.cfg, self.dev
+        bf = lambda *s: torch.empty(*s, dtype=torch.bfloat16, device=dev)  # noqa: E731
+        f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
+        d, dff = c.d_model, c.expansion_ratio * c.d_model
+        x = {"h": bf(n, d) if h is None else h, "ln": bf(n, d), "m": f32(n), "r": f32(n), "qkv": bf(n, 3 * d), "attn": bf(n, d),
+             "hmid": bf(n, d), "u": bf(n, dff), "z": bf(n, dff)}
+        if c.qk_ln:
+            x.update(qk_pre=bf(n, d), qk_tmp=bf(n, d))
+        return x
 
     @property
     def logits(self) -> torch.Tensor:
@@ -95,25 +107,19 @@ class KVDecoder:
                 qkv3[:, j].copy_(tmp)
 
     # ------------------------------------------------------------------ prefill
-    @torch.no_grad()
-    def start(self, prompts: list[list[int]], max_new_tokens: int) -> list[int]:
-        """Prefill ``prompts`` (a batch of token lists) and return the first greedy token of each."""
+    def _prefill(self, prompts: list[list[int]], slots: list[int]) -> torch.Tensor:
+        """Run ``prompts`` (right-padded to a multiple of 128) through the blocks on the training kernels, writing every layer's
+        k / v of prompt ``i`` into cache slot ``slots[i]``; returns the hidden state of each prompt's last token ``[len, d]``."""
         c, e = self.cfg, self.e
         b = len(prompts)
-        if not 1 <= b <= self.max_batch:
-            raise ValueError(f"batch of {b} prompts; this decoder runs 1..{self.max_batch}")
         lens = [len(p) for p in prompts]
-        for n in lens:
-            if n < 1 or n + int(max_new_tokens) > self.max_seq_len:
-                raise ValueError(f"a prompt of {n} tokens plus {max_new_tokens} new tokens does not fit the {self.max_seq_len}-position cache")
-        self._ensure_capacity(b)
-        self._b = b
         S = -(-max(lens) // 128) * 128
         d, H, dh, T = c.d_model, c.n_heads, c.d_head, b * S
         ids = torch.zeros(b, S, dtype=torch.long)
         for i, p in enumerate(prompts):
             ids[i, : len(p)] = torch.tensor(p, dtype=torch.long)
         ids = ids.to(self.dev, non_blocking=True)
+        dst = torch.tensor(slots, dtype=torch.long).to(self.dev, non_blocking=True)
         bf = lambda *s: torch.empty(*s, dtype=torch.bfloat16, device=self.dev)  # noqa: E731
         f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=self.dev)  # noqa: E731
         h, hmid, ln, qkv, attn = bf(T, d), bf(T, d), bf(T, d), bf(T, 3 * d), bf(T, d)
@@ -129,16 +135,31 @@ class KVDecoder:
                 ops.rope_(qkv.view(b, S, 3 * d), e.rope[0], e.rope[1], H)
             ops.attention_fwd(qkv.view(b, S, 3 * d), attn.view(b, S, d), lse, H, self.scale, True, e.alibi)
             kv = qkv.view(b, S, 3, H, dh)
-            self.cache[i, 0, :b, :, :S].copy_(kv[:, :, 1].transpose(1, 2))   # k / v after clip, qk_ln and RoPE
-            self.cache[i, 1, :b, :, :S].copy_(kv[:, :, 2].transpose(1, 2))
+            self.cache[i, 0, :, :, :S].index_copy_(0, dst, kv[:, :, 1].transpose(1, 2))   # k / v after clip, qk_ln and RoPE
+            self.cache[i, 1, :, :, :S].index_copy_(0, dst, kv[:, :, 2].transpose(1, 2))
             ops.linear_fwd(attn, w.wo, w.bo, hmid, residual=h)
             ops.layernorm_fwd(hmid, w.g2, w.b2, ln, m, r, c.norm_eps)
             ops.linear_gelu_fwd(ln, w.wup, w.bup, z, u)
             ops.linear_fwd(u, w.wdown, w.bdown, h, residual=hmid)
-        # only the last prompt row of every sequence goes through the final LN and the LM head
         last = torch.tensor([i * S + n - 1 for i, n in enumerate(lens)], dtype=torch.long).to(self.dev, non_blocking=True)
+        return torch.index_select(h, 0, last)
+
+    @torch.no_grad()
+    def start(self, prompts: list[list[int]], max_new_tokens: int) -> list[int]:
+        """Prefill ``prompts`` (a batch of token lists) and return the first greedy token of each."""
+        c, e = self.cfg, self.e
+        b = len(prompts)
+        if not 1 <= b <= self.max_batch:
+            raise ValueError(f"batch of {b} prompts; this decoder runs 1..{self.max_batch}")
+        lens = [len(p) for p in prompts]
+        for n in lens:
+            if n < 1 or n + int(max_new_tokens) > self.max_seq_len:
+                raise ValueError(f"a prompt of {n} tokens plus {max_new_tokens} new tokens does not fit the {self.max_seq_len}-position cache")
+        self._ensure_capacity(b)
+        self._b = b
         B = self.buf
-        torch.index_select(h, 0, last, out=B["h"][:b])
+        # only the last prompt row of every sequence goes through the final LN and the LM head
+        B["h"][:b].copy_(self._prefill(prompts, list(range(b))))
         ops.layernorm_fwd(B["h"][:b], e.gf, e.bf, B["ln"][:b], B["m"][:b], B["r"][:b], c.norm_eps)
         self._linear(B["ln"][:b], e.wte16, None, B["logits"][:b])
         self.pos[:b].copy_(torch.tensor(lens, dtype=torch.int32), non_blocking=True)
@@ -146,25 +167,38 @@ class KVDecoder:
         self._pos_host = list(lens)
         return self.tok[:b].tolist()
 
-    # --------------------------------------------------------------------- step
-    def _step_kernels(self, b: int) -> None:
-        c, e, B = self.cfg, self.e, self.buf
-        h, ln, m, r, qkv, attn, hmid, u, z = (B[k][:b] for k in ("h", "ln", "m", "r", "qkv", "attn", "hmid", "u", "z"))
-        pre, tmp = (B["qk_pre"][:b], B["qk_tmp"][:b]) if c.qk_ln else (None, None)
-        ops.embed_pos(self.tok, self.pos, e.wte16, e.wpe16, h)
+    # --------------------------------------------------------------------- blocks over cached rows
+    def _blocks(self, x: dict[str, torch.Tensor], pos: torch.Tensor, slot: torch.Tensor | None = None,
+                tiles: torch.Tensor | None = None) -> None:
+        """Every block over the rows of ``x`` (see ``_row_buffers``; ``h`` holds the embedded rows on entry and the last block's
+        output on return). Row ``r`` sits at position ``pos[r]`` of cache slot ``slot[r]`` (slot ``r`` when None) and appends its
+        k / v there. Attention is decode attention (one row per slot) or, given a ``tiles`` table, cache attention over
+        several rows per slot."""
+        c, e = self.cfg, self.e
+        h, ln, m, r, qkv, attn, hmid, u, z = (x[k] for k in ("h", "ln", "m", "r", "qkv", "attn", "hmid", "u", "z"))
         for i, w in enumerate(e.layers):
             kc, vc = self.cache[i, 0], self.cache[i, 1]
             ops.layernorm_fwd(h, w.g1, w.b1, ln, m, r, c.norm_eps)
             self._linear(ln, w.wqkv, w.bqkv, qkv)
-            self._qkv_post(w, qkv, pre, tmp, m, r)
-            ops.decode_append(qkv, self.pos, kc, vc, e.rope, c.n_heads)
-            ops.decode_attention(qkv, kc, vc, self.pos, attn, c.n_heads, self.scale, e.alibi)
+            self._qkv_post(w, qkv, x.get("qk_pre"), x.get("qk_tmp"), m, r)
+            ops.decode_append(qkv, pos, kc, vc, e.rope, c.n_heads, slot)
+            if tiles is None:
+                ops.decode_attention(qkv, kc, vc, pos, attn, c.n_heads, self.scale, e.alibi)
+            else:
+                ops.cache_attention(qkv, kc, vc, tiles, attn, c.n_heads, self.scale, e.alibi)
             self._linear(attn, w.wo, w.bo, hmid, residual=h)
             ops.layernorm_fwd(hmid, w.g2, w.b2, ln, m, r, c.norm_eps)
             self._linear(ln, w.wup, w.bup, u, gelu=True, pre=z)
             self._linear(u, w.wdown, w.bdown, h, residual=hmid)
-        ops.layernorm_fwd(h, e.gf, e.bf, ln, m, r, c.norm_eps)
-        self._linear(ln, e.wte16, None, B["logits"][:b])
+
+    # --------------------------------------------------------------------- step
+    def _step_kernels(self, b: int) -> None:
+        c, e, B = self.cfg, self.e, self.buf
+        x = {k: v[:b] for k, v in B.items() if k != "logits"}
+        ops.embed_pos(self.tok, self.pos, e.wte16, e.wpe16, x["h"])
+        self._blocks(x, self.pos)
+        ops.layernorm_fwd(x["h"], e.gf, e.bf, x["ln"], x["m"], x["r"], c.norm_eps)
+        self._linear(x["ln"], e.wte16, None, B["logits"][:b])
         ops.argmax_advance(B["logits"][:b], self.tok, self.pos)
 
     @torch.no_grad()
@@ -187,6 +221,86 @@ class KVDecoder:
             self._graphs[b] = g
         self._pos_host = [p + 1 for p in self._pos_host]
         return self.tok[:b].tolist()
+
+    # ------------------------------------------------------------------ scoring
+    @torch.no_grad()
+    def score(self, pairs: list[tuple[list[int], list[int]]]) -> list[tuple[float, bool]]:
+        """Log-likelihood of each pair's scored tokens after its context: ``[(sum log p(scored | context), every scored token is
+        the argmax)]``. Pairs that share a context share one prefill; each pair holds one cache slot, so a call takes at most
+        ``max_batch`` pairs. Contexts and scored tokens are taken as given (no truncation). Eager: shapes change every call.
+
+        Steps: (1) prefill every distinct context once, into the slot of its first pair; (2) the last context row's logits
+        score ``scored[0]`` of every pair of the group; (3) the context k / v is copied into the slot of every other pair of
+        the group; (4) ``scored[:-1]`` of every pair run through the blocks at positions ``P ..`` of its slot (cache attention);
+        (5) final LN + LM head over all those rows, log p and the argmax match of each scored token on the device, one copy to
+        the host, and each pair's tokens summed in order there."""
+        c, e = self.cfg, self.e
+        if not 1 <= len(pairs) <= self.max_batch:
+            raise ValueError(f"{len(pairs)} pairs; this decoder scores 1..{self.max_batch} at a time")
+        for ctx, sc in pairs:
+            if not ctx or not sc:
+                raise ValueError("every scored pair needs a non-empty context and at least one scored token")
+            if len(ctx) + len(sc) > self.max_seq_len:
+                raise ValueError(f"a context of {len(ctx)} plus {len(sc)} scored tokens does not fit the {self.max_seq_len}-position cache")
+        self._ensure_capacity(len(pairs))
+        self._b = 0   # the slots are overwritten: a generation started before cannot step on
+        groups: dict[tuple[int, ...], list[int]] = {}
+        for i, (ctx, _) in enumerate(pairs):
+            groups.setdefault(tuple(ctx), []).append(i)
+        members = list(groups.values())
+        G = len(members)
+        last = self._prefill([pairs[g[0]][0] for g in members], [g[0] for g in members])
+        for g in members:
+            P = len(pairs[g[0]][0])
+            for i in g[1:]:
+                self.cache[:, :, i, :, :P].copy_(self.cache[:, :, g[0], :, :P])
+        # extend rows: scored[:-1] of every pair at positions P .. P + n - 2 of its slot (the last scored token is no input)
+        toks: list[int] = []
+        pos: list[int] = []
+        runs: list[tuple[int, int, int, int]] = []
+        first = [0] * len(pairs)
+        for i, (ctx, sc) in enumerate(pairs):
+            first[i] = G + len(toks)
+            if len(sc) > 1:
+                runs.append((i, len(toks), len(sc) - 1, len(ctx)))
+                toks += sc[:-1]
+                pos += range(len(ctx), len(ctx) + len(sc) - 1)
+        R = G + len(toks)
+        hid = torch.empty(R, c.d_model, dtype=torch.bfloat16, device=self.dev)
+        hid[:G].copy_(last)
+        if toks:
+            x = self._row_buffers(len(toks), h=hid[G:])
+            i32 = lambda v: torch.tensor(v, dtype=torch.int32).to(self.dev, non_blocking=True)  # noqa: E731
+            pos_t = i32(pos)
+            ops.embed_pos(i32(toks), pos_t, e.wte16, e.wpe16, x["h"])
+            self._blocks(x, pos_t, i32([s for s, _, n, _ in runs for _ in range(n)]), ops.cache_tiles(runs, self.dev))
+        ln = torch.empty_like(hid)
+        m, r = (torch.empty(R, dtype=torch.float32, device=self.dev) for _ in range(2))
+        ops.layernorm_fwd(hid, e.gf, e.bf, ln, m, r, c.norm_eps)
+        logits = torch.empty(R, c.vocab_size, dtype=torch.bfloat16, device=self.dev)
+        self._linear(ln, e.wte16, None, logits)
+        # scored token k of pair i is predicted by its group's last context row (k = 0) or by extend row first[i] + k - 1
+        group = {i: gi for gi, g in enumerate(members) for i in g}
+        rows = [group[i] if k == 0 else first[i] + k - 1 for i, (_, sc) in enumerate(pairs) for k in range(len(sc))]
+        tgts = [t for _, sc in pairs for t in sc]
+        lse = torch.empty(R, dtype=torch.float32, device=self.dev)
+        stats = torch.zeros(4, dtype=torch.float64, device=self.dev)
+        ops.cross_entropy(logits, torch.full((R,), -1, dtype=torch.long, device=self.dev), 0.0, False, stats, row_lse=lse)
+        top = torch.empty(R, dtype=torch.int32, device=self.dev)
+        ops.argmax_advance(logits, top)
+        row_t = torch.tensor(rows, dtype=torch.long).to(self.dev, non_blocking=True)
+        tgt_t = torch.tensor(tgts, dtype=torch.long).to(self.dev, non_blocking=True)
+        logp = logits[row_t, tgt_t].float() - lse[row_t]
+        host = torch.stack([logp, (top[row_t].long() == tgt_t).float()]).cpu().tolist()
+        out, k = [], 0
+        for _, sc in pairs:
+            total, hit = 0.0, True
+            for _ in sc:
+                total += host[0][k]
+                hit = hit and host[1][k] == 1.0
+                k += 1
+            out.append((total, hit))
+        return out
 
     def close(self) -> None:
         self._graphs.clear()

@@ -289,11 +289,27 @@ def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
 
 
 def decode_append(qkv: torch.Tensor, pos: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor,
-                  rope: tuple[torch.Tensor, torch.Tensor] | None, n_heads: int) -> None:
+                  rope: tuple[torch.Tensor, torch.Tensor] | None, n_heads: int, slot: torch.Tensor | None = None) -> None:
     """Rotate q / k of every row of the fused ``qkv`` [B, 3d] at position ``pos[b]`` (``rope`` = the ``rope_`` tables, or None)
-    and write k / v into the cache at ``pos[b]``."""
+    and write k / v into the cache at ``pos[b]`` of slot ``slot[b]`` (int32 on the device; None: row ``b`` writes slot ``b``)."""
     cos, sin = rope if rope is not None else (None, None)
-    ext().decode_append(qkv, pos, k_cache, v_cache, cos, sin, int(n_heads))
+    ext().decode_append(qkv, pos, k_cache, v_cache, cos, sin, int(n_heads), slot)
+
+
+def cache_attention(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, tiles: torch.Tensor, out: torch.Tensor,
+                    n_heads: int, scale: float, alibi_slopes: torch.Tensor | None = None) -> torch.Tensor:
+    """Several query rows per cache slot on the tensor cores. ``tiles`` int32 [T, 4] on the device, one row per tile
+    ``(slot, first_row, n_rows <= 64, first_pos)``: rows ``first_row + i`` of ``qkv`` [N, 3d] (q after RoPE) sit at positions
+    ``first_pos + i`` of that slot and attend to its keys ``0 .. first_pos + i``. Writes those rows of ``out`` [N, d] only."""
+    ext().cache_attention(qkv, k_cache, v_cache, tiles, out, int(n_heads), float(scale), alibi_slopes)
+    return out
+
+
+def cache_tiles(runs: list[tuple[int, int, int, int]], device: torch.device | str) -> torch.Tensor:
+    """The tile table of :func:`cache_attention` for runs ``(slot, first_row, n_rows, first_pos)`` of any length: each run
+    is cut into tiles of at most 64 rows."""
+    tiles = [(s, r + o, min(64, n - o), p + o) for s, r, n, p in runs for o in range(0, n, 64)]
+    return torch.tensor(tiles, dtype=torch.int32).reshape(-1, 4).to(device)
 
 
 def embed_pos(ids: torch.Tensor, pos: torch.Tensor, wte: torch.Tensor, wpe: torch.Tensor | None, out: torch.Tensor) -> torch.Tensor:
