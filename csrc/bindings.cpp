@@ -489,13 +489,36 @@ void embed_fwd(const Tensor& ids, const Tensor& wte, const c10::optional<Tensor>
                 int(wte.size(0)), stream_of(ids));
   g_launches += 1;
 }
-void embed_bwd(const Tensor& ids, const Tensor& dh, Tensor& dwte, c10::optional<Tensor> dwpe, int S) {
+// dwte / dwpe: either may be None (a frozen embedding); the kernel of a missing one is not launched
+void embed_bwd(const Tensor& ids, const Tensor& dh, c10::optional<Tensor> dwte, c10::optional<Tensor> dwpe, int S) {
+  check_cuda(ids, "ids");
+  TORCH_CHECK(ids.scalar_type() == at::kLong && ids.is_contiguous(), "ids must be contiguous int64");
   check_bf16(dh, "dh");
-  check_f32(dwte, "dwte");
+  TORCH_CHECK(dh.dim() == 2 && dh.is_contiguous() && dh.size(0) == ids.numel() && dh.size(1) % 8 == 0, "dh must be contiguous [T,d], d % 8 == 0");
+  TORCH_CHECK(S > 0 && ids.numel() % S == 0, "the token count must be a multiple of seq_len");
+  const int d = int(dh.size(1));
+  if (dwte.has_value()) {
+    check_f32(*dwte, "dwte");
+    TORCH_CHECK(dwte->dim() == 2 && dwte->size(1) == d && dwte->is_contiguous(), "dwte must be contiguous [V,d]");
+  }
+  if (dwpe.has_value()) {
+    check_f32(*dwpe, "dwpe");
+    TORCH_CHECK(dwpe->dim() == 2 && dwpe->size(1) == d && dwpe->size(0) >= S && dwpe->is_contiguous(), "dwpe must be contiguous [>=S,d]");
+  }
   c10::cuda::CUDAGuard guard(ids.device());
-  pb::embed_bwd(ids.data_ptr<int64_t>(), dh.data_ptr(), dwte.data_ptr<float>(), dwpe.has_value() ? dwpe->data_ptr<float>() : nullptr,
-                ids.numel(), S, int(dwte.size(1)), int(dwte.size(0)), stream_of(ids));
-  g_launches += dwpe.has_value() ? 2 : 1;
+  pb::embed_bwd(ids.data_ptr<int64_t>(), dh.data_ptr(), dwte.has_value() ? dwte->data_ptr<float>() : nullptr,
+                dwpe.has_value() ? dwpe->data_ptr<float>() : nullptr, ids.numel(), S, d, dwte.has_value() ? int(dwte->size(0)) : 0,
+                stream_of(ids));
+  g_launches += int(dwte.has_value()) + int(dwpe.has_value());
+}
+// dst[C,R] = src[R,C]^T for a 1-byte matrix (row stride ld): the K-major copy of an fp8 operand that is stored MN-major
+void transpose_u8(const Tensor& src, Tensor& dst) {
+  TORCH_CHECK(is_byte(src) && is_byte(dst) && src.dim() == 2 && dst.dim() == 2 && src.stride(1) == 1 && dst.is_contiguous(),
+              "transpose_u8 expects 1-byte 2-D tensors with unit inner stride");
+  TORCH_CHECK(dst.size(0) == src.size(1) && dst.size(1) == src.size(0), "dst must be [C,R] for src [R,C]");
+  c10::cuda::CUDAGuard guard(src.device());
+  pb::transpose_u8(src.data_ptr(), src.stride(0), dst.data_ptr(), int(src.size(0)), int(src.size(1)), stream_of(src));
+  g_launches += 1;
 }
 void layernorm_fwd(const Tensor& x, const Tensor& gamma, const c10::optional<Tensor>& beta, Tensor& y, Tensor& mean, Tensor& rstd,
                    double eps) {
@@ -798,6 +821,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("embed_pos", &embed_pos, py::arg("ids"), py::arg("pos"), py::arg("wte"), py::arg("wpe"), py::arg("out"));
   m.def("argmax_advance", &argmax_advance, py::arg("logits"), py::arg("ids"), py::arg("pos") = py::none());
   m.def("embed_bwd", &embed_bwd);
+  m.def("transpose_u8", &transpose_u8);
   m.def("layernorm_fwd", &layernorm_fwd);
   m.def("layernorm_bwd", &layernorm_bwd);
   m.def("col_sum", &col_sum);

@@ -395,7 +395,7 @@ __global__ void __launch_bounds__(256) col_reduce_kernel(const __nv_bfloat16* __
     float s = 0.f, t = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) s += ssum[i][c], t += sdot[i][c];
-    atomicAdd(out_sum + blockIdx.x * 256 + c, s);
+    if (out_sum) atomicAdd(out_sum + blockIdx.x * 256 + c, s);   // null: LN dgamma only (frozen or absent beta)
     if (out_dot) atomicAdd(out_dot + blockIdx.x * 256 + c, t);
   }
 }
@@ -671,8 +671,10 @@ void embed_fwd(const int64_t* ids, const void* wte, const void* wpe, void* out, 
   PB_CHECK_LAUNCH("embed_fwd");
 }
 void embed_bwd(const int64_t* ids, const void* dh, float* dwte, float* dwpe, long long T, int S, int d, int V, cudaStream_t st) {
-  embed_bwd_wte_kernel<<<grid_for(T, 1, 132 * 16), 128, 0, st>>>(ids, (const __nv_bfloat16*)dh, dwte, T, d, V);
-  PB_CHECK_LAUNCH("embed_bwd_wte");
+  if (dwte) {   // null when the token embedding is frozen
+    embed_bwd_wte_kernel<<<grid_for(T, 1, 132 * 16), 128, 0, st>>>(ids, (const __nv_bfloat16*)dh, dwte, T, d, V);
+    PB_CHECK_LAUNCH("embed_bwd_wte");
+  }
   if (dwpe) {
     embed_bwd_wpe_kernel<<<S, 128, 0, st>>>((const __nv_bfloat16*)dh, dwpe, int(T / S), S, d);
     PB_CHECK_LAUNCH("embed_bwd_wpe");

@@ -35,7 +35,61 @@ import torch.nn.functional as F
 from photon_b200 import ops
 from photon_b200.models.mpt import MPTConfig, MPTForCausalLM, shift_labels
 from photon_b200.train.backend import apply_freeze
-from photon_b200.utils.flat import FlatParams
+from photon_b200.utils.flat import FlatLayout, FlatParams
+
+# One block's backward as stages in execution order, each with the parameters whose gradients it produces (a stage's input
+# gradient feeds the next one; the residual path joins at ln2 / ln1). "attn" is the attention backward with the q/k LayerNorms.
+BLOCK_STAGES = (("down", ("ffn.down_proj.weight", "ffn.down_proj.bias")),
+                ("up", ("ffn.up_proj.weight", "ffn.up_proj.bias")),
+                ("ln2", ("norm_2.weight", "norm_2.bias")),
+                ("out", ("attn.out_proj.weight", "attn.out_proj.bias")),
+                ("attn", ("attn.q_ln.weight", "attn.q_ln.bias", "attn.k_ln.weight", "attn.k_ln.bias")),
+                ("qkv", ("attn.Wqkv.weight", "attn.Wqkv.bias")),
+                ("ln1", ("norm_1.weight", "norm_1.bias")))
+
+
+class BackwardPlan:
+    """Which parts of the backward run, given the trainable parameter names (a pure function of the config and that set).
+
+    The backward is one chain of stages: LM head, final LayerNorm, the blocks from the last down to the first
+    (:data:`BLOCK_STAGES` each), embeddings. A stage runs when it, or any stage after it, has a trainable parameter; its input
+    gradient (the dgrad GEMM, the LayerNorm dx) is computed only when a later stage has one. So the backward stops right after the
+    last stage that produces a trainable gradient, and weight / bias / LayerNorm-parameter gradients run for trainable names
+    only. With every parameter trainable this is the full schedule."""
+
+    def __init__(self, n_layers: int, trainable: Any) -> None:
+        self.n_layers = int(n_layers)
+        self.trainable = frozenset(trainable)
+        t = lambda names, pre="transformer.": any(pre + n in self.trainable for n in names)  # noqa: E731
+        chain = [("head", t(("wte.weight",))), ("norm_f", t(("norm_f.weight", "norm_f.bias")))]
+        for i in range(self.n_layers - 1, -1, -1):
+            chain += [((i, s), t(names, f"transformer.blocks.{i}.")) for s, names in BLOCK_STAGES]
+        chain.append(("embed", t(("wte.weight", "wpe.weight"))))
+        self._pos = {k: j for j, (k, _) in enumerate(chain)}
+        self.last = max((j for j, (_, has) in enumerate(chain) if has), default=-1)   # the last stage that runs
+
+    def runs(self, stage: Any) -> bool:
+        """``stage``: "head", "norm_f", "embed" or ``(block, name)`` with a name of :data:`BLOCK_STAGES`."""
+        return self._pos[stage] <= self.last
+
+    def dx(self, stage: Any) -> bool:
+        """Whether the stage computes the gradient of its input (some stage after it needs it)."""
+        return self._pos[stage] < self.last
+
+    def grad(self, name: str) -> bool:
+        return name in self.trainable
+
+    @property
+    def head_wgrad(self) -> bool:
+        return self.grad("transformer.wte.weight")
+
+    @property
+    def lowest_block(self) -> int:
+        """The lowest block whose backward runs (``n_layers`` when none does)."""
+        return next((i for i in range(self.n_layers) if self.runs((i, BLOCK_STAGES[0][0]))), self.n_layers)
+
+    def block_stages(self, i: int) -> list[str]:
+        return [s for s, _ in BLOCK_STAGES if self.runs((i, s))]
 
 
 class _LayerW:
@@ -64,8 +118,8 @@ class B200Engine:
             raise RuntimeError("B200Engine needs a CUDA (sm_90a) device")
         if precision not in ("amp_bf16", "amp_fp8"):
             raise NotImplementedError(f"B200Engine computes in bf16 (got precision={precision}); use kernels.*=torch for fp32/fp16")
-        if frozen_layers or unfrozen_layers:
-            raise NotImplementedError("frozen/unfrozen layers run on the torch backend (kernels.*=torch)")
+        if (frozen_layers or unfrozen_layers) and zero3 is not None:
+            raise NotImplementedError("freeze lists are not covered under full parameter sharding (kernels.*=torch runs them)")
         ops.ext()  # fail loudly if the extension is missing
         self.precision = precision
         self.zero3 = zero3
@@ -108,6 +162,8 @@ class B200Engine:
                 self.flat.layout.total, dtype=torch.bfloat16, device=self.device)
             if self.bf16_params.numel() != self.flat.layout.total or self.bf16_params.dtype != torch.bfloat16:
                 raise ValueError("shadow_storage must be a bf16 tensor with layout.total elements")
+        self._init_frozen_planes()
+        self.plan = BackwardPlan(cfg.n_layers, self.flat.layout.names)
         self.unigram_log_probs = unigram_log_probs.to(self.device) if unigram_log_probs is not None else None
         self.lm_head_chunk = int(lm_head_chunk)
         # positional variants of the MPT attention block (ref: SURVEY §5.7): ALiBi slopes enter the attention kernels,
@@ -130,14 +186,43 @@ class B200Engine:
         self.params_updated()
 
     # ------------------------------------------------------------------ binding
+    def _init_frozen_planes(self) -> None:
+        """Storage of the frozen tensors (``fl.frozen_layers`` / ``fl.unfrozen_layers``): they are not in the trainable flat, so
+        they get a flat layout of their own, an fp32 plane (read by LayerNorms, bias epilogues, q/k-LN) and its bf16 cast (read by
+        the GEMMs). The module's frozen parameters become views of the fp32 plane, like the trainable ones of :class:`FlatParams`.
+        Nothing trains them: the optimizer, the round kernels and the gradient all-reduce only see the trainable flat."""
+        self.frozen_layout: FlatLayout | None = None
+        self.frozen_params = self.frozen_bf16 = None
+        named = sorted(((n, p) for n, p in self.model.named_parameters() if not p.requires_grad), key=lambda kv: kv[0]) \
+            if self.model is not None else []
+        if not named:
+            return
+        lay = self.frozen_layout = FlatLayout.build((n, p.shape) for n, p in named)
+        self.frozen_params = torch.zeros(lay.total, dtype=torch.float32, device=self.device)
+        self.frozen_bf16 = torch.zeros(lay.total, dtype=torch.bfloat16, device=self.device)
+        with torch.no_grad():
+            for i, (_, p) in enumerate(named):
+                v = lay.view(self.frozen_params, i)
+                v.copy_(p.detach())
+                p.data = v
+
     def _bind(self) -> None:
         lay, P, G, Sd = self.flat.layout, self.flat.params, self.flat.grads, self.bf16_params
         have = set(lay.names)
+        flay, FP, F16 = self.frozen_layout, self.frozen_params, self.frozen_bf16
+        frozen = set(flay.names) if flay is not None else set()
+
         # biases are absent under `no_bias`: every consumer below accepts None (GEMM without bias, LN without beta,
-        # no bias-gradient column sums)
-        v32 = lambda n: lay.view(P, "transformer." + n) if "transformer." + n in have else None  # noqa: E731
+        # no bias-gradient column sums); a frozen tensor is read from the frozen planes and has no gradient (None)
+        def v32(n: str) -> torch.Tensor | None:
+            n = "transformer." + n
+            return lay.view(P, n) if n in have else flay.view(FP, n) if n in frozen else None
+
+        def v16(n: str) -> torch.Tensor:
+            n = "transformer." + n
+            return flay.view(F16, n) if n in frozen else lay.view(Sd, n)
+
         vg = lambda n: lay.view(G, "transformer." + n) if "transformer." + n in have else None  # noqa: E731
-        v16 = lambda n: lay.view(Sd, "transformer." + n)  # noqa: E731
         if self.zero3 is not None:
             # weights: views into the two rotating block buffers (block i -> buffer i % 2) / the resident embedding buffer;
             # 1-D fp32 parameters: the packed resident buffer; gradients: the block's staging plane (reduced after its backward)
@@ -180,6 +265,16 @@ class B200Engine:
             self.zero3.params_changed()
             return
         ops.cast_bf16(self.flat.params, self.bf16_params)
+        self._frozen_updated()
+
+    def _frozen_updated(self) -> None:
+        """Re-derive the frozen tensors' compute copies (bf16 cast; under amp_fp8 their E4M3 copies and weight scales) from the
+        fp32 frozen plane. Training never changes that plane, so this runs only when its values are set."""
+        if self.frozen_params is None:
+            return
+        ops.cast_bf16(self.frozen_params, self.frozen_bf16)
+        if self.fp8 and self.w8f_seg is not None:
+            self._fp8_quantize_frozen()
 
     # ---------------------------------------------------------------------- fp8
     _DYN_ROLES = ("x_ln1", "x_attn", "x_ln2", "x_u", "g_dqkv", "g_dhmid", "g_dz", "g_dh")   # per block: 4 × E4M3, 4 × E5M2
@@ -189,7 +284,11 @@ class B200Engine:
         """Device-resident scaling state: ``meta`` = [3, n_roles] (scale, 1/scale, running amax). Roles [0, 8L) are activations
         and gradients (delayed scaling: amax history → next scale, ``ops.fp8_update_scales``); roles [8L, 12L) are the weight
         matrices (current scaling, re-quantised from the bf16 shadow at the start of every microbatch — two passes over
-        ≤ 2 bytes/param, so whoever wrote the shadow (optimizer, round broadcast, ZeRO step) needs no hook)."""
+        ≤ 2 bytes/param, so whoever wrote the shadow (optimizer, round broadcast, ZeRO step) needs no hook).
+
+        Frozen matrices never change: they are quantised once, whenever their values are set (:meth:`_frozen_updated`), into a
+        plane at the frozen layout's offsets, with a transposed (K-major) copy next to it that their dgrad GEMMs read directly.
+        Their weight roles come after the trainable ones, so each group is one contiguous role range."""
         L, lay, dev = self.cfg.n_layers, self.flat.layout, self.device
         self._n_dyn = len(self._DYN_ROLES) * L
         n_roles = self._n_dyn + len(self._W_ROLES) * L
@@ -199,28 +298,49 @@ class B200Engine:
         self.fp8_fmax = torch.tensor([ops.FP8_MAX[0 if j < 4 else 1] for _ in range(L) for j in range(8)], dtype=torch.float32, device=dev)
         self.fp8_pos = torch.zeros(1, dtype=torch.int32, device=dev)
         self.fp8_margin_mult = float(2.0 ** margin)
+        flay = self.frozen_layout
         self.w8 = torch.zeros(lay.total, dtype=torch.uint8, device=dev)      # E4M3 weights at the flat layout's offsets
-        seg, self.w8_views = [], []
+        self.w8f = torch.zeros(flay.total, dtype=torch.uint8, device=dev) if flay is not None else None   # ... at the frozen layout's
+        seg, fseg, order, self.w8_views, self.w8t_views = [], [], [], [], []
         for i in range(L):
-            views = {}
             for key, name in zip(self._W_ROLES, ("attn.Wqkv.weight", "attn.out_proj.weight", "ffn.up_proj.weight", "ffn.down_proj.weight")):
-                j = lay.index(f"transformer.blocks.{i}.{name}")
-                seg.append((lay.offsets[j], lay.numels[j]))
-                views[key] = lay.view(self.w8, j)
-            self.w8_views.append(views)
-        self.w8_seg = torch.tensor(seg, dtype=torch.int64, device=dev)
+                n = f"transformer.blocks.{i}.{name}"
+                (fseg if flay is not None and n in flay.names else seg).append((i, key, n))
+            self.w8_views.append({})
+            self.w8t_views.append({})
+        self._w_role = {}
+        for r, (i, key, n) in enumerate(seg + fseg):
+            self._w_role[(i, key)] = self._n_dyn + r
+        for i, key, n in seg:
+            self.w8_views[i][key] = lay.view(self.w8, n)
+        for i, key, n in fseg:
+            self.w8_views[i][key] = flay.view(self.w8f, n)
+            N, K = flay.shapes[flay.index(n)]
+            self.w8t_views[i][key] = torch.empty(K, N, dtype=torch.uint8, device=dev)   # W^T: the dgrad GEMM's K-major B operand
+        table = lambda lo, s: torch.tensor([(lo.offsets[lo.index(n)], lo.numels[lo.index(n)]) for _, _, n in s],  # noqa: E731
+                                           dtype=torch.int64, device=dev).reshape(-1, 2)
+        self.w8_seg = table(lay, seg)
+        self.w8f_seg = table(flay, fseg) if fseg else None
+        self._n_w8 = len(seg)
         self._fp8_calibrated = False
 
     def _role(self, name: str, layer: int) -> int:
         if name in self._DYN_ROLES:
             return layer * len(self._DYN_ROLES) + self._DYN_ROLES.index(name)
-        return self._n_dyn + layer * len(self._W_ROLES) + self._W_ROLES.index(name)
+        return self._w_role[(layer, name)]
+
+    def _fp8_quantize_frozen(self) -> None:
+        ops.fp8_quantize_segments(self.frozen_bf16, self.w8f, self.w8f_seg, self.fp8_meta, self._n_dyn + self._n_w8)
+        for w8, w8t in zip(self.w8_views, self.w8t_views):
+            for key, t in w8t.items():
+                ops.transpose_u8(w8[key], t)
 
     def _fp8_prologue(self, train: bool) -> None:
-        """Start of a microbatch: roll the delayed scales (training only) and re-quantise the weights from the shadow."""
+        """Start of a microbatch: roll the delayed scales (training only) and re-quantise the trainable weights from the shadow."""
         if train:
             ops.fp8_update_scales(self.fp8_meta, self.fp8_hist, self.fp8_fmax, self.fp8_pos, self._n_dyn, self.fp8_margin_mult)
-        ops.fp8_quantize_segments(self.bf16_params, self.w8, self.w8_seg, self.fp8_meta, self._n_dyn)
+        if self._n_w8:
+            ops.fp8_quantize_segments(self.bf16_params, self.w8, self.w8_seg, self.fp8_meta, self._n_dyn)
 
     def fp8_state_dict(self) -> dict[str, Any] | None:
         """Scales / amax histories, checkpointed next to the optimizer so a resumed run casts with the scales it stopped with."""
@@ -232,6 +352,8 @@ class B200Engine:
         if self.fp8 and sd and "meta" in sd and tuple(sd["meta"].shape) == tuple(self.fp8_meta.shape):
             self.fp8_meta.copy_(sd["meta"]), self.fp8_hist.copy_(sd["hist"]), self.fp8_pos.copy_(sd["pos"])
             self._fp8_calibrated = bool(sd.get("calibrated", True))
+            if self.w8f_seg is not None:   # the frozen E4M3 bytes must stay paired with their (current-scaling) weight scales
+                self._fp8_quantize_frozen()
 
     # ---------------------------------------------------------------- workspace
     def _workspace(self, b: int, S: int) -> dict[str, Any]:
@@ -378,67 +500,101 @@ class B200Engine:
             ops.gemm(ws["lnf"][lo:hi], self.wte16, logits)
             ops.cross_entropy(logits, targets[lo:hi], grad_scale, train, self._stats, None, self.unigram_log_probs)
             if train:
-                ops.linear_dgrad(logits, self.wte16, ws["dlnf"][lo:hi])
-                ops.linear_wgrad(logits, ws["lnf"][lo:hi], self.d_wte, accumulate=True)
+                if self.plan.dx("head"):
+                    ops.linear_dgrad(logits, self.wte16, ws["dlnf"][lo:hi])
+                if self.plan.head_wgrad:
+                    ops.linear_wgrad(logits, ws["lnf"][lo:hi], self.d_wte, accumulate=True)
 
     # ----------------------------------------------------------------- backward
     def _linear_bwd(self, i: int, ws: dict[str, Any], dy: torch.Tensor, g_role: str, x: torch.Tensor, x_role: str, w_role: str,
-                    w16: torch.Tensor, dw: torch.Tensor, db: torch.Tensor | None, dx: torch.Tensor, mul: torch.Tensor | None = None) -> None:
-        """Backward of ``y = x @ w^T + b``: db += colsum(dy); dw += dy^T x; dx = dy w (optionally ``* mul``).
+                    w16: torch.Tensor, dw: torch.Tensor | None, db: torch.Tensor | None, dx: torch.Tensor | None,
+                    mul: torch.Tensor | None = None) -> None:
+        """Backward of ``y = x @ w^T + b``: db += colsum(dy); dw += dy^T x; dx = dy w (optionally ``* mul``). A None ``dw`` /
+        ``db`` / ``dx`` (frozen weight / bias, no trainable tensor below) skips that GEMM or column sum.
         fp8: the column-sum pass also emits the E5M2 copy of ``dy`` both GEMMs read; ``x`` is the saved E4M3 input."""
         if not self.fp8:
             if db is not None:
                 ops.col_sum(dy, db)
-            ops.linear_wgrad(dy, x, dw)
-            ops.linear_dgrad(dy, w16, dx, mul=mul)
+            if dw is not None:
+                ops.linear_wgrad(dy, x, dw)
+            if dx is not None:
+                ops.linear_dgrad(dy, w16, dx, mul=mul)
             return
         M, R = self.fp8_meta, self._role
         T, n = dy.shape
-        dy8 = ws["g8"][: T * n].view(T, n)
-        ops.colsum_quant(dy, db, dy8, ops.E5M2, M, R(g_role, i))
-        ops.gemm_fp8(dy8, x, dw, M, R(g_role, i), R(x_role, i), a_mn=True, b_mn=True, epi=ops.EPI_F32, a_fmt=ops.E5M2, b_fmt=ops.E4M3,
-                     accumulate=True)
-        ops.gemm_fp8(dy8, self.w8_views[i][w_role], dx, M, R(g_role, i), R(w_role, i), b_mn=True, epi=ops.EPI_MUL if mul is not None else ops.EPI_BF16,
-                     a_fmt=ops.E5M2, b_fmt=ops.E4M3, aux=mul)
+        dy8 = ws["g8"][: T * n].view(T, n) if dw is not None or dx is not None else None
+        if dy8 is not None or db is not None:
+            ops.colsum_quant(dy, db, dy8, ops.E5M2, M, R(g_role, i))
+        if dw is not None:
+            ops.gemm_fp8(dy8, x, dw, M, R(g_role, i), R(x_role, i), a_mn=True, b_mn=True, epi=ops.EPI_F32, a_fmt=ops.E5M2,
+                         b_fmt=ops.E4M3, accumulate=True)
+        if dx is not None:
+            # a frozen weight has a resident K-major (transposed) copy; a trainable one is transposed by the GEMM binding
+            wt = self.w8t_views[i].get(w_role)
+            ops.gemm_fp8(dy8, wt if wt is not None else self.w8_views[i][w_role], dx, M, R(g_role, i), R(w_role, i), b_mn=wt is None,
+                         epi=ops.EPI_MUL if mul is not None else ops.EPI_BF16, a_fmt=ops.E5M2, b_fmt=ops.E4M3, aux=mul)
 
     def _backward(self, ids: torch.Tensor, ws: dict[str, Any]) -> None:
         c = self.cfg
         b, S = ids.shape
         h = ws["h"]
-        dh, dhmid, dln = ws["dh"], ws["dhmid"], ws["dln"]
-        z = self.zero3
-        ops.layernorm_bwd(ws["dlnf"], h[c.n_layers], self.gf, ws["mf"], ws["rf"], None, dh, self.d_gf, self.d_bf)
-        for i in range(c.n_layers - 1, -1, -1):
-            w, lw = self.layers[i], ws["layers"][i]
+        dh = ws["dh"]
+        z, P = self.zero3, self.plan
+        if P.runs("norm_f"):
+            ops.layernorm_bwd(ws["dlnf"], h[c.n_layers], self.gf, ws["mf"], ws["rf"], None, dh, self.d_gf, self.d_bf)
+        # blocks below the lowest one with a trainable tensor (and their recompute) are skipped: see BackwardPlan
+        for i in range(c.n_layers - 1, P.lowest_block - 1, -1):
             if z is not None:
                 z.acquire(i)
                 z.prefetch(i - 1)
                 z.zero_stage(i)       # this microbatch's gradient of block i (the shard accumulates over microbatches)
             if self.activation_checkpointing and i < c.n_layers - 1:
                 self._block_fwd(i, ws, b, S)   # recompute (the shared buffers still hold the LAST block after the forward)
-            # ---- FFN: h[i+1] = hmid + down(gelu(up(ln2(hmid))))
-            self._linear_bwd(i, ws, dh, "g_dh", lw["u"], "x_u", "wdown", w.wdown, w.d_wdown, w.d_bdown, ws["dz"], mul=lw["z"])
-            self._linear_bwd(i, ws, ws["dz"], "g_dz", lw["ln2"], "x_ln2", "wup", w.wup, w.d_wup, w.d_bup, dln)
-            ops.layernorm_bwd(dln, lw["hmid"], w.g2, lw["m2"], lw["r2"], dh, dhmid, w.d_g2, w.d_b2)
-            # ---- attention: hmid = h[i] + out_proj(attn(qkv(ln1(h[i]))))
-            self._linear_bwd(i, ws, dhmid, "g_dhmid", lw["attn8"] if self.fp8 else lw["attn"], "x_attn", "wo", w.wo, w.d_wo, w.d_bo, ws["dattn"])
-            self._attention_bwd(lw, ws, b, S)
-            if c.qk_ln:
-                dqkv3 = ws["dqkv"].view(-1, 3, c.d_model)
-                for j in range(2):
-                    ws["qk_tmp"].copy_(dqkv3[:, j])
-                    ops.layernorm_bwd(ws["qk_tmp"], lw["qk_pre"][j], w.qk_g[j], lw["qk_m"][j], lw["qk_r"][j], None, ws["qk_tmp2"],
-                                      w.d_qk_g[j], w.d_qk_b[j])
-                    dqkv3[:, j].copy_(ws["qk_tmp2"])
-            if c.clip_qkv:
-                ws["dqkv"].mul_(lw["clipmask"])
-            self._linear_bwd(i, ws, ws["dqkv"], "g_dqkv", lw["ln1"], "x_ln1", "wqkv", w.wqkv, w.d_wqkv, w.d_bqkv, dln)
-            ops.layernorm_bwd(dln, h[i], w.g1, lw["m1"], lw["r1"], dhmid, dh, w.d_g1, w.d_b1)
+            self._block_bwd(i, ws, b, S)
             if z is not None:
                 z.reduce(i)           # reduce-scatter: every rank adds the mean of ITS slice into its gradient shard
-        ops.embed_bwd(ids.reshape(-1), dh, self.d_wte, self.d_wpe, S)
+        if P.runs("embed"):
+            ops.embed_bwd(ids.reshape(-1), dh, self.d_wte, self.d_wpe, S)
         if z is not None:
             z.reduce(z.plan.rest)
+
+    def _block_bwd(self, i: int, ws: dict[str, Any], b: int, S: int) -> None:
+        """dh (gradient w.r.t. h[i+1]) -> dh (w.r.t. h[i]), accumulating block i's trainable parameter gradients; returns after the
+        last stage the plan runs (the lowest trainable block only)."""
+        c, h, w, lw, P = self.cfg, ws["h"], self.layers[i], ws["layers"][i], self.plan
+        dh, dhmid, dln = ws["dh"], ws["dhmid"], ws["dln"]
+        dx = lambda s, t: t if P.dx((i, s)) else None  # noqa: E731
+        # ---- FFN: h[i+1] = hmid + down(gelu(up(ln2(hmid))))
+        self._linear_bwd(i, ws, dh, "g_dh", lw["u"], "x_u", "wdown", w.wdown, w.d_wdown, w.d_bdown, dx("down", ws["dz"]), mul=lw["z"])
+        if not P.runs((i, "up")):
+            return
+        self._linear_bwd(i, ws, ws["dz"], "g_dz", lw["ln2"], "x_ln2", "wup", w.wup, w.d_wup, w.d_bup, dx("up", dln))
+        if not P.runs((i, "ln2")):
+            return
+        ops.layernorm_bwd(dln, lw["hmid"], w.g2, lw["m2"], lw["r2"], dh, dhmid, w.d_g2, w.d_b2)
+        if not P.runs((i, "out")):
+            return
+        # ---- attention: hmid = h[i] + out_proj(attn(qkv(ln1(h[i]))))
+        self._linear_bwd(i, ws, dhmid, "g_dhmid", lw["attn8"] if self.fp8 else lw["attn"], "x_attn", "wo", w.wo, w.d_wo, w.d_bo,
+                         dx("out", ws["dattn"]))
+        if not P.runs((i, "attn")):
+            return
+        self._attention_bwd(lw, ws, b, S)
+        if c.qk_ln:
+            dqkv3 = ws["dqkv"].view(-1, 3, c.d_model)
+            for j in range(2):
+                ws["qk_tmp"].copy_(dqkv3[:, j])
+                ops.layernorm_bwd(ws["qk_tmp"], lw["qk_pre"][j], w.qk_g[j], lw["qk_m"][j], lw["qk_r"][j], None, ws["qk_tmp2"],
+                                  w.d_qk_g[j], w.d_qk_b[j])
+                dqkv3[:, j].copy_(ws["qk_tmp2"])
+        if c.clip_qkv:
+            ws["dqkv"].mul_(lw["clipmask"])
+        if not P.runs((i, "qkv")):
+            return
+        self._linear_bwd(i, ws, ws["dqkv"], "g_dqkv", lw["ln1"], "x_ln1", "wqkv", w.wqkv, w.d_wqkv, w.d_bqkv, dx("qkv", dln))
+        if not P.runs((i, "ln1")):
+            return
+        ops.layernorm_bwd(dln, h[i], w.g1, lw["m1"], lw["r1"], dhmid, dh, w.d_g1, w.d_b1)
 
     # ---------------------------------------------------------------- protocol
     def _fwd_bwd_eager(self, ids: torch.Tensor, grad_scale: float) -> None:

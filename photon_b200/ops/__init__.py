@@ -147,6 +147,12 @@ def fp8_quantize_segments(src_bf16: torch.Tensor, dst8: torch.Tensor, seg: torch
     ext().fp8_quantize_segments(src_bf16, dst8, seg, meta, int(role0))
 
 
+def transpose_u8(src: torch.Tensor, dst: torch.Tensor) -> torch.Tensor:
+    """``dst[C,R] = src[R,C]^T`` for 1-byte matrices: a K-major copy of an fp8 operand stored MN-major."""
+    ext().transpose_u8(src, dst)
+    return dst
+
+
 def fp8_update_scales(meta: torch.Tensor, hist: torch.Tensor, fmax: torch.Tensor, pos: torch.Tensor, n: int, margin_mult: float = 1.0) -> None:
     """Delayed scaling for roles [0, n): amax → history ring → scale for the next cast; amax reset."""
     ext().fp8_update_scales(meta, hist, fmax, pos, int(n), float(margin_mult))
@@ -158,7 +164,8 @@ def embed_fwd(ids: torch.Tensor, wte: torch.Tensor, wpe: torch.Tensor | None, ou
     return out
 
 
-def embed_bwd(ids: torch.Tensor, dh: torch.Tensor, dwte: torch.Tensor, dwpe: torch.Tensor | None, seq_len: int) -> None:
+def embed_bwd(ids: torch.Tensor, dh: torch.Tensor, dwte: torch.Tensor | None, dwpe: torch.Tensor | None, seq_len: int) -> None:
+    """``dwte[ids[t]] += dh[t]`` and ``dwpe[t % seq_len] += dh[t]`` (fp32); a None gradient (frozen embedding) is skipped."""
     ext().embed_bwd(ids, dh, dwte, dwpe, int(seq_len))
 
 

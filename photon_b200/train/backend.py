@@ -156,8 +156,8 @@ def build_backend(model_cfg: MPTConfig, device: torch.device, precision: str, ke
         unsupported = []
         if precision not in ("amp_bf16", "amp_fp8"):
             unsupported.append(f"precision={precision}")
-        if kw.get("frozen_layers") or kw.get("unfrozen_layers"):
-            unsupported.append("frozen/unfrozen layers")
+        if (kw.get("frozen_layers") or kw.get("unfrozen_layers")) and kw.get("zero3") is not None:
+            unsupported.append("frozen/unfrozen layers")   # the ZeRO-3 unit plan assumes every block tensor is in the flat
         if unsupported:
             print(f"[backend] {', '.join(unsupported)} not covered by the sm_90a engine -> stock PyTorch backend "
                   "(explicit, logged; set kernels.*=torch to silence)", flush=True)

@@ -11,15 +11,16 @@ SEL='layernorm or cross_entropy or embedding or colsum or optimizer or gemm_kk_b
 # synccheck treats an mbarrier phase that completes without a waiter as "Missing wait" and kills the kernel: the attention kernels
 # commit `pv_done` after every P·V but only wait on it when a row's reference maximum moved (a rescale) — by design — so they are
 # left out of the synccheck pass; initcheck tracks every global byte and is run on a smaller selection. memcheck also covers the
-# scoring kernels (cache attention, slotted cache append).
+# scoring kernels (cache attention, slotted cache append) and the embedding backward without a token-embedding gradient.
 rc=0
 for TOOL in $TOOLS; do
   CUR="$SEL"
-  [ "$TOOL" = memcheck ] && CUR="$SEL or cache_attention or slotted_decode_append"
+  EXTRA=""
+  [ "$TOOL" = memcheck ] && CUR="$SEL or cache_attention or slotted_decode_append or embed_bwd_without" && EXTRA="tests/test_frozen_gpu.py"
   [ "$TOOL" = synccheck ] && CUR="layernorm or cross_entropy or embedding or colsum or optimizer or gemm_kk_bias or gemm_fp8_forward or gemm_fp8_wgrad or gelu_epilogue or weight_segments or fed_round_matches_oracle or allreduce"
   [ "$TOOL" = initcheck ] && CUR="layernorm or gemm_kk_bias or gemm_fp8_wgrad or weight_segments or (fed_round_matches_oracle and fedadam)"
   compute-sanitizer --tool "$TOOL" --error-exitcode 3 --print-limit 20 \
-    python -m pytest tests/test_kernels_gpu.py tests/test_fp8_gpu.py tests/test_attention_gpu.py tests/test_score_gpu.py tests/test_multigpu.py -x -q -k "$CUR" \
+    python -m pytest tests/test_kernels_gpu.py tests/test_fp8_gpu.py tests/test_attention_gpu.py tests/test_score_gpu.py tests/test_multigpu.py $EXTRA -x -q -k "$CUR" \
     2>&1 | tail -25 | tee "gpurun_out/sanitizer_$TOOL.log"
   [ "${PIPESTATUS[0]}" -ne 0 ] && rc=1
 done
