@@ -727,6 +727,34 @@ void zero3_reduce(const std::vector<int64_t>& ctl_ptrs, int rank, int device, in
                           at::cuda::getCurrentCUDAStream(device).stream());
   g_launches += 1;
 }
+// ZeRO-3 under amp_fp8: global amax exchange + E4M3 quantisation of this rank's pieces of every block weight matrix (see comm.cu)
+void zero3_fp8_requant(const std::vector<int64_t>& ctl_ptrs, int rank, int device, int64_t epoch, const Tensor& w16, Tensor& w8,
+                       const Tensor& pieces, Tensor& amax_local, const std::vector<int64_t>& amax_ptrs, Tensor& meta, const Tensor& roles) {
+  c10::cuda::CUDAGuard guard(static_cast<c10::DeviceIndex>(device));
+  pb::CommCtl c = make_ctl(ctl_ptrs, rank);
+  check_bf16(w16, "w16");
+  check_f32(amax_local, "amax_local");
+  check_f32(meta, "meta");
+  check_cuda(pieces, "pieces");
+  check_cuda(roles, "roles");
+  TORCH_CHECK(is_byte(w8) && w8.numel() == w16.numel() && w8.is_contiguous() && w16.is_contiguous(), "w8: a 1-byte shard as long as w16");
+  TORCH_CHECK(pieces.scalar_type() == at::kLong && pieces.dim() == 2 && pieces.size(1) == 3 && pieces.is_contiguous(),
+              "pieces must be int64 [n,3] (shard offset, numel, weight slot) on the device");
+  TORCH_CHECK(roles.scalar_type() == at::kInt && roles.dim() == 1 && roles.is_contiguous(), "roles must be int32 [n_weights]");
+  TORCH_CHECK(amax_local.numel() == roles.numel() && amax_local.is_contiguous(), "amax_local: one fp32 per weight");
+  TORCH_CHECK(meta.dim() == 2 && meta.size(0) == 3 && meta.is_contiguous(), "meta must be fp32 [3, n_roles]");
+  TORCH_CHECK(int(amax_ptrs.size()) == c.n, "one amax plane per rank");
+  pb::Zero3RequantArgs a{};
+  a.w16 = w16.data_ptr(), a.w8 = static_cast<uint8_t*>(w8.data_ptr());
+  a.pieces = reinterpret_cast<const long long*>(pieces.data_ptr<int64_t>()), a.n_pieces = int(pieces.size(0));
+  a.n_w = int(roles.numel()), a.amax_local = amax_local.data_ptr<float>();
+  for (int i = 0; i < c.n; ++i) a.amax[i] = reinterpret_cast<float*>(amax_ptrs[i]);
+  a.meta = meta.data_ptr<float>(), a.n_roles = meta.size(1), a.roles = roles.data_ptr<int>();
+  a.fmax = 448.0f;
+  pb::zero3_fp8_requant_launch(a, c, uint32_t(epoch), at::cuda::getCurrentDeviceProperties()->multiProcessorCount,
+                               at::cuda::getCurrentCUDAStream(device).stream());
+  g_launches += 1;
+}
 
 // device-to-device copy between (possibly peer-mapped) raw addresses on the current stream: the copy engines pull a parameter
 // slice from its owner over NVLink without occupying an SM
@@ -849,6 +877,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("lo"), py::arg("hi"), py::arg("out_norm") = py::none(), py::arg("buf_mc") = 0);
   m.def("zero3_reduce", &zero3_reduce, py::arg("ctl_ptrs"), py::arg("rank"), py::arg("device"), py::arg("epoch"), py::arg("stage_ptrs"),
         py::arg("stage_mc"), py::arg("dst"), py::arg("per"));
+  m.def("zero3_fp8_requant", &zero3_fp8_requant, py::arg("ctl_ptrs"), py::arg("rank"), py::arg("device"), py::arg("epoch"), py::arg("w16"),
+        py::arg("w8"), py::arg("pieces"), py::arg("amax_local"), py::arg("amax_ptrs"), py::arg("meta"), py::arg("roles"));
   m.def("memcpy_async", &memcpy_async);
   m.def("ddp_zero_step", &ddp_zero_step, py::arg("ctl_ptrs"), py::arg("rank"), py::arg("device"), py::arg("epoch"), py::arg("grad_ptrs"),
         py::arg("param_ptrs"), py::arg("shadow_ptrs"), py::arg("m"), py::arg("v"), py::arg("lo"), py::arg("hi"), py::arg("kind"),

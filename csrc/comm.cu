@@ -8,6 +8,8 @@
 //                      AND their bf16 cast straight into every peer's parameter planes with P2P stores.
 //   ddp_allreduce_kernel  N1: one-pass reduce-scatter + all-gather of the flat gradient bucket over peer
 //                      pointers, fused with the mean (1/n) and the squared-norm partials for clipping.
+//   zero3_reduce_kernel   ZeRO-3 reduce-scatter of one unit's gradient into the owner's shard.
+//   zero3_fp8_requant_kernel  ZeRO-3 under amp_fp8: global per-tensor amax exchange + E4M3 quantisation of the weight shards.
 //
 // Cross-GPU ordering uses epoch-valued flags in each rank's control page (st.release.sys /
 // ld.acquire.sys); all CTAs are co-resident (grid <= #SMs) so in-kernel spinning is deadlock-free.
@@ -19,6 +21,7 @@
 #include <string>
 
 #include "comm.h"
+#include "fp8_round.cuh"
 #include "optim_dev.cuh"
 #include "ptx.cuh"
 
@@ -399,6 +402,101 @@ __global__ void __launch_bounds__(512) zero3_reduce_kernel(const ShardReduceArgs
   if (grid_done(c)) peer_barrier_end(c, epoch);
 }
 
+// ------------------------------------------------------------------------------------------ ZeRO-3 E4M3 weight shards
+// Launched once per parameter version, after every rank has written its new bf16 shard. Phase 1: the partial amax of every block
+// weight matrix over this rank's pieces of it; the last block publishes this rank's amax vector into row `rank` of every peer's
+// amax plane. Mid barrier. Phase 2: global amax = max over the rows (order independent: every rank gets the same value), scale
+// exactly as seg_quant_kernel computes it, the weight-role columns of meta, and this rank's pieces quantised into its E4M3 shard
+// with the shared rounding code. End barrier: every rank's E4M3 shard is complete before anybody pulls from it.
+__global__ void __launch_bounds__(512) zero3_fp8_requant_kernel(const Zero3RequantArgs a, const CommCtl c, const uint32_t epoch) {
+  if (!grid_peer_barrier_start(c, epoch)) return;
+  uint32_t* mine = c.ctl[c.rank];
+  extern __shared__ float s_scale[];   // [n_w]
+  __shared__ float smax[16];
+  const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x, nthr = (long long)gridDim.x * blockDim.x;
+  const __nv_bfloat16* w16 = static_cast<const __nv_bfloat16*>(a.w16);
+  // ---- phase 1: partial amax per weight over this rank's pieces
+  for (int p = 0; p < a.n_pieces; ++p) {
+    const long long off = a.pieces[3 * p], n8 = a.pieces[3 * p + 1] / 8;
+    const uint4* src = reinterpret_cast<const uint4*>(w16 + off);
+    float am = 0.f;
+    for (long long i = tid; i < n8; i += nthr) {
+      float f[8];
+      unpack8f(src[i], f);
+      am = amax8(f, am);
+    }
+    am = warp_max_f(am);
+    if ((threadIdx.x & 31) == 0) smax[threadIdx.x >> 5] = am;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float m = smax[0];
+      for (int w = 1; w < (blockDim.x >> 5); ++w) m = fmaxf(m, smax[w]);
+      if (m > 0.f) atomic_max_pos_f32(a.amax_local + a.pieces[3 * p + 2], m);
+    }
+    __syncthreads();
+  }
+  // ---- publish (last block), mid barrier, release the grid
+  if (grid_done(c)) {
+    for (int j = threadIdx.x; j < a.n_w; j += blockDim.x) {
+      const float v = *reinterpret_cast<volatile float*>(a.amax_local + j);
+      for (int p = 0; p < c.n; ++p) {
+        float* dst = a.amax[p] + (long long)c.rank * a.n_w + j;
+        asm volatile("st.relaxed.sys.global.f32 [%0], %1;" ::"l"(dst), "f"(v) : "memory");
+      }
+      a.amax_local[j] = 0.f;   // ready for the next version
+    }
+    __syncthreads();
+    __threadfence_system();
+    if (threadIdx.x < c.n) {
+      st_release_sys(c.ctl[threadIdx.x] + CP_MID + c.rank, epoch);
+      if (!wait_flag_sys(mine + CP_MID + threadIdx.x, epoch, c.timeout_ns)) atomicOr(mine + CP_STATUS, 0x100u << threadIdx.x);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      __threadfence();
+      asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(mine + CP_GO2), "r"(epoch) : "memory");
+    }
+  }
+  if (threadIdx.x == 0) {
+    uint32_t v;
+    do {
+      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(mine + CP_GO2) : "memory");
+    } while (v < epoch);
+  }
+  __syncthreads();
+  // ---- phase 2: global amax -> scale (every weight: each rank computes with all of them), then this rank's pieces
+  const float* rows = a.amax[c.rank];
+  for (int j = threadIdx.x; j < a.n_w; j += blockDim.x) {
+    float m = 0.f;
+    for (int p = 0; p < c.n; ++p) {
+      float x;
+      asm volatile("ld.relaxed.sys.global.f32 %0, [%1];" : "=f"(x) : "l"(rows + (long long)p * a.n_w + j) : "memory");
+      m = fmaxf(m, x);
+    }
+    const float s = weight_scale(m, a.fmax);
+    s_scale[j] = s;
+    if (blockIdx.x == 0) {
+      const long long r = a.roles[j];
+      a.meta[r] = s;
+      a.meta[a.n_roles + r] = 1.0f / s;
+      a.meta[2 * a.n_roles + r] = m;
+    }
+  }
+  __syncthreads();
+  for (int p = 0; p < a.n_pieces; ++p) {
+    const long long off = a.pieces[3 * p], n8 = a.pieces[3 * p + 1] / 8;
+    const float s = s_scale[a.pieces[3 * p + 2]];
+    const uint4* src = reinterpret_cast<const uint4*>(w16 + off);
+    uint2* dst = reinterpret_cast<uint2*>(a.w8 + off);
+    for (long long i = tid; i < n8; i += nthr) {
+      float f[8];
+      unpack8f(src[i], f);
+      dst[i] = quant8<0>(f, s);
+    }
+  }
+  if (grid_done(c)) peer_barrier_end(c, epoch);
+}
+
 // ------------------------------------------------------------------------------------------ N1 + K11 + K12
 // Phase 1: every rank sums its shard of all gradient planes over NVLink (mean folded in), keeps the result in its own
 // plane and publishes the shard's squared norm to every rank. Mid barrier. Phase 2: clip coefficient from the global norm,
@@ -562,6 +660,12 @@ void zero3_reduce_launch(const ShardReduceArgs& a, const CommCtl& c, uint32_t ep
   zero3_reduce_kernel<<<grid, 512, 0, st>>>(a, c, epoch);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) throw std::runtime_error(std::string("zero3_reduce launch: ") + cudaGetErrorString(e));
+}
+void zero3_fp8_requant_launch(const Zero3RequantArgs& a, const CommCtl& c, uint32_t epoch, int num_sms, cudaStream_t st) {
+  if (a.n_w <= 0 || a.n_w > 12288) throw std::runtime_error("zero3_fp8_requant: 1..12288 weight matrices (one fp32 scale each in shared memory)");
+  zero3_fp8_requant_kernel<<<sm_count(num_sms), 512, sizeof(float) * a.n_w, st>>>(a, c, epoch);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) throw std::runtime_error(std::string("zero3_fp8_requant launch: ") + cudaGetErrorString(e));
 }
 
 void set_wsum(uint32_t* ctl, float w, bool zero_sums, cudaStream_t st) { set_wsum_kernel<<<1, 1, 0, st>>>(ctl, w, zero_sums ? 1 : 0); }

@@ -76,6 +76,23 @@ struct ShardReduceArgs {
 };
 void zero3_reduce_launch(const ShardReduceArgs& a, const CommCtl& c, uint32_t epoch, int num_sms, cudaStream_t st);
 
+// ZeRO-3 under amp_fp8: the E4M3 copy of every block weight matrix, quantised once per parameter version by the owners of its
+// pieces with the tensor's GLOBAL amax (per-tensor current scaling, the same bytes the unsharded engine produces).
+struct Zero3RequantArgs {
+  const void* w16;                // this rank's bf16 shard
+  uint8_t* w8;                    // this rank's E4M3 shard (same element offsets)
+  const long long* pieces;        // [n_pieces][3]: shard offset, numel (both multiples of 8), weight slot
+  int n_pieces;
+  int n_w;                        // number of weight matrices (slots)
+  float* amax_local;              // [n_w] this rank's partial amax; zero between launches (the kernel leaves it zeroed)
+  float* amax[MAX_PEERS];         // every rank's amax plane [world][n_w]: row r is written by rank r
+  float* meta;                    // the engine's fp8 scaling state [3][n_roles]: scale, 1/scale, amax
+  long long n_roles;
+  const int* roles;               // [n_w] weight slot -> role column of meta
+  float fmax;                     // largest finite E4M3 value
+};
+void zero3_fp8_requant_launch(const Zero3RequantArgs& a, const CommCtl& c, uint32_t epoch, int num_sms, cudaStream_t st);
+
 void ddp_zero_step_launch(const ZeroStepArgs& a, const CommCtl& c, uint32_t epoch, float* out_norm, int num_sms, cudaStream_t st);
 void fed_round_launch(const FedRoundArgs& a, const CommCtl& c, uint32_t epoch, int num_sms, cudaStream_t st);
 void ddp_allreduce_launch(const AllReduceArgs& a, const CommCtl& c, uint32_t epoch, float* out_norm, int num_sms, cudaStream_t st);

@@ -21,6 +21,7 @@
 #include <string>
 
 #include "fp8_ops.h"
+#include "fp8_round.cuh"
 #include "ptx.cuh"
 
 namespace pb {
@@ -31,27 +32,6 @@ __device__ __forceinline__ float warp_sum_f(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffff, v, o);
   return v;
-}
-__device__ __forceinline__ void unpack8f(const uint4& u, float (&f)[8]) {
-  float2 a = unpack_bf16(u.x), b = unpack_bf16(u.y), c = unpack_bf16(u.z), d = unpack_bf16(u.w);
-  f[0] = a.x, f[1] = a.y, f[2] = b.x, f[3] = b.y, f[4] = c.x, f[5] = c.y, f[6] = d.x, f[7] = d.y;
-}
-template <int FMT>
-__device__ __forceinline__ uint2 quant8(const float (&f)[8], float s) {
-  uint2 o;
-  if (FMT == 0) {
-    o.x = pack_e4m3x4(f[0] * s, f[1] * s, f[2] * s, f[3] * s);
-    o.y = pack_e4m3x4(f[4] * s, f[5] * s, f[6] * s, f[7] * s);
-  } else {
-    o.x = pack_e5m2x4(f[0] * s, f[1] * s, f[2] * s, f[3] * s);
-    o.y = pack_e5m2x4(f[4] * s, f[5] * s, f[6] * s, f[7] * s);
-  }
-  return o;
-}
-__device__ __forceinline__ float amax8(const float (&f)[8], float m) {
-#pragma unroll
-  for (int k = 0; k < 8; ++k) m = fmaxf(m, fabsf(f[k]));
-  return m;
 }
 
 // ------------------------------------------------------------------ LayerNorm forward -> E4M3 (one warp per row)
@@ -221,7 +201,7 @@ __global__ void __launch_bounds__(256) seg_quant_kernel(const __nv_bfloat16* __r
                                                          float* __restrict__ scale, float* __restrict__ scale_inv, float fmax) {
   const long long off = seg[2 * blockIdx.y], n8 = seg[2 * blockIdx.y + 1] / 8;
   const float a = amax[blockIdx.y];
-  const float s = (a > 0.f && a < 3.0e38f) ? fmax / a : 1.0f;
+  const float s = weight_scale(a, fmax);
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     scale[blockIdx.y] = s;
     scale_inv[blockIdx.y] = 1.0f / s;

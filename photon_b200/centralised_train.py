@@ -88,7 +88,8 @@ def run_centralised(cfg: Any, *, device: torch.device | None = None, rank: int |
 
                 # fsdp_config FULL_SHARD on a model whose replicated state would crowd the GPU: parameters, gradients and
                 # optimizer state all live as 1/world shards (ZeRO-3); smaller models keep the faster fused ZeRO-1 step
-                grad_comm = NvlZero3Comm(lay, int(cfg["llm_config"]["model"]["n_layers"]), rank=rank, world_size=world_size, device=device)
+                grad_comm = NvlZero3Comm(lay, int(cfg["llm_config"]["model"]["n_layers"]), rank=rank, world_size=world_size, device=device,
+                                         fp8=cfg["llm_config"].get("precision", "amp_bf16") == "amp_fp8")
                 print(f"[centralised_train] full parameter sharding over {world_size} GPUs "
                       f"({lay.n_params / 1e9:.2f} B parameters, {16 * grad_comm.plan.shard_len / 2**30:.1f} GiB of state per GPU)", flush=True)
             else:

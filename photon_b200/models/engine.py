@@ -111,7 +111,8 @@ class B200Engine:
                  shadow_storage: torch.Tensor | None = None, zero3: Any = None) -> None:
         """``zero3``: a :class:`photon_b200.parallel.zero3.NvlZero3Comm` — full parameter sharding: this rank keeps 1/world of the
         masters / gradients / bf16 weights, block weights are pulled into two rotating buffers one block ahead of the compute
-        stream and every block's gradient is reduce-scattered right after its backward (ref: fsdp_config FULL_SHARD)."""
+        stream and every block's gradient is reduce-scattered right after its backward (ref: fsdp_config FULL_SHARD). Under
+        ``amp_fp8`` it must be built with ``fp8=True``: the block weights then travel as E4M3 (see :meth:`_init_fp8`)."""
         self.cfg = cfg
         self.device = torch.device(device)
         if self.device.type != "cuda":
@@ -123,13 +124,14 @@ class B200Engine:
         ops.ext()  # fail loudly if the extension is missing
         self.precision = precision
         self.zero3 = zero3
-        if zero3 is not None and precision != "amp_bf16":
-            raise NotImplementedError("full parameter sharding runs in amp_bf16 (the fp8 weight copies are quantised from a resident bf16 plane)")
         kernels = dict(kernels or {})
         # amp_fp8 (ref: scripts/centralised_training.sh:91, Composer amp_fp8 -> TransformerEngine): the four GEMMs of every block
         # and their dgrad / wgrad run on fp8 wgmma (E4M3 activations / weights, E5M2 gradients, per-tensor
         # scaling, fp32 accumulation); LayerNorm, attention, residuals, LM head, loss and optimizer stay bf16 / fp32
         self.fp8 = precision == "amp_fp8"
+        if zero3 is not None and bool(getattr(zero3, "fp8", False)) != self.fp8:
+            raise ValueError(f"precision={precision} needs NvlZero3Comm(..., fp8={self.fp8}): block units are gathered as "
+                             f"{'E4M3' if self.fp8 else 'bf16'}")
         self.attn_mode = "torch" if kernels.get("attention", "auto") == "torch" else "b200"
         # kernels.cuda_graph: the ~330 launches of one microbatch are captured once per (batch, seq, loss scaling) and
         # replayed (the schedule is static: preallocated workspace, TMA descriptors baked into the launches)
@@ -288,7 +290,11 @@ class B200Engine:
 
         Frozen matrices never change: they are quantised once, whenever their values are set (:meth:`_frozen_updated`), into a
         plane at the frozen layout's offsets, with a transposed (K-major) copy next to it that their dgrad GEMMs read directly.
-        Their weight roles come after the trainable ones, so each group is one contiguous role range."""
+        Their weight roles come after the trainable ones, so each group is one contiguous role range.
+
+        Under full parameter sharding no rank holds whole matrices: the communicator quantises them once per parameter version
+        (every parameter write ends in ``params_changed``), each owner its pieces with the tensor's global amax, and gathers the
+        E4M3 bytes. The weight views point into its rotating E4M3 unit buffers and the prologue re-quantises nothing."""
         L, lay, dev = self.cfg.n_layers, self.flat.layout, self.device
         self._n_dyn = len(self._DYN_ROLES) * L
         n_roles = self._n_dyn + len(self._W_ROLES) * L
@@ -298,8 +304,9 @@ class B200Engine:
         self.fp8_fmax = torch.tensor([ops.FP8_MAX[0 if j < 4 else 1] for _ in range(L) for j in range(8)], dtype=torch.float32, device=dev)
         self.fp8_pos = torch.zeros(1, dtype=torch.int32, device=dev)
         self.fp8_margin_mult = float(2.0 ** margin)
-        flay = self.frozen_layout
-        self.w8 = torch.zeros(lay.total, dtype=torch.uint8, device=dev)      # E4M3 weights at the flat layout's offsets
+        flay, z = self.frozen_layout, self.zero3
+        # E4M3 weights at the flat layout's offsets (under full sharding: the communicator's gathered units instead)
+        self.w8 = torch.zeros(lay.total, dtype=torch.uint8, device=dev) if z is None else None
         self.w8f = torch.zeros(flay.total, dtype=torch.uint8, device=dev) if flay is not None else None   # ... at the frozen layout's
         seg, fseg, order, self.w8_views, self.w8t_views = [], [], [], [], []
         for i in range(L):
@@ -312,16 +319,24 @@ class B200Engine:
         for r, (i, key, n) in enumerate(seg + fseg):
             self._w_role[(i, key)] = self._n_dyn + r
         for i, key, n in seg:
-            self.w8_views[i][key] = lay.view(self.w8, n)
+            self.w8_views[i][key] = lay.view(self.w8, n) if z is None else z.weight8(n)
         for i, key, n in fseg:
             self.w8_views[i][key] = flay.view(self.w8f, n)
             N, K = flay.shapes[flay.index(n)]
             self.w8t_views[i][key] = torch.empty(K, N, dtype=torch.uint8, device=dev)   # W^T: the dgrad GEMM's K-major B operand
         table = lambda lo, s: torch.tensor([(lo.offsets[lo.index(n)], lo.numels[lo.index(n)]) for _, _, n in s],  # noqa: E731
                                            dtype=torch.int64, device=dev).reshape(-1, 2)
-        self.w8_seg = table(lay, seg)
         self.w8f_seg = table(flay, fseg) if fseg else None
-        self._n_w8 = len(seg)
+        if z is None:
+            self.w8_seg = table(lay, seg)
+            self._n_w8 = len(seg)
+        else:
+            slot = {n: j for j, n in enumerate(z.plan.weight_names)}
+            roles = [0] * len(slot)
+            for i, key, n in seg:
+                roles[slot[n]] = self._w_role[(i, key)]
+            z.attach_fp8(self.fp8_meta, roles)   # quantised from now on by every params_changed (the first one ends __init__)
+            self.w8_seg, self._n_w8 = None, 0
         self._fp8_calibrated = False
 
     def _role(self, name: str, layer: int) -> int:
@@ -354,6 +369,9 @@ class B200Engine:
             self._fp8_calibrated = bool(sd.get("calibrated", True))
             if self.w8f_seg is not None:   # the frozen E4M3 bytes must stay paired with their (current-scaling) weight scales
                 self._fp8_quantize_frozen()
+            if self.zero3 is not None:     # likewise the sharded E4M3 weights (a collective: every rank loads the state)
+                self.zero3.before_param_write()
+                self.zero3.params_changed()
 
     # ---------------------------------------------------------------- workspace
     def _workspace(self, b: int, S: int) -> dict[str, Any]:

@@ -30,7 +30,8 @@ import torch.distributed as dist
 
 from photon_b200 import ops
 
-_DT = {torch.float32: ("float32", 4), torch.bfloat16: ("bfloat16", 2), torch.float64: ("float64", 8), torch.int32: ("int32", 4)}
+_DT = {torch.float32: ("float32", 4), torch.bfloat16: ("bfloat16", 2), torch.float64: ("float64", 8), torch.int32: ("int32", 4),
+       torch.uint8: ("uint8", 1)}
 _ALIGN = 4096
 
 

@@ -20,6 +20,13 @@ its gradient is reduce-scattered right after. Here, on one NVSwitch domain:
 
 The 1-D parameters (LayerNorm gains, biases: < 0.1 % of the model) are needed in fp32 by the normalisation kernels: they are pulled
 once per optimizer step from their owners' fp32 planes into a small resident buffer.
+
+Under ``precision: amp_fp8`` (``NvlZero3Comm(..., fp8=True)``) the block GEMMs read E4M3 weights, so the block units are gathered
+as E4M3 bytes (half the bf16 traffic) and no bf16 block buffers exist. Every parameter write already ends in
+:meth:`NvlZero3Comm.params_changed`; there one ``zero3_fp8_requant_kernel`` per parameter version exchanges every block matrix's
+amax over the ranks and lets each owner quantise its pieces of the matrix into an E4M3 shard plane, with the scale the unsharded
+engine would compute from the whole tensor (bitwise the same bytes and scales). The embeddings / final norm and the 1-D
+parameters are gathered as without fp8.
 """
 from __future__ import annotations
 
@@ -35,6 +42,10 @@ from photon_b200.utils.flat import FlatLayout
 
 def _round_up(x: int, m: int) -> int:
     return (x + m - 1) // m * m
+
+
+# the weight matrices of every block, in the engine's weight-role order (the four fp8 GEMMs of a block)
+BLOCK_MATRICES = ("attn.Wqkv.weight", "attn.out_proj.weight", "ffn.up_proj.weight", "ffn.down_proj.weight")
 
 
 @dataclass(frozen=True)
@@ -143,12 +154,39 @@ class UnitPlan:
                 pos, left, dst = pos + k, left - k, dst + k
         return out
 
-    def bytes_per_rank(self, n_moments: int = 2) -> dict[str, int]:
-        """Persistent + transient device bytes of one rank (the memory table in DESIGN.md)."""
+    # -- block weight matrices (amp_fp8: their E4M3 copies are quantised piecewise by the owners) --------
+    @property
+    def weight_names(self) -> list[str]:
+        """Block weight matrices in slot order: block by block, :data:`BLOCK_MATRICES` within a block."""
+        return [f"transformer.blocks.{i}.{m}" for i in range(self.n_layers) for m in BLOCK_MATRICES]
+
+    def weight_pieces(self, rank: int) -> list[tuple[int, int, int]]:
+        """(offset in ``rank``'s shard, numel, weight slot) of every non-empty piece of every block weight matrix inside that
+        rank's slices. A matrix meets one slice in at most one contiguous piece; offsets and lengths are multiples of 8 (the
+        kernel moves 8 elements per vector access)."""
+        out = []
+        for j, name in enumerate(self.weight_names):
+            u, rel, n = self.rel(name)
+            un = self.units[u]
+            if rel % 8 or n % 8:
+                raise ValueError(f"{name}: offset / size must be multiples of 8 for the E4M3 weight shards")
+            lo, hi = max(rel, rank * un.per), min(rel + n, (rank + 1) * un.per)
+            if hi > lo:
+                out.append((un.off + lo - rank * un.per, hi - lo, j))
+        return out
+
+    def bytes_per_rank(self, n_moments: int = 2, fp8: bool = False) -> dict[str, int]:
+        """Persistent + transient device bytes of one rank (the memory table in DESIGN.md). ``fp8``: the block units travel as
+        E4M3 (no bf16 block buffers) and the E4M3 shard plane, the amax planes and this rank's partial amax are added."""
         S = self.shard_len
-        return {"masters_fp32": 4 * S, "bf16_copy": 2 * S, "grad_shard_fp32": 4 * S, "moments_fp32": 4 * n_moments * S,
-                "unit_weight_buffers_bf16": 2 * 2 * self.max_block_span + 2 * self.rest_span,
-                "grad_staging_fp32": 4 * 2 * self.max_block_span + 4 * self.rest_span, "small_fp32": 4 * self.small_len}
+        out = {"masters_fp32": 4 * S, "bf16_copy": 2 * S, "grad_shard_fp32": 4 * S, "moments_fp32": 4 * n_moments * S,
+               "unit_weight_buffers_bf16": 2 * 2 * self.max_block_span + 2 * self.rest_span,
+               "grad_staging_fp32": 4 * 2 * self.max_block_span + 4 * self.rest_span, "small_fp32": 4 * self.small_len}
+        if fp8:
+            n_w = len(self.weight_names)
+            out.update(unit_weight_buffers_bf16=2 * self.rest_span, e4m3_shard=S, unit_weight_buffers_e4m3=2 * self.max_block_span,
+                       amax_fp32=4 * (self.world_size + 1) * n_w)
+        return out
 
 
 class ShardedFlat:
@@ -185,23 +223,31 @@ class ShardedFlat:
 
 
 class NvlZero3Comm:
-    """Arena, buffers, streams and the gather / reduce schedule of one rank. The engine asks for views (``weight`` / ``small`` /
-    ``grad``) once at bind time and calls ``acquire`` / ``prefetch`` / ``reduce`` around every block."""
+    """Arena, buffers, streams and the gather / reduce schedule of one rank. The engine asks for views (``weight`` / ``weight8`` /
+    ``small`` / ``grad``) once at bind time and calls ``acquire`` / ``prefetch`` / ``reduce`` around every block."""
 
     zero3 = True
 
     def __init__(self, layout: FlatLayout, n_layers: int, *, rank: int, world_size: int, device: torch.device | int | None = None,
-                 group: Any = None) -> None:
+                 group: Any = None, fp8: bool = False) -> None:
+        """``fp8``: the engine runs ``precision: amp_fp8`` — block units are gathered as E4M3 from a shard plane that
+        :meth:`params_changed` requantises (after :meth:`attach_fp8`), instead of as bf16."""
         from photon_b200 import ops
         from photon_b200.parallel.symm import SymmArena
 
         self.ext = ops.ext()
         self.plan = UnitPlan(layout, n_layers, world_size)
         self.rank, self.world_size, self.group = int(rank), int(world_size), group
+        self.fp8 = bool(fp8)
         pl = self.plan
-        self.arena = SymmArena({"p32": (pl.shard_len, torch.float32), "w16": (pl.shard_len, torch.bfloat16),
-                                "gs0": (pl.max_block_span, torch.float32), "gs1": (pl.max_block_span, torch.float32),
-                                "gsr": (pl.rest_span, torch.float32)}, rank=rank, world_size=world_size, device=device, group=group)
+        planes = {"p32": (pl.shard_len, torch.float32), "w16": (pl.shard_len, torch.bfloat16),
+                  "gs0": (pl.max_block_span, torch.float32), "gs1": (pl.max_block_span, torch.float32),
+                  "gsr": (pl.rest_span, torch.float32)}
+        if self.fp8:
+            self._pieces = pl.weight_pieces(self.rank)
+            self.n_weights = len(pl.weight_names)
+            planes.update(w8=(pl.shard_len, torch.uint8), amax=(self.world_size * self.n_weights, torch.float32))
+        self.arena = SymmArena(planes, rank=rank, world_size=world_size, device=device, group=group)
         self.dev = torch.device("cuda", self.arena.devices[0])
         ar = self.arena
         self.p32, self.w16 = ar.plane("p32"), ar.plane("w16")
@@ -209,7 +255,17 @@ class NvlZero3Comm:
         self.gstage = [ar.plane("gs0"), ar.plane("gs1")]
         self.gstage_rest = ar.plane("gsr")
         self.gshard = torch.zeros(pl.shard_len, dtype=torch.float32, device=self.dev)
-        self.wbuf = [torch.zeros(pl.max_block_span, dtype=torch.bfloat16, device=self.dev) for _ in range(2)]
+        self.wbuf: list[torch.Tensor] | None = None         # bf16 block units (without fp8)
+        self.wbuf8: list[torch.Tensor] | None = None        # E4M3 block units (fp8)
+        self._fp8_meta: torch.Tensor | None = None
+        if self.fp8:
+            self.w8, self.amax = ar.plane("w8"), ar.plane("amax")
+            self.w8.zero_(), self.amax.zero_()
+            self.amax_local = torch.zeros(self.n_weights, dtype=torch.float32, device=self.dev)
+            self.pieces = torch.tensor(self._pieces, dtype=torch.int64).reshape(-1, 3).to(self.dev)
+            self.wbuf8 = [torch.zeros(pl.max_block_span, dtype=torch.uint8, device=self.dev) for _ in range(2)]
+        else:
+            self.wbuf = [torch.zeros(pl.max_block_span, dtype=torch.bfloat16, device=self.dev) for _ in range(2)]
         self.wrest = torch.zeros(pl.rest_span, dtype=torch.bfloat16, device=self.dev)
         self.small32 = torch.zeros(pl.small_len, dtype=torch.float32, device=self.dev)
         self._small_copies = pl.small_copies()
@@ -221,10 +277,38 @@ class NvlZero3Comm:
         self.norm = torch.zeros(1, dtype=torch.float32, device=self.dev)
 
     # ------------------------------------------------------------------ views for the engine
-    def weight(self, name: str) -> torch.Tensor:
+    def weight(self, name: str) -> torch.Tensor | None:
+        """bf16 view of a gathered weight; None for a block matrix under fp8 (its GEMMs read :meth:`weight8`)."""
         u, rel, n = self.plan.rel(name)
+        if u != self.plan.rest and self.wbuf is None:
+            return None
         buf = self.wrest if u == self.plan.rest else self.wbuf[u % 2]
         return buf[rel: rel + n].view(self.plan.layout.shapes[self.plan.layout.index(name)])
+
+    def weight8(self, name: str) -> torch.Tensor:
+        """E4M3 view of a gathered block weight matrix (fp8 only)."""
+        u, rel, n = self.plan.rel(name)
+        if self.wbuf8 is None or u == self.plan.rest:
+            raise ValueError(f"{name}: E4M3 weights exist for the block matrices of an fp8 communicator only")
+        return self.wbuf8[u % 2][rel: rel + n].view(self.plan.layout.shapes[self.plan.layout.index(name)])
+
+    def attach_fp8(self, meta: torch.Tensor, roles: Sequence[int]) -> None:
+        """The engine's fp8 scaling state ``meta`` [3, n_roles] and the role column of every weight slot
+        (:attr:`UnitPlan.weight_names` order): from now on :meth:`params_changed` requantises the weights and writes their
+        scale / 1/scale / amax there."""
+        if not self.fp8:
+            raise ValueError("attach_fp8 needs NvlZero3Comm(..., fp8=True)")
+        if len(roles) != self.n_weights:
+            raise ValueError(f"expected {self.n_weights} weight roles, got {len(roles)}")
+        self._fp8_meta = meta
+        self._roles = torch.tensor(list(roles), dtype=torch.int32, device=self.dev)
+
+    def requantize(self) -> None:
+        """One ``zero3_fp8_requant_kernel``: every rank's E4M3 shard and the weight scales from the current bf16 shards (a
+        collective: every rank calls it, in the same order as the other collectives of this communicator)."""
+        ar = self.arena
+        self.ext.zero3_fp8_requant(ar.ctl_ptrs(), ar.rank, ar.devices[0], ar.next_epoch(), self.w16, self.w8, self.pieces,
+                                   self.amax_local, ar.ptrs("amax"), self._fp8_meta, self._roles)
 
     def small(self, name: str) -> torch.Tensor:
         i, o = self.plan.small_index[name], self.plan.small_offsets[name]
@@ -247,7 +331,10 @@ class NvlZero3Comm:
         k, un = u % 2, self.plan.units[u]
         self.side.wait_stream(torch.cuda.current_stream(self.dev))
         with torch.cuda.stream(self.side):
-            self._pull(self.wbuf[k], "w16", un.off, un.per, 2)
+            if self.fp8:
+                self._pull(self.wbuf8[k], "w8", un.off, un.per, 1)
+            else:
+                self._pull(self.wbuf[k], "w16", un.off, un.per, 2)
             ev = torch.cuda.Event()
             ev.record(self.side)
         self.resident[k], self._ready[k] = u, ev
@@ -296,8 +383,12 @@ class NvlZero3Comm:
         self.barrier()
 
     def params_changed(self) -> None:
-        """Every rank's new shard is in place before anybody pulls from it; local copies of the old version are dropped."""
-        self.barrier()
+        """Every rank's new shard is in place before anybody pulls from it; local copies of the old version are dropped. Under
+        fp8 (once attached) the requantisation kernel takes the place of the barrier: it ends with the same one."""
+        if self._fp8_meta is not None:
+            self.requantize()
+        else:
+            self.barrier()
         self.resident, self._ready = [None, None], [None, None]
         self._rest_valid = False
         self.version += 1
