@@ -463,9 +463,6 @@ void set_smem(K kern, int bytes) {
   if (e != cudaSuccess) throw std::runtime_error(std::string("attention smem attr: ") + cudaGetErrorString(e));
 }
 
-float* g_dq_acc = nullptr;
-size_t g_dq_acc_bytes = 0;
-
 }  // namespace
 
 void attention_fwd_launch(const void* qkv, void* out, float* lse, int B, int S, int H, int dh, float scale, bool causal, int num_sms,
@@ -492,20 +489,14 @@ void attention_fwd_launch(const void* qkv, void* out, float* lse, int B, int S, 
   if (e != cudaSuccess) throw std::runtime_error(std::string("attention fwd launch: ") + cudaGetErrorString(e));
 }
 
-int attention_bwd_launch(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta, int B, int S, int H,
-                         int dh, float scale, bool causal, int num_sms, cudaStream_t st, const float* alibi_slopes) {
+int attention_bwd_launch(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta, float* dq_acc,
+                         int B, int S, int H, int dh, float scale, bool causal, int num_sms, cudaStream_t st, const float* alibi_slopes) {
   if (S % 128) throw std::runtime_error("photon_b200 attention: sequence length must be a multiple of 128");
   if (dh != 64 && dh != 128) throw std::runtime_error("photon_b200 attention backward: d_head must be 64 or 128");
   const int sms = num_sms > 0 ? num_sms : 132;
   const int d = H * dh;
   const long long rows = (long long)B * S;
-  const size_t need = size_t(rows) * d * sizeof(float);
-  if (need > g_dq_acc_bytes) {
-    if (g_dq_acc) cudaFree(g_dq_acc);
-    if (cudaMalloc(&g_dq_acc, need) != cudaSuccess) throw std::runtime_error("attention bwd: dq accumulator allocation failed");
-    g_dq_acc_bytes = need;
-  }
-  cudaMemsetAsync(g_dq_acc, 0, need, st);
+  cudaMemsetAsync(dq_acc, 0, size_t(rows) * d * sizeof(float), st);
   {
     const long long n8 = rows * H * (dh / 8);
     const int blocks = int(std::min<long long>((n8 + 255) / 256, sms * 16));
@@ -520,14 +511,14 @@ int attention_bwd_launch(const void* qkv, const void* out, const void* dout, con
     static bool once = (set_smem(attn_bwd_kernel<DHV, AL>, BwdCfg<DHV>::SMEM), true);                                \
     (void)once;                                                                                                      \
     attn_bwd_kernel<DHV, AL><<<grid, 384, BwdCfg<DHV>::SMEM, st>>>(tmKV, tmQ, tmDO, lse, delta, (__nv_bfloat16*)dqkv, S, H, scale, \
-                                                                  causal ? 1 : 0, g_dq_acc, alibi_slopes);           \
+                                                                  causal ? 1 : 0, dq_acc, alibi_slopes);             \
   }
   if (dh == 64 && !alibi_slopes) PB_BWD(64, false)
   else if (dh == 64) PB_BWD(64, true)
   else if (!alibi_slopes) PB_BWD(128, false)
   else PB_BWD(128, true)
 #undef PB_BWD
-  attn_bwd_dq_convert_kernel<<<sms * 8, 256, 0, st>>>(g_dq_acc, (__nv_bfloat16*)dqkv, rows, d, scale);
+  attn_bwd_dq_convert_kernel<<<sms * 8, 256, 0, st>>>(dq_acc, (__nv_bfloat16*)dqkv, rows, d, scale);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) throw std::runtime_error(std::string("attention bwd launch: ") + cudaGetErrorString(e));
   return 3;

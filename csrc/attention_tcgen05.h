@@ -8,9 +8,11 @@ namespace pb {
 // alibi_slopes: optional fp32 [H] (score += slope_h * (key - query)), nullptr = off
 void attention_fwd_launch(const void* qkv, void* out, float* lse, int B, int S, int H, int dh, float scale, bool causal, int num_sms,
                           cudaStream_t st, const float* alibi_slopes = nullptr);
-// returns the number of kernels launched. dqkv: bf16 [B,S,3*H*dh]; delta: fp32 scratch [B,H,S]
-int attention_bwd_launch(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta, int B, int S,
-                         int H, int dh, float scale, bool causal, int num_sms, cudaStream_t st, const float* alibi_slopes = nullptr);
+// returns the number of kernels launched. dqkv: bf16 [B,S,3*H*dh]; delta: fp32 scratch [B,H,S]; dq_acc: fp32 scratch [B*S, H*dh],
+// owned by the caller (zeroed here on st, then read by the last kernel on st)
+int attention_bwd_launch(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta, float* dq_acc,
+                         int B, int S, int H, int dh, float scale, bool causal, int num_sms, cudaStream_t st,
+                         const float* alibi_slopes = nullptr);
 // in-place rotary embedding on the q and k thirds of qkv [T, 3*H*dh] (rotate-half); inverse = transposed rotation
 void rope_launch(void* qkv, const float* cosT, const float* sinT, long long T, int S, int H, int dh, bool inverse, cudaStream_t st);
 

@@ -267,18 +267,28 @@ void fp8_update_scales(Tensor& meta, Tensor& hist, const Tensor& fmax, Tensor& p
 }
 
 // ---------------------------------------------------------------------------------- attention
+// shapes shared by the forward and the backward: qkv [B,S,3d]; o-like tensors [B,S,d]; row statistics fp32 [B,H,S]
+void check_attention_args(const Tensor& qkv, const Tensor& out, const Tensor& lse, int n_heads, bool causal,
+                          const c10::optional<Tensor>& alibi_slopes) {
+  TORCH_CHECK(qkv.dim() == 3 && qkv.is_contiguous() && qkv.size(2) % 3 == 0, "qkv must be contiguous [B,S,3*d]");
+  const int64_t B = qkv.size(0), S = qkv.size(1), d = qkv.size(2) / 3;
+  TORCH_CHECK(n_heads > 0 && d % n_heads == 0, "attention: d = ", d, " is not a multiple of n_heads = ", n_heads);
+  TORCH_CHECK(out.is_contiguous() && out.sizes() == at::IntArrayRef({B, S, d}), "out must be contiguous [B,S,d]");
+  TORCH_CHECK(lse.is_contiguous() && lse.sizes() == at::IntArrayRef({B, int64_t(n_heads), S}), "lse must be contiguous float32 [B,H,S]");
+  if (alibi_slopes.has_value()) {
+    TORCH_CHECK(causal, "attention: ALiBi slopes are only supported with the causal mask");
+    check_f32(*alibi_slopes, "alibi_slopes");
+    TORCH_CHECK(alibi_slopes->numel() == n_heads && alibi_slopes->is_contiguous(), "alibi_slopes must be contiguous with n_heads elements");
+  }
+}
 void attention_fwd(const Tensor& qkv, Tensor& out, Tensor& lse, int n_heads, double scale, bool causal,
                    const c10::optional<Tensor>& alibi_slopes) {
   check_bf16(qkv, "qkv");
   check_bf16(out, "out");
   check_f32(lse, "lse");
-  TORCH_CHECK(qkv.dim() == 3 && qkv.is_contiguous(), "qkv must be contiguous [B,S,3*d]");
+  check_attention_args(qkv, out, lse, n_heads, causal, alibi_slopes);
   c10::cuda::CUDAGuard guard(qkv.device());
   const int B = int(qkv.size(0)), S = int(qkv.size(1)), d = int(qkv.size(2) / 3);
-  if (alibi_slopes.has_value()) {
-    check_f32(*alibi_slopes, "alibi_slopes");
-    TORCH_CHECK(alibi_slopes->numel() == n_heads, "alibi_slopes must have n_heads elements");
-  }
   pb::attention_fwd_launch(qkv.data_ptr(), out.data_ptr(), lse.data_ptr<float>(), B, S, n_heads, d / n_heads, float(scale), causal,
                            at::cuda::getCurrentDeviceProperties()->multiProcessorCount, stream_of(qkv),
                            alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr);
@@ -292,10 +302,17 @@ void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, con
   check_bf16(dqkv, "dqkv");
   check_f32(lse, "lse");
   check_f32(delta, "delta");
+  check_attention_args(qkv, out, lse, n_heads, causal, alibi_slopes);
+  TORCH_CHECK(dout.is_contiguous() && dout.sizes() == out.sizes(), "dout must be contiguous [B,S,d]");
+  TORCH_CHECK(delta.is_contiguous() && delta.sizes() == lse.sizes(), "delta must be contiguous float32 [B,H,S]");
+  TORCH_CHECK(dqkv.is_contiguous() && dqkv.sizes() == qkv.sizes(), "dqkv must be contiguous and shaped like qkv");
   c10::cuda::CUDAGuard guard(qkv.device());
   const int B = int(qkv.size(0)), S = int(qkv.size(1)), d = int(qkv.size(2) / 3);
+  // the fp32 dQ accumulator comes from the caching allocator on this stream: eagerly it is recycled in stream order, under
+  // CUDA-graph capture it comes from the graph's private pool and lives as long as the graph
+  Tensor dq_acc = at::empty({(int64_t)B * S, d}, qkv.options().dtype(at::kFloat));
   const int launched = pb::attention_bwd_launch(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr<float>(), dqkv.data_ptr(),
-                                                delta.data_ptr<float>(), B, S, n_heads, d / n_heads, float(scale), causal,
+                                                delta.data_ptr<float>(), dq_acc.data_ptr<float>(), B, S, n_heads, d / n_heads, float(scale), causal,
                                                 at::cuda::getCurrentDeviceProperties()->multiProcessorCount, stream_of(qkv),
                                                 alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr);
   g_launches += launched;

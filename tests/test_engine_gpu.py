@@ -127,6 +127,44 @@ def test_engine_cuda_graph_replay_matches_eager():
     assert b.launches_per_microbatch == a.launches_per_microbatch > 0
 
 
+def test_engine_graph_replay_after_a_larger_attention_backward():
+    """A captured graph keeps its own dQ accumulator: an attention backward at a larger shape elsewhere in the process,
+    between capture and replay, must not move or free the memory the graph's nodes point at."""
+    from photon_b200 import ops
+    from photon_b200.models.engine import B200Engine
+    from photon_b200.models.mpt import MPTConfig
+
+    cfg = MPTConfig(d_model=256, n_heads=4, n_layers=2, max_seq_len=256, vocab_size=2048, attn_impl="flash")
+    dev = torch.device("cuda", 0)
+    a = B200Engine(cfg, dev, "amp_bf16", {"cuda_graph": False}, seed=5)
+    b = B200Engine(cfg, dev, "amp_bf16", {"cuda_graph": True}, seed=5)
+    a.flat.zero_grad(), b.flat.zero_grad()
+    denom = float(cfg.max_seq_len - 1)
+    ids = torch.randint(0, cfg.vocab_size, (1, cfg.max_seq_len), device=dev)
+    a.fwd_bwd(ids, denom)
+    b.fwd_bwd(ids, denom)   # captures the b = 1 graph
+    assert len(b._graphs) == 1
+    # a larger attention backward: [8 x 2048] rows x 2048 columns of fp32 accumulator, 64x the engine's
+    B, S, H, dh = 8, 2048, 16, 128
+    qkv = torch.randn(B, S, 3 * H * dh, device=dev).bfloat16()
+    out = torch.empty(B, S, H * dh, dtype=torch.bfloat16, device=dev)
+    lse = torch.empty(B, H, S, device=dev)
+    ops.attention_fwd(qkv, out, lse, H, dh ** -0.5, True)
+    ops.attention_bwd(qkv, out, torch.randn_like(out), lse, torch.empty_like(qkv), torch.empty_like(lse), H, dh ** -0.5, True)
+    torch.cuda.synchronize()
+    del qkv, out, lse
+    for _ in range(2):   # replays of the b = 1 graph after it
+        ids = torch.randint(0, cfg.vocab_size, (1, cfg.max_seq_len), device=dev)
+        la, _ = a.fwd_bwd(ids, denom)
+        lb, _ = b.fwd_bwd(ids, denom)
+        torch.cuda.synchronize()
+        assert abs(float(la) - float(lb)) <= 1e-3 * abs(float(la)), (float(la), float(lb))
+    assert len(b._graphs) == 1
+    assert bool(torch.isfinite(b.flat.grads).all())
+    rel = ((a.flat.grads - b.flat.grads).norm() / a.flat.grads.norm()).item()
+    assert rel < 1e-3, rel
+
+
 def test_engine_d_head_128_runs_on_own_attention():
     """MPT-1B/3B/7B geometry (d_head = 128): forward and backward attention stay on the wgmma kernels."""
     from photon_b200.models.engine import B200Engine

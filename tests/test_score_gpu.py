@@ -30,39 +30,45 @@ def _layout(runs):
 @pytest.mark.parametrize("dh", [64, 128])
 @pytest.mark.parametrize("alibi", [False, True])
 def test_cache_attention_matches_fp32(dh, alibi):
+    """Every tile of the tile table against the fp64 oracle at its rows' own cache positions, bounded by the bf16 baseline of
+    the same tile (the max part per tile and head, the mean part over all rows). The query rows of a run are the slot's own
+    sequence at positions first_pos .. first_pos + n - 1."""
+    import attention_oracle as A
     from photon_b200 import ops
     from photon_b200.models.mpt import alibi_slopes
 
     H, S, Bm = 3, 2048, 6
     runs, N = _layout(RUNS)
-    g = torch.Generator(device=DEV).manual_seed(dh * 2 + alibi)
-    kc = torch.randn(Bm, H, S, dh, device=DEV, generator=g).bfloat16()
-    vc = torch.randn(Bm, H, S, dh, device=DEV, generator=g).bfloat16()
-    qkv = torch.randn(N, 3 * H * dh, device=DEV, generator=g).bfloat16()
     slopes = alibi_slopes(H).to(DEV) if alibi else None
     scale = 1.0 / math.sqrt(dh)
     tiles = ops.cache_tiles(runs, DEV)
     assert tiles.shape[0] == 1 + 1 + 1 + 1 + 2 + 4 + 1 + 1 + 1
-    out = torch.full((N, H * dh), SENTINEL, dtype=torch.bfloat16, device=DEV)
-    ops.cache_attention(qkv, kc, vc, tiles, out, H, scale, slopes)
-    again = torch.full_like(out, SENTINEL)
-    ops.cache_attention(qkv, kc, vc, tiles, again, H, scale, slopes)
-    torch.cuda.synchronize()
-    assert torch.equal(out, again), "two runs differ"
-    covered = torch.zeros(N, dtype=torch.bool)
-    for slot, r0, n, p in runs:
-        covered[r0: r0 + n] = True
-        q = qkv[r0: r0 + n, : H * dh].float().view(n, H, dh)
-        keys = torch.arange(p + n, device=DEV)
-        qpos = p + torch.arange(n, device=DEV)
-        s = torch.einsum("nhd,hkd->hnk", q, kc[slot, :, : p + n].float()) * scale
-        if alibi:
-            s = s + slopes[:, None, None] * (keys[None, None] - qpos[None, :, None]).float()
-        s = s.masked_fill(keys[None, None] > qpos[None, :, None], float("-inf"))
-        o = torch.einsum("hnk,hkd->nhd", s.softmax(-1), vc[slot, :, : p + n].float())
-        torch.testing.assert_close(out[r0: r0 + n].float().view(n, H, dh), o, rtol=2e-2, atol=2e-2,
-                                   msg=lambda m: f"run {(slot, n, p)}: {m}")
-    assert bool((out[~covered.to(DEV)] == SENTINEL).all()), "a row outside the tiles was written"
+    for case in ("normal", "peaked", "rising"):
+        seq, _ = A.make_inputs(case, Bm, S, H, dh, DEV, seed=dh * 2 + alibi)
+        _, k, v = A.split_heads(seq, H)
+        kc, vc = k.contiguous(), v.contiguous()
+        qkv = torch.randn(N, 3 * H * dh, device=DEV).bfloat16()
+        for slot, r0, n, p in runs:
+            qkv[r0: r0 + n] = seq[slot, p: p + n]
+        out = torch.full((N, H * dh), SENTINEL, dtype=torch.bfloat16, device=DEV)
+        ops.cache_attention(qkv, kc, vc, tiles, out, H, scale, slopes)
+        again = torch.full_like(out, SENTINEL)
+        ops.cache_attention(qkv, kc, vc, tiles, again, H, scale, slopes)
+        torch.cuda.synchronize()
+        assert torch.equal(out, again), "two runs differ"
+        covered = torch.zeros(N, dtype=torch.bool)
+        got, refs, bases = [], [], []
+        for slot, r0, n, p in tiles.tolist():
+            covered[r0: r0 + n] = True
+            q = qkv[r0: r0 + n, : H * dh].view(1, n, H, dh).transpose(1, 2)
+            kw = dict(causal=True, slopes=None if slopes is None else slopes.tolist(), q_pos=(p + torch.arange(n, device=DEV))[None],
+                      lengths=[p + n])
+            ks, vs = kc[slot: slot + 1], vc[slot: slot + 1]
+            refs.append(A.oracle(q, ks, vs, scale, **kw).o)
+            bases.append(A.baseline(q, ks, vs, scale, **kw).o)
+            got.append(out[r0: r0 + n].view(1, n, H, dh).transpose(1, 2))
+        A.check_tiles("cache o", got, refs, bases, case=f"{case}, runs {RUNS}")
+        assert bool((out[~covered.to(DEV)] == SENTINEL).all()), "a row outside the tiles was written"
 
 
 @pytest.mark.parametrize("use_rope", [False, True])
