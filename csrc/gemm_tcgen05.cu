@@ -4,8 +4,9 @@
 //     producer thread (its warpgroup hands its registers to the MMA warpgroups with setmaxnreg)
 //   * two MMA warpgroups, 64 rows of the 128 x 256 tile each: wgmma.mma_async (bf16: m64n256k16, fp8: m64n256k32) with the
 //     fp32 accumulators in registers; a stage is released as soon as the next stage's MMAs are issued (wait_group 1)
-//   * epilogue straight from the accumulator registers: bias / residual / GELU / dGELU / fp8 re-quantisation, bf16 or fp32
-//     stores (fp32 weight-gradient accumulation and split-K partials by red.global.add)
+//   * epilogue: bias / residual / GELU / dGELU / fp8 re-quantisation in registers, then stmatrix into a per-warpgroup 128B-swizzled
+//     staging buffer and TMA stores (cp.async.bulk.tensor) that drain while the next tile's mainloop runs; fp32 outputs (weight
+//     gradients, split-K partials) go straight from registers, accumulated by red.global.add
 //   * bf16 operands may be K-major ([rows,K] row-major) or MN-major ([K,rows] row-major) so forward, dgrad (B = W as stored)
 //     and wgrad (A = dY^T, B = X^T as stored) need no transposes; wgmma reads 8-bit operands K-major only, so an MN-major fp8
 //     operand is transposed into scratch first (transpose_u8)
@@ -35,7 +36,10 @@ constexpr int A_STAGE = BM * ROW_BYTES;   // 16 KiB
 constexpr int B_STAGE = BN * ROW_BYTES;   // 32 KiB
 constexpr int STAGE_BYTES = A_STAGE + B_STAGE;
 constexpr int STAGES = 4;
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;
+// epilogue staging: per MMA warpgroup two 8 KiB slots, each one TMA store box of 64 rows x 128 bytes
+constexpr int EPI_SLOT = 64 * 128;
+constexpr int EPI_WG_BYTES = 2 * EPI_SLOT;
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * EPI_WG_BYTES + 256 + 1024;
 static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KiB dynamic shared memory of sm_90");
 constexpr int NUM_THREADS = 384;   // warpgroup 0: TMA producer (one thread); warpgroups 1, 2: MMA + epilogue
 
@@ -45,10 +49,8 @@ struct Params {
   const float* bias;            // [N] fp32 or nullptr
   const __nv_bfloat16* aux;     // residual (EPI_RESIDUAL) or pre-activation z (EPI_DGELU) or multiplier (EPI_MUL)
   long long ld_aux;             // row stride of aux, elements
-  void* d;                      // primary output (bf16, or fp32 for EPI_F32)
+  float* d;                     // EPI_F32 output (the other outputs are written through their tensor maps)
   long long ldd;
-  __nv_bfloat16* d2;            // second output of the two-output epilogues
-  long long ldd2;
   int accumulate;               // EPI_F32: reduce-add into D instead of overwrite
   float alpha;                  // scale applied to the accumulator before the epilogue
   int splits, kb_per_split;     // split-K (EPI_F32 + accumulate): work item = (tile, k-range)
@@ -58,8 +60,6 @@ struct Params {
   const float* sinv_a;
   const float* sinv_b;
   // EPI_GELU_GRAD_Q8: the activation leaves as E4M3 (scaled by *out_scale, amax recorded) for the next fp8 GEMM
-  uint8_t* d8;
-  long long ld_d8;
   const float* out_scale;
   float* out_amax;
 };
@@ -74,18 +74,25 @@ __device__ __forceinline__ uint16_t pack_e4m3x2(float a, float b) {
 // CL = 2: a cluster of two CTAs computes two M-adjacent 128x256 tiles that share their B tile: each CTA loads 128 of the 256
 //         B rows and multicasts them into both CTAs' shared memory, halving the L2 -> SM traffic of B. A stage may only be
 //         refilled when the MMA warpgroups of BOTH CTAs released it, so every consumer warp arrives on both empty barriers.
+//
+// Outputs other than fp32 leave through TMA: tmD is D (bf16) or, for EPI_GELU_GRAD_Q8, the E4M3 output D8; tmD2 is D2. Their dims
+// are the logical [M, N], so the TMA clips the M and N tails.
 template <int A_MN, int B_MN, int EPI, int CL, int F8>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Params p) {
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmD,
+            const __grid_constant__ CUtensorMap tmD2, const Params p) {
   constexpr int BK = F8 ? 128 : 64;            // K elements per stage (128 bytes per row)
   constexpr int MNC = F8 ? 128 : 64;           // MN elements in one 128-byte row of an MN-major tile
   constexpr int CHUNK = BK * ROW_BYTES;        // bytes of one MN-major chunk: BK k-rows of 128 bytes
+  constexpr bool TWO_OUT = EPI == EPI_GELU_DUAL || EPI == EPI_GELU_GRAD || EPI == EPI_GELU_GRAD_Q8;
+  constexpr bool AUX = EPI == EPI_RESIDUAL || EPI == EPI_DGELU || EPI == EPI_MUL;
   static_assert(!F8 || (!A_MN && !B_MN), "8-bit wgmma operands are K-major");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = sA + STAGES * A_STAGE;
-  uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * B_STAGE);
+  uint8_t* sE = sB + STAGES * B_STAGE;         // epilogue staging, EPI_WG_BYTES per MMA warpgroup (1024-byte aligned)
+  uint64_t* full = reinterpret_cast<uint64_t*>(sE + 2 * EPI_WG_BYTES);
   uint64_t* empty = full + STAGES;
 
   const int wg = threadIdx.x >> 7;
@@ -94,6 +101,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
+    if (EPI != EPI_F32) prefetch_tmap(&tmD);
+    if (TWO_OUT) prefetch_tmap(&tmD2);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 8 * CL);   // one arrival per MMA warp of every CTA that reads the stage
@@ -168,6 +177,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     if (F8) alpha *= (p.sinv_a ? __ldg(p.sinv_a) : 1.0f) * (p.sinv_b ? __ldg(p.sinv_b) : 1.0f);
     const float q8_scale = (EPI == EPI_GELU_GRAD_Q8 && p.out_scale) ? __ldg(p.out_scale) : 1.0f;
     float q8_amax = 0.f;
+    uint32_t pass_ctr = 0;   // epilogue passes so far: which staging slot a one-box pass uses
     int stage = 0;
     uint32_t phase = 0;
     float acc[128];
@@ -176,6 +186,15 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       const int m_blk = (p.m_fastest ? tile % tiles_mu : tile / p.tiles_n) * CL + crank;
       const int n_blk = p.m_fastest ? tile / tiles_mu : tile % p.tiles_n;
       const int kb0 = sp * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
+      const int row0 = m_blk * BM + cw * 64;   // first output row of this warpgroup
+      if (AUX) {
+        // pull this tile's aux into L2 while the mainloop runs: the warp's 16 rows x 512 bytes = 64 lines, two per lane
+#pragma unroll
+        for (int i = lane; i < 64; i += 32) {
+          const int r = row0 + wq * 16 + (i >> 2), c = n_blk * BN + (i & 3) * 64;
+          if (r < p.M && c < p.N) prefetch_l2(p.aux + (long long)r * p.ld_aux + c);
+        }
+      }
       int prev = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full[stage], phase);
@@ -221,57 +240,146 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
       }
       if (kb1 <= kb0) continue;
-      // ---------------------------------------------------------------- epilogue from registers
+      if (row0 >= p.M) continue;              // the empty half of an M tail, or the idle CTA of a cluster on an odd tile count
+      if (EPI == EPI_F32) {
+        // ---------------------------------------------------------------- fp32 epilogue, straight from the registers
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const long long row = (long long)m_blk * BM + cw * 64 + wq * 16 + g + 8 * h;
-        if (row >= p.M) continue;
+        for (int h = 0; h < 2; ++h) {
+          const long long row = (long long)row0 + wq * 16 + g + 8 * h;
+          if (row >= p.M) continue;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int col = n_blk * BN + 8 * j + 2 * t4;
-          if (col >= p.N) continue;   // N % 8 == 0: col + 1 < N as well
-          float v0 = acc[4 * j + 2 * h] * alpha, v1 = acc[4 * j + 2 * h + 1] * alpha;
-          if (EPI == EPI_F32) {
-            float* dst = reinterpret_cast<float*>(p.d) + row * p.ldd + col;
+          for (int j = 0; j < 32; ++j) {
+            const int col = n_blk * BN + 8 * j + 2 * t4;
+            if (col >= p.N) continue;   // N % 8 == 0: col + 1 < N as well
+            const float v0 = acc[4 * j + 2 * h] * alpha, v1 = acc[4 * j + 2 * h + 1] * alpha;
+            float* dst = p.d + row * p.ldd + col;
             if (p.accumulate || p.splits > 1) {
               red_add_f32x2(dst, v0, v1);
             } else {
               *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
             }
-            continue;
           }
-          if (p.bias != nullptr) {
-            const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-            v0 += b.x, v1 += b.y;
+        }
+        continue;
+      }
+      // ---------------------------------------------------------------- bf16 / E4M3 epilogue through shared memory
+      // A pass converts CPP columns of the warpgroup's 64 x 256 slice into the staging slots and stores them by TMA:
+      //   * two outputs, 64 columns: D2's box in slot 0, D's in slot 1;
+      //   * one output read with aux, 64 columns: one box, in the slot the previous pass did not use (the aux loads of a wider
+      //     pass would not fit the register budget);
+      //   * one output, 128 columns: two boxes, one per slot.
+      // Only the issuing thread waits for its earlier stores to have been read out of the slots, so the writes to global memory
+      // drain under the next pass and the next tile's mainloop.
+      constexpr int CPP = (TWO_OUT || AUX) ? 64 : 128;
+      constexpr int JP = CPP / 8;                 // 8-column accumulator groups per pass
+      constexpr bool ONE_SLOT = !TWO_OUT && CPP == 64;
+      uint8_t* stg = sE + cw * EPI_WG_BYTES;
+      const uint32_t stg_u32 = smem_u32(stg);
+      // aux of one pass (bf16 pairs; 0 outside [M, N]): the next pass's are loaded before this pass's barriers and stores
+      uint32_t ax[JP][2];
+      const auto load_aux = [&](int q) {
+#pragma unroll
+        for (int jj = 0; jj < JP; ++jj)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const long long row = (long long)row0 + wq * 16 + g + 8 * h;
+            const int col = n_blk * BN + q * CPP + 8 * jj + 2 * t4;
+            ax[jj][h] = (col < p.N && row < p.M) ? __ldg(reinterpret_cast<const uint32_t*>(p.aux + row * p.ld_aux + col)) : 0u;
           }
-          if (EPI == EPI_RESIDUAL || EPI == EPI_DGELU || EPI == EPI_MUL) {
-            const float2 f = unpack_bf16(__ldg(reinterpret_cast<const uint32_t*>(p.aux + row * p.ld_aux + col)));
-            if (EPI == EPI_RESIDUAL) v0 += f.x, v1 += f.y;
-            else if (EPI == EPI_MUL) v0 *= f.x, v1 *= f.y;
-            else v0 *= gelu_grad(f.x), v1 *= gelu_grad(f.y);
+      };
+      if (AUX) load_aux(0);
+#pragma unroll
+      for (int q = 0; q < BN / CPP; ++q) {
+        const int cq = n_blk * BN + q * CPP;      // first output column of the pass
+        if (cq >= p.N) break;
+        const uint32_t slot = ONE_SLOT ? (pass_ctr++ & 1) * EPI_SLOT : 0;
+        const auto slots_free = [&] {             // the previous boxes in the slots this pass writes have been read out
+          if ((threadIdx.x & 127) == 0) {
+            if (ONE_SLOT) tma_wait_read<1>();
+            else tma_wait_read<0>();
           }
-          __nv_bfloat16* drow = reinterpret_cast<__nv_bfloat16*>(p.d) + row * p.ldd + col;
-          if (EPI == EPI_GELU_DUAL) {
-            *reinterpret_cast<uint32_t*>(p.d2 + row * p.ldd2 + col) = pack_bf16(v0, v1);   // z (pre-activation)
-            v0 = gelu_exact(v0), v1 = gelu_exact(v1);
-          } else if (EPI == EPI_GELU_GRAD || EPI == EPI_GELU_GRAD_Q8) {
-            // gelu and its derivative share the CDF / PDF evaluation; the derivative replaces the pre-activation as the
-            // tensor saved for backward, so the dgrad epilogue is a plain multiply
-            float c0, pd0, c1, pd1;
-            gelu_cdf_pdf(v0, c0, pd0);
-            gelu_cdf_pdf(v1, c1, pd1);
-            *reinterpret_cast<uint32_t*>(p.d2 + row * p.ldd2 + col) = pack_bf16(fmaf(v0, pd0, c0), fmaf(v1, pd1, c1));
-            v0 *= c0, v1 *= c1;
-            if (EPI == EPI_GELU_GRAD_Q8) {
-              q8_amax = fmaxf(q8_amax, fmaxf(fabsf(v0), fabsf(v1)));
-              *reinterpret_cast<uint16_t*>(p.d8 + row * p.ld_d8 + col) = pack_e4m3x2(v0 * q8_scale, v1 * q8_scale);
-              continue;
+          named_bar_sync(1 + cw, 128);
+        };
+        uint32_t o1[JP][2], o2[JP][2];            // packed outputs: D and D2
+        // one stmatrix.x4 covers the warp's 16 rows x 16 columns (groups jj, jj + 1): lane l addresses row l % 8 of matrix l / 8,
+        // matrices ordered (rows 0-7, jj), (rows 8-15, jj), (rows 0-7, jj + 1), (rows 8-15, jj + 1). 128B swizzle: the 16-byte
+        // chunk c of row r sits at chunk c ^ (r % 8).
+        const auto stage_pair = [&](int jj) {
+          const int r = wq * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
+          const int cg = jj + (lane >> 4);        // 8-column group inside the pass
+          const uint32_t off = r * 128 + (((cg & 7) ^ (r & 7)) << 4);
+          if (TWO_OUT) {
+            stmatrix_x4(stg_u32 + off, o2[jj][0], o2[jj][1], o2[jj + 1][0], o2[jj + 1][1]);
+            if (EPI != EPI_GELU_GRAD_Q8) stmatrix_x4(stg_u32 + EPI_SLOT + off, o1[jj][0], o1[jj][1], o1[jj + 1][0], o1[jj + 1][1]);
+          } else {
+            stmatrix_x4(stg_u32 + slot + (cg >> 3) * EPI_SLOT + off, o1[jj][0], o1[jj][1], o1[jj + 1][0], o1[jj + 1][1]);
+          }
+        };
+        // Q8 stages its outputs as they are made (the E4M3 bytes in slot 1, unswizzled: 64 rows of 64 bytes): holding a whole
+        // pass for later does not fit the register budget
+        if (EPI == EPI_GELU_GRAD_Q8) slots_free();
+#pragma unroll
+        for (int jj = 0; jj < JP; ++jj) {
+          const int j = q * JP + jj;
+          const int col = cq + 8 * jj + 2 * t4;
+          const bool col_ok = col < p.N;          // N % 8 == 0: col + 1 < N as well
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const long long row = (long long)row0 + wq * 16 + g + 8 * h;
+            const bool in = col_ok && row < p.M;  // elements outside [M, N] are computed but clipped by the TMA store
+            float v0 = acc[4 * j + 2 * h] * alpha, v1 = acc[4 * j + 2 * h + 1] * alpha;
+            if (p.bias != nullptr && col_ok) {
+              const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+              v0 += b.x, v1 += b.y;
             }
+            if (AUX) {
+              const float2 f = unpack_bf16(ax[jj][h]);
+              if (EPI == EPI_RESIDUAL) v0 += f.x, v1 += f.y;
+              else if (EPI == EPI_MUL) v0 *= f.x, v1 *= f.y;
+              else v0 *= gelu_grad(f.x), v1 *= gelu_grad(f.y);
+            }
+            if (EPI == EPI_GELU_DUAL) {
+              o2[jj][h] = pack_bf16(v0, v1);   // z (pre-activation)
+              v0 = gelu_exact(v0), v1 = gelu_exact(v1);
+            } else if (EPI == EPI_GELU_GRAD || EPI == EPI_GELU_GRAD_Q8) {
+              // gelu and its derivative share the CDF / PDF evaluation; the derivative replaces the pre-activation as the
+              // tensor saved for backward, so the dgrad epilogue is a plain multiply
+              float c0, pd0, c1, pd1;
+              gelu_cdf_pdf(v0, c0, pd0);
+              gelu_cdf_pdf(v1, c1, pd1);
+              o2[jj][h] = pack_bf16(fmaf(v0, pd0, c0), fmaf(v1, pd1, c1));
+              v0 *= c0, v1 *= c1;
+              if (EPI == EPI_GELU_GRAD_Q8) {
+                if (in) q8_amax = fmaxf(q8_amax, fmaxf(fabsf(v0), fabsf(v1)));
+                st_shared_u16(stg_u32 + EPI_SLOT + (wq * 16 + g + 8 * h) * 64 + 8 * jj + 2 * t4, pack_e4m3x2(v0 * q8_scale, v1 * q8_scale));
+                continue;
+              }
+            }
+            o1[jj][h] = pack_bf16(v0, v1);
           }
-          *reinterpret_cast<uint32_t*>(drow) = pack_bf16(v0, v1);
+          if (EPI == EPI_GELU_GRAD_Q8 && (jj & 1)) stage_pair(jj - 1);
+        }
+        if (AUX && q + 1 < BN / CPP) load_aux(q + 1);
+        if (EPI != EPI_GELU_GRAD_Q8) {
+          slots_free();
+#pragma unroll
+          for (int jj = 0; jj < JP; jj += 2) stage_pair(jj);
+        }
+        fence_proxy_async_smem();   // the generic-proxy writes become visible to the TMA (async proxy) reads
+        named_bar_sync(1 + cw, 128);
+        if ((threadIdx.x & 127) == 0) {
+          if (TWO_OUT) {
+            tma_store_2d(&tmD2, stg, cq, row0);
+            tma_store_2d(&tmD, stg + EPI_SLOT, cq, row0);
+          } else {
+            tma_store_2d(&tmD, stg + slot, cq, row0);
+            if (CPP == 128 && cq + 64 < p.N) tma_store_2d(&tmD, stg + EPI_SLOT, cq + 64, row0);
+          }
+          tma_commit();
         }
       }
     }
+    if (EPI != EPI_F32 && (threadIdx.x & 127) == 0) tma_wait_all<0>();   // the last stores complete before the CTA exits
     if (EPI == EPI_GELU_GRAD_Q8 && p.out_amax) {
       q8_amax = warp_max_f(q8_amax);
       if (lane == 0 && q8_amax > 0.f) atomic_max_pos_f32(p.out_amax, q8_amax);
@@ -333,7 +441,7 @@ EncodeFn get_encode() {
 }  // namespace
 
 CUtensorMap make_tmap_2d(const void* ptr, int elem_bytes, bool is_float32, uint64_t inner, uint64_t outer,
-                         uint64_t ld_bytes, uint32_t box_inner, uint32_t box_outer) {
+                         uint64_t ld_bytes, uint32_t box_inner, uint32_t box_outer, bool swizzle_128b) {
   if ((reinterpret_cast<uintptr_t>(ptr) & 15) || (ld_bytes & 15))
     throw std::runtime_error("photon_b200 TMA: base pointer and row stride must be 16-byte aligned");
   CUtensorMap m;
@@ -344,14 +452,15 @@ CUtensorMap make_tmap_2d(const void* ptr, int elem_bytes, bool is_float32, uint6
   CUtensorMapDataType dt = is_float32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
                                       : (elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8);
   CUresult r = get_encode()(&m, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            swizzle_128b ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) throw std::runtime_error("photon_b200: cuTensorMapEncodeTiled failed, code " + std::to_string(int(r)));
   return m;
 }
 
 template <int A_MN, int B_MN, int EPI, int CL, int F8>
-static void launch_cl(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, int grid, cudaStream_t stream) {
+static void launch_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& td, const CUtensorMap& td2, const Params& p, int grid,
+                      cudaStream_t stream) {
   auto kern = gemm_kernel<A_MN, B_MN, EPI, CL, F8>;
   static bool configured = false;
   if (!configured) {
@@ -371,14 +480,15 @@ static void launch_cl(const CUtensorMap& ta, const CUtensorMap& tb, const Params
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, p);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, td, td2, p);
   if (e != cudaSuccess) throw std::runtime_error(std::string("gemm launch: ") + cudaGetErrorString(e));
 }
 
 template <int A_MN, int B_MN, int EPI, int F8>
-static void launch_inst(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, int grid, int cluster, cudaStream_t stream) {
-  if (cluster == 2) launch_cl<A_MN, B_MN, EPI, 2, F8>(ta, tb, p, grid, stream);
-  else launch_cl<A_MN, B_MN, EPI, 1, F8>(ta, tb, p, grid, stream);
+static void launch_inst(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& td, const CUtensorMap& td2, const Params& p, int grid,
+                        int cluster, cudaStream_t stream) {
+  if (cluster == 2) launch_cl<A_MN, B_MN, EPI, 2, F8>(ta, tb, td, td2, p, grid, stream);
+  else launch_cl<A_MN, B_MN, EPI, 1, F8>(ta, tb, td, td2, p, grid, stream);
 }
 
 void transpose_u8(const void* src, long long ld, void* dst, int R, int C, cudaStream_t stream) {
@@ -410,13 +520,22 @@ void gemm_launch(const GemmArgs& g, cudaStream_t stream) {
                           : make_tmap_2d(g.B, eb, false, g.K, g.N, g.ldb * eb, BKE, BN / cluster);
   const bool two_out = g.epi == EPI_GELU_DUAL || g.epi == EPI_GELU_GRAD || g.epi == EPI_GELU_GRAD_Q8;
   if (two_out && !g.D2) throw std::runtime_error("photon_b200 gemm: the two-output GELU epilogues need the second output");
-  if (g.epi == EPI_GELU_GRAD_Q8 && (!g.fp8 || !g.D8 || (g.ldd8 % 2) || (reinterpret_cast<uintptr_t>(g.D8) & 1)))
-    throw std::runtime_error("photon_b200 gemm: the fp8-output epilogue needs fp8 operands and a 2-byte aligned fp8 output with an even row stride");
+  const auto aligned16 = [](const void* ptr, long long ld_bytes) { return !(reinterpret_cast<uintptr_t>(ptr) & 15) && !(ld_bytes % 16); };
+  // the TMA store writes whole 16-byte pieces of a row, so the E4M3 output also needs N % 16 == 0 (bf16 rows: N % 8 == 0)
+  if (g.epi == EPI_GELU_GRAD_Q8 && (!g.fp8 || !g.D8 || !aligned16(g.D8, g.ldd8) || g.N % 16))
+    throw std::runtime_error("photon_b200 gemm: the fp8-output epilogue needs fp8 operands, a 16-byte aligned fp8 output and row stride, and N % 16 == 0");
   if ((g.epi == EPI_RESIDUAL || g.epi == EPI_DGELU || g.epi == EPI_MUL) && (!g.aux || (g.ld_aux % 8) || (reinterpret_cast<uintptr_t>(g.aux) & 15)))
     throw std::runtime_error("photon_b200 gemm: aux operand missing or not 16-byte aligned");
   if (g.bias && (reinterpret_cast<uintptr_t>(g.bias) & 15)) throw std::runtime_error("photon_b200 gemm: bias must be 16-byte aligned");
   if (g.epi != EPI_GELU_GRAD_Q8 && ((reinterpret_cast<uintptr_t>(g.D) & 15) || (g.ldd % 8)))
     throw std::runtime_error("photon_b200 gemm: output must be 16-byte aligned");
+  if (two_out && !aligned16(g.D2, g.ldd2 * 2))
+    throw std::runtime_error("photon_b200 gemm: the second output and its row stride must be 16-byte aligned");
+  // output tensor maps: dims = the logical [M, N] (the TMA clips the tails), one box = 64 rows x 64 columns
+  CUtensorMap td = ta, td2 = ta;   // ta stands in for the maps an epilogue does not use
+  if (g.epi == EPI_GELU_GRAD_Q8) td = make_tmap_2d(g.D8, 1, false, g.N, g.M, g.ldd8, 64, 64, false);
+  else if (!f32) td = make_tmap_2d(g.D, 2, false, g.N, g.M, g.ldd * 2, 64, 64);
+  if (two_out) td2 = make_tmap_2d(g.D2, 2, false, g.N, g.M, g.ldd2 * 2, 64, 64);
   Params p{};
   p.M = g.M, p.N = g.N, p.K = g.K;
   p.tiles_m = (g.M + BM - 1) / BM;
@@ -426,12 +545,11 @@ void gemm_launch(const GemmArgs& g, cudaStream_t stream) {
   p.bias = g.bias;
   p.aux = reinterpret_cast<const __nv_bfloat16*>(g.aux);
   p.ld_aux = g.ld_aux;
-  p.d = g.D, p.ldd = g.ldd;
-  p.d2 = reinterpret_cast<__nv_bfloat16*>(g.D2), p.ldd2 = g.ldd2;
+  p.d = reinterpret_cast<float*>(g.D), p.ldd = g.ldd;
   p.accumulate = g.accumulate;
   p.alpha = g.alpha;
   p.a_fmt = g.a_fmt, p.b_fmt = g.b_fmt, p.sinv_a = g.sinv_a, p.sinv_b = g.sinv_b;
-  p.d8 = reinterpret_cast<uint8_t*>(g.D8), p.ld_d8 = g.ldd8, p.out_scale = g.out_scale, p.out_amax = g.out_amax;
+  p.out_scale = g.out_scale, p.out_amax = g.out_amax;
   int sms = g.num_sms;
   if (sms <= 0) {
     int dev = 0;
@@ -460,7 +578,7 @@ void gemm_launch(const GemmArgs& g, cudaStream_t stream) {
 
 #define PB_CASE(AM, BMJ, E, F)                                              \
   if (g.a_mn == AM && g.b_mn == BMJ && g.epi == E && int(g.fp8) == F) {     \
-    launch_inst<AM, BMJ, E, F>(ta, tb, p, grid, cluster, stream);           \
+    launch_inst<AM, BMJ, E, F>(ta, tb, td, td2, p, grid, cluster, stream);  \
     return;                                                                 \
   }
   PB_CASE(0, 0, EPI_BF16, 0)

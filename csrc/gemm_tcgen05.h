@@ -12,6 +12,7 @@ enum Epilogue : int {
   EPI_GELU_DUAL = 2,  // D2 = bf16(z = acc*alpha + bias);  D = bf16(gelu(z))
   EPI_DGELU = 3,      // D = bf16((acc*alpha + bias) * gelu'(aux))
   EPI_F32 = 4,        // D (fp32) = acc*alpha   or  D += acc*alpha   (accumulate, red.global.add)
+  // every other epilogue stores by TMA: D, D2 and D8 need 16-byte aligned base addresses and row strides
   EPI_GELU_GRAD = 5,  // z = acc*alpha + bias;  D = bf16(gelu(z));  D2 = bf16(gelu'(z))  — the backward then needs no erf/exp
   EPI_MUL = 6,        // D = bf16((acc*alpha + bias) * aux)
   EPI_GELU_GRAD_Q8 = 7,  // fp8 operands only: z = acc*alpha + bias;  D8 = e4m3(gelu(z) * *out_scale) (+ amax);  D2 = bf16(gelu'(z))
@@ -56,6 +57,6 @@ void gemm_mxfp8_launch(const void* A, const void* B, void* D, const void* sfa, c
                        long long ldd, int num_sms, cudaStream_t stream);
 
 CUtensorMap make_tmap_2d(const void* ptr, int elem_bytes, bool is_float32, uint64_t inner, uint64_t outer,
-                         uint64_t ld_bytes, uint32_t box_inner, uint32_t box_outer);
+                         uint64_t ld_bytes, uint32_t box_inner, uint32_t box_outer, bool swizzle_128b = true);
 
 }  // namespace pb

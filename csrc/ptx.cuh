@@ -61,6 +61,15 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// four 8x8 b16 matrices to shared memory: lane l gives the 16-byte row address of matrix l / 8, row l % 8; register k holds
+// this lane's two elements (row lane / 4, columns 2 * (lane % 4) + {0, 1}) of matrix k - the wgmma accumulator fragment
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+               : "memory");
+}
+__device__ __forceinline__ void st_shared_u16(uint32_t addr, uint16_t v) {
+  asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"(v) : "memory");
+}
 
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
@@ -226,6 +235,9 @@ __device__ __forceinline__ uint32_t ld_acquire_sys(const uint32_t* p) {
 }
 __device__ __forceinline__ void red_add_release_sys(uint32_t* p, uint32_t v) {
   asm volatile("red.release.sys.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ void prefetch_l2(const void* p) {
+  asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
 }
 __device__ __forceinline__ float4 ld_nc_f4(const float4* p) {
   float4 r;

@@ -95,7 +95,7 @@ def linear_dgrad(dy: torch.Tensor, w: torch.Tensor, dx: torch.Tensor, gelu_pre: 
 
 
 def linear_wgrad(dy: torch.Tensor, x: torch.Tensor, dw: torch.Tensor, accumulate: bool = True, alpha: float = 1.0) -> torch.Tensor:
-    """dw[N,K] (+)= dy^T @ x in fp32 (both operands consumed MN-major; TMA reduce-add when accumulating)."""
+    """dw[N,K] (+)= dy^T @ x in fp32 (both operands consumed MN-major; red.global.add when accumulating)."""
     return gemm(dy, x, dw, a_mn=True, b_mn=True, epi=EPI_F32, accumulate=accumulate, alpha=alpha)
 
 

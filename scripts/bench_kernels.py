@@ -52,7 +52,7 @@ def main():
         b = torch.randn((K, N) if bmn else (N, K), device=dev).to(torch.bfloat16) * 0.05
         f32 = amn and bmn
         out = torch.empty(M, N, device=dev, dtype=torch.float32 if f32 else torch.bfloat16)
-        # weight gradients are timed the way the engine issues them: accumulating into the fp32 bucket (split-K + TMA reduce-add)
+        # weight gradients are timed the way the engine issues them: accumulating into the fp32 bucket (split-K + red.global.add)
         ours = timeit(lambda: ops.gemm(a, b, out, a_mn=bool(amn), b_mn=bool(bmn), epi=ops.EPI_F32 if f32 else ops.EPI_BF16, accumulate=bool(f32)))
         A = a.t() if amn else a
         Bt = b if bmn else b.t()
