@@ -52,10 +52,12 @@ __device__ __forceinline__ void wgmma_pv(float (&o)[DH / 2], const uint32_t (&a)
   else wgmma_bf16_rs_n128<1>(o, a, db, 1u);
 }
 
-template <int DH, bool ALIBI>
+// DOC (document mask): doc_start [B*S] holds the first row of each row's document (rows of one sequence). Query q sees key k
+// iff doc_start[q] <= k <= q. Key tiles that end before the document of the tile's first row are never loaded.
+template <int DH, bool ALIBI, bool DOC>
 __global__ void __launch_bounds__(384, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __restrict__ out, float* __restrict__ lse, int S, int H,
-                float scale, int causal, const float* __restrict__ alibi_slopes) {
+                float scale, int causal, const float* __restrict__ alibi_slopes, const int* __restrict__ doc_start) {
   using C = FwdCfg<DH>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -74,6 +76,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __rest
   const int bh = blockIdx.y, b = bh / H, h = bh - b * H;
   const int d_model = H * DH;
   const int n_kv = causal ? qt + 1 : S / BKV;
+  const int j0 = DOC ? doc_start[b * S + qt * BQ] / BKV : 0;   // first key tile any row of this query tile sees
   const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
 
@@ -97,9 +100,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __rest
       mbar_expect_tx(q_full, C::TILE);
 #pragma unroll
       for (int c = 0; c < C::CH; ++c) tma_load_2d(sQ + c * 16384, &tmQKV, q_full, h * DH + c * 64, b * S + qt * BQ);
-      for (int j = 0; j < n_kv; ++j) {
-        const int st = j & 1;
-        const uint32_t ph = ((j >> 1) & 1) ^ 1;
+      for (int j = j0; j < n_kv; ++j) {
+        const int n = j - j0, st = n & 1;
+        const uint32_t ph = ((n >> 1) & 1) ^ 1;
         mbar_wait(&k_empty[st], ph);
         mbar_expect_tx(&k_full[st], C::TILE);
 #pragma unroll
@@ -127,10 +130,17 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __rest
 #pragma unroll
   for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
   float sacc[64];
+  // DOC: first visible key of this thread's two rows, and of the tile's last row (the largest, ids being runs): key tiles
+  // starting at or after the latter need no document mask
+  int dstart[2] = {0, 0}, dstart_last = 0;
+  if (DOC) {
+    dstart[0] = doc_start[b * S + qrow0], dstart[1] = doc_start[b * S + qrow0 + 8];
+    dstart_last = doc_start[b * S + qt * BQ + BQ - 1];
+  }
   mbar_wait(q_full, 0);
-  for (int j = 0; j < n_kv; ++j) {
-    const int st = j & 1;
-    const uint32_t ph = (j >> 1) & 1;
+  for (int j = j0; j < n_kv; ++j) {
+    const int n = j - j0, st = n & 1;
+    const uint32_t ph = (n >> 1) & 1;
     mbar_wait(&k_full[st], ph);
     wgmma_fence();
 #pragma unroll
@@ -147,6 +157,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __rest
     if (lane == 0) mbar_arrive(&k_empty[st]);
     // scaled (log2-domain) scores, causal mask on the diagonal tile, ALiBi bias slope * (key - query)
     const bool diag = causal && j == qt;
+    const bool dmask = DOC && j * BKV < dstart_last;
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int j8 = 0; j8 < 16; ++j8) {
@@ -158,17 +169,26 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __rest
         float x = sacc[4 * j8 + e] * sc;
         if (ALIBI) x = fmaf(slope2, float(key - q), x);
         if (diag && key > q) x = -INFINITY;
+        if (dmask && key < dstart[hh]) x = -INFINITY;
         sacc[4 * j8 + e] = x;
         mx[hh] = fmaxf(mx[hh], x);
       }
     }
     float alpha[2];
+    [[maybe_unused]] float msub[2];
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffff, mx[hh], 1));
       mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffff, mx[hh], 2));
       const float m_new = fmaxf(m[hh], mx[hh]);
-      alpha[hh] = exp2f(m[hh] - m_new);   // 0 on the first tile (m = -inf)
+      if constexpr (DOC) {
+        // a row can meet a tile with no visible key before its first one (m_new = -inf); subtracting 0 there keeps
+        // exp2(-inf - -inf) = NaN out of alpha and P (both become 0, and l, O are still 0)
+        msub[hh] = m_new == -INFINITY ? 0.f : m_new;
+        alpha[hh] = exp2f(m[hh] - msub[hh]);
+      } else {
+        alpha[hh] = exp2f(m[hh] - m_new);   // 0 on the first tile (m = -inf)
+      }
       m[hh] = m_new;
       l[hh] *= alpha[hh];
     }
@@ -177,7 +197,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __rest
     for (int j8 = 0; j8 < 16; ++j8) {
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const float pv = exp2f(sacc[4 * j8 + e] - m[e >> 1]);
+        const float pv = exp2f(sacc[4 * j8 + e] - (DOC ? msub[e >> 1] : m[e >> 1]));
         sacc[4 * j8 + e] = pv;
         l[e >> 1] += pv;
       }
@@ -275,11 +295,14 @@ __device__ __forceinline__ void wgmma_acc_rs(float (&d)[DH / 2], const uint32_t 
   else wgmma_bf16_rs_n128<1>(d, a, db, 1u);
 }
 
-template <int DH, bool ALIBI>
+// DOC: as in the forward; doc_end [B*S] holds the last row of each row's document, so the query walk of a key tile stops at
+// the 64-row tile holding the end of its last key's document.
+template <int DH, bool ALIBI, bool DOC>
 __global__ void __launch_bounds__(384, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
                 const float* __restrict__ lse, const float* __restrict__ delta, __nv_bfloat16* __restrict__ dqkv, int S, int H, float scale,
-                int causal, float* __restrict__ dq_acc, const float* __restrict__ alibi_slopes) {
+                int causal, float* __restrict__ dq_acc, const float* __restrict__ alibi_slopes, const int* __restrict__ doc_start,
+                const int* __restrict__ doc_end) {
   using C = BwdCfg<DH>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -296,7 +319,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
   const int jt = int(gridDim.x) - 1 - int(blockIdx.x);   // causal: small key tiles see the most query tiles - start them first
   const int bh = blockIdx.y, b = bh / H, h = bh - b * H;
   const int d_model = H * DH;
-  const int i0 = causal ? jt * 2 : 0, n_q = S / 64;        // 64-row query tiles
+  const int i0 = causal ? jt * 2 : 0;                      // 64-row query tiles
+  const int n_q = DOC ? doc_end[b * S + jt * 128 + 127] / 64 + 1 : S / 64;
   const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
 
@@ -345,6 +369,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
   const float slope2 = ALIBI ? alibi_slopes[h] * LOG2E : 0.f;
   const float* lse_bh = lse + (long long)bh * S;
   const float* delta_bh = delta + (long long)bh * S;
+  const int* dstart_b = DOC ? doc_start + (long long)b * S : nullptr;
   float dv[DH / 2], dk[DH / 2];
 #pragma unroll
   for (int i = 0; i < DH / 2; ++i) dv[i] = 0.f, dk[i] = 0.f;
@@ -380,6 +405,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
       const int qa = q0 + 8 * j8 + 2 * t4;
       const float2 L = *reinterpret_cast<const float2*>(lse_bh + qa);
       const float2 D = *reinterpret_cast<const float2*>(delta_bh + qa);
+      int2 DS = make_int2(0, 0);
+      if (DOC) DS = *reinterpret_cast<const int2*>(dstart_b + qa);   // through L1, like lse / delta
       float pv[4], dsv[4];
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
@@ -388,8 +415,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
         if (ALIBI) x = fmaf(slope2, float(key - q), x);
         float pr = exp2f(x);
         if (causal && q < key) pr = 0.f;
+        if (DOC && ((e & 1) ? DS.y : DS.x) > key) pr = 0.f;
         pv[e] = pr;
         dsv[e] = pr * (dp[4 * j8 + e] - ((e & 1) ? D.y : D.x));
+        // a masked query of another document may carry a non-finite delta (its own keys' fault): keep it out of dK
+        if (DOC && pr == 0.f) dsv[e] = 0.f;
       }
       // accumulator columns 16 kc .. 16 kc + 15 (queries) are the A fragment of k-step kc
       const int kc = j8 >> 1, hi = (j8 & 1) * 2;
@@ -457,6 +487,53 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
   }
 }
 
+// ======================================================================================= document bounds
+// One CTA per sequence: documents are maximal runs of equal ids. Each thread takes a contiguous chunk of rows, finds the
+// last document start and the first document end in it, and a block-wide max- / min-scan over the chunks carries them across.
+constexpr int DOC_THREADS = 1024;
+__global__ void __launch_bounds__(DOC_THREADS) doc_bounds_kernel(const long long* __restrict__ ids, int* __restrict__ doc_start,
+                                                                 int* __restrict__ doc_end, int S) {
+  const long long* row = ids + (long long)blockIdx.x * S;
+  int* ds = doc_start + (long long)blockIdx.x * S;
+  int* de = doc_end + (long long)blockIdx.x * S;
+  const int per = (S + DOC_THREADS - 1) / DOC_THREADS;
+  const int lo = min(S, int(threadIdx.x) * per), hi = min(S, lo + per);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  auto starts = [&](int s) { return s == 0 || row[s] != row[s - 1]; };
+  auto ends = [&](int s) { return s == S - 1 || row[s] != row[s + 1]; };
+  int last_start = -1, first_end = S;   // none in this chunk
+  for (int s = lo; s < hi; ++s)
+    if (starts(s)) last_start = s;
+  for (int s = hi - 1; s >= lo; --s)
+    if (ends(s)) first_end = s;
+  // inclusive scans inside the warp: max of starts from the left, min of ends from the right
+  int inc_start = last_start, inc_end = first_end;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int a = __shfl_up_sync(0xffffffff, inc_start, o), z = __shfl_down_sync(0xffffffff, inc_end, o);
+    if (lane >= o) inc_start = max(inc_start, a);
+    if (lane + o < 32) inc_end = min(inc_end, z);
+  }
+  __shared__ int warp_start[DOC_THREADS / 32], warp_end[DOC_THREADS / 32];
+  if (lane == 31) warp_start[warp] = inc_start;
+  if (lane == 0) warp_end[warp] = inc_end;
+  __syncthreads();
+  // exclusive: what the chunks before (after) this one contribute
+  int carry_start = __shfl_up_sync(0xffffffff, inc_start, 1), carry_end = __shfl_down_sync(0xffffffff, inc_end, 1);
+  if (lane == 0) carry_start = -1;
+  if (lane == 31) carry_end = S;
+  for (int w = 0; w < warp; ++w) carry_start = max(carry_start, warp_start[w]);
+  for (int w = warp + 1; w < DOC_THREADS / 32; ++w) carry_end = min(carry_end, warp_end[w]);
+  for (int s = lo; s < hi; ++s) {
+    if (starts(s)) carry_start = s;
+    ds[s] = carry_start;
+  }
+  for (int s = hi - 1; s >= lo; --s) {
+    if (ends(s)) carry_end = s;
+    de[s] = carry_end;
+  }
+}
+
 template <typename K>
 void set_smem(K kern, int bytes) {
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
@@ -466,33 +543,44 @@ void set_smem(K kern, int bytes) {
 }  // namespace
 
 void attention_fwd_launch(const void* qkv, void* out, float* lse, int B, int S, int H, int dh, float scale, bool causal, int num_sms,
-                          cudaStream_t st, const float* alibi_slopes) {
+                          cudaStream_t st, const float* alibi_slopes, const int* doc_start) {
   (void)num_sms;
   if (S % 128) throw std::runtime_error("photon_b200 attention: sequence length must be a multiple of 128");
   if (dh != 64 && dh != 128) throw std::runtime_error("photon_b200 attention: d_head must be 64 or 128");
+  if (doc_start && !causal) throw std::runtime_error("photon_b200 attention: the document mask needs the causal mask");
   const int d = H * dh;
   CUtensorMap tm = make_tmap_2d(qkv, 2, false, uint64_t(3) * d, uint64_t(B) * S, uint64_t(3) * d * 2, 64, 128);
   const dim3 grid(S / 128, B * H);
-#define PB_FWD(DHV, AL)                                                                                              \
+#define PB_FWD(DHV, AL, DOC)                                                                                         \
   {                                                                                                                  \
-    static bool once = (set_smem(attn_fwd_kernel<DHV, AL>, FwdCfg<DHV>::SMEM), true);                                \
+    static bool once = (set_smem(attn_fwd_kernel<DHV, AL, DOC>, FwdCfg<DHV>::SMEM), true);                           \
     (void)once;                                                                                                      \
-    attn_fwd_kernel<DHV, AL><<<grid, 384, FwdCfg<DHV>::SMEM, st>>>(tm, (__nv_bfloat16*)out, lse, S, H, scale, causal ? 1 : 0, \
-                                                                  alibi_slopes);                                     \
+    attn_fwd_kernel<DHV, AL, DOC><<<grid, 384, FwdCfg<DHV>::SMEM, st>>>(tm, (__nv_bfloat16*)out, lse, S, H, scale,   \
+                                                                       causal ? 1 : 0, alibi_slopes, doc_start);    \
   }
-  if (dh == 64 && !alibi_slopes) PB_FWD(64, false)
-  else if (dh == 64) PB_FWD(64, true)
-  else if (!alibi_slopes) PB_FWD(128, false)
-  else PB_FWD(128, true)
+  if (!doc_start) {
+    if (dh == 64 && !alibi_slopes) PB_FWD(64, false, false)
+    else if (dh == 64) PB_FWD(64, true, false)
+    else if (!alibi_slopes) PB_FWD(128, false, false)
+    else PB_FWD(128, true, false)
+  } else {
+    if (dh == 64 && !alibi_slopes) PB_FWD(64, false, true)
+    else if (dh == 64) PB_FWD(64, true, true)
+    else if (!alibi_slopes) PB_FWD(128, false, true)
+    else PB_FWD(128, true, true)
+  }
 #undef PB_FWD
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) throw std::runtime_error(std::string("attention fwd launch: ") + cudaGetErrorString(e));
 }
 
 int attention_bwd_launch(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta, float* dq_acc,
-                         int B, int S, int H, int dh, float scale, bool causal, int num_sms, cudaStream_t st, const float* alibi_slopes) {
+                         int B, int S, int H, int dh, float scale, bool causal, int num_sms, cudaStream_t st, const float* alibi_slopes,
+                         const int* doc_start, const int* doc_end) {
   if (S % 128) throw std::runtime_error("photon_b200 attention: sequence length must be a multiple of 128");
   if (dh != 64 && dh != 128) throw std::runtime_error("photon_b200 attention backward: d_head must be 64 or 128");
+  if (bool(doc_start) != bool(doc_end)) throw std::runtime_error("photon_b200 attention backward: doc_start and doc_end go together");
+  if (doc_start && !causal) throw std::runtime_error("photon_b200 attention: the document mask needs the causal mask");
   const int sms = num_sms > 0 ? num_sms : 132;
   const int d = H * dh;
   const long long rows = (long long)B * S;
@@ -506,22 +594,36 @@ int attention_bwd_launch(const void* qkv, const void* out, const void* dout, con
   CUtensorMap tmQ = make_tmap_2d(qkv, 2, false, uint64_t(3) * d, uint64_t(rows), uint64_t(3) * d * 2, 64, 64);
   CUtensorMap tmDO = make_tmap_2d(dout, 2, false, uint64_t(d), uint64_t(rows), uint64_t(d) * 2, 64, 64);
   const dim3 grid(S / 128, B * H);
-#define PB_BWD(DHV, AL)                                                                                              \
+#define PB_BWD(DHV, AL, DOC)                                                                                         \
   {                                                                                                                  \
-    static bool once = (set_smem(attn_bwd_kernel<DHV, AL>, BwdCfg<DHV>::SMEM), true);                                \
+    static bool once = (set_smem(attn_bwd_kernel<DHV, AL, DOC>, BwdCfg<DHV>::SMEM), true);                           \
     (void)once;                                                                                                      \
-    attn_bwd_kernel<DHV, AL><<<grid, 384, BwdCfg<DHV>::SMEM, st>>>(tmKV, tmQ, tmDO, lse, delta, (__nv_bfloat16*)dqkv, S, H, scale, \
-                                                                  causal ? 1 : 0, dq_acc, alibi_slopes);             \
+    attn_bwd_kernel<DHV, AL, DOC><<<grid, 384, BwdCfg<DHV>::SMEM, st>>>(tmKV, tmQ, tmDO, lse, delta, (__nv_bfloat16*)dqkv, S, H, \
+                                                                       scale, causal ? 1 : 0, dq_acc, alibi_slopes,  \
+                                                                       doc_start, doc_end);                          \
   }
-  if (dh == 64 && !alibi_slopes) PB_BWD(64, false)
-  else if (dh == 64) PB_BWD(64, true)
-  else if (!alibi_slopes) PB_BWD(128, false)
-  else PB_BWD(128, true)
+  if (!doc_start) {
+    if (dh == 64 && !alibi_slopes) PB_BWD(64, false, false)
+    else if (dh == 64) PB_BWD(64, true, false)
+    else if (!alibi_slopes) PB_BWD(128, false, false)
+    else PB_BWD(128, true, false)
+  } else {
+    if (dh == 64 && !alibi_slopes) PB_BWD(64, false, true)
+    else if (dh == 64) PB_BWD(64, true, true)
+    else if (!alibi_slopes) PB_BWD(128, false, true)
+    else PB_BWD(128, true, true)
+  }
 #undef PB_BWD
   attn_bwd_dq_convert_kernel<<<sms * 8, 256, 0, st>>>(dq_acc, (__nv_bfloat16*)dqkv, rows, d, scale);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) throw std::runtime_error(std::string("attention bwd launch: ") + cudaGetErrorString(e));
   return 3;
+}
+
+void doc_bounds_launch(const long long* sequence_id, int* doc_start, int* doc_end, int B, int S, cudaStream_t st) {
+  doc_bounds_kernel<<<B, DOC_THREADS, 0, st>>>(sequence_id, doc_start, doc_end, S);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) throw std::runtime_error(std::string("doc_bounds launch: ") + cudaGetErrorString(e));
 }
 
 // ---------------------------------------------------------------------------------------------- RoPE

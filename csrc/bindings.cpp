@@ -281,21 +281,38 @@ void check_attention_args(const Tensor& qkv, const Tensor& out, const Tensor& ls
     TORCH_CHECK(alibi_slopes->numel() == n_heads && alibi_slopes->is_contiguous(), "alibi_slopes must be contiguous with n_heads elements");
   }
 }
+// document-mask bounds (doc_bounds): int32 [B*S] on the device of qkv, contiguous; the mask is a refinement of the causal one
+void check_doc_bound(const c10::optional<Tensor>& t, const char* name, const Tensor& qkv) {
+  if (!t.has_value()) return;
+  check_cuda(*t, name);
+  TORCH_CHECK(t->scalar_type() == at::kInt, name, " must be int32");
+  TORCH_CHECK(t->device() == qkv.device(), name, " must be on the device of qkv");
+  TORCH_CHECK(t->is_contiguous() && t->numel() == qkv.size(0) * qkv.size(1), name, " must be contiguous int32 with B*S elements");
+}
+void check_doc_args(const Tensor& qkv, bool causal, const c10::optional<Tensor>& doc_start, const c10::optional<Tensor>& doc_end) {
+  TORCH_CHECK(!doc_end.has_value() || doc_start.has_value(), "attention: doc_end without doc_start");
+  TORCH_CHECK(!doc_start.has_value() || causal, "attention: the document mask is only supported with the causal mask");
+  check_doc_bound(doc_start, "doc_start", qkv);
+  check_doc_bound(doc_end, "doc_end", qkv);
+}
 void attention_fwd(const Tensor& qkv, Tensor& out, Tensor& lse, int n_heads, double scale, bool causal,
-                   const c10::optional<Tensor>& alibi_slopes) {
+                   const c10::optional<Tensor>& alibi_slopes, const c10::optional<Tensor>& doc_start) {
   check_bf16(qkv, "qkv");
   check_bf16(out, "out");
   check_f32(lse, "lse");
   check_attention_args(qkv, out, lse, n_heads, causal, alibi_slopes);
+  check_doc_args(qkv, causal, doc_start, c10::nullopt);
   c10::cuda::CUDAGuard guard(qkv.device());
   const int B = int(qkv.size(0)), S = int(qkv.size(1)), d = int(qkv.size(2) / 3);
   pb::attention_fwd_launch(qkv.data_ptr(), out.data_ptr(), lse.data_ptr<float>(), B, S, n_heads, d / n_heads, float(scale), causal,
                            at::cuda::getCurrentDeviceProperties()->multiProcessorCount, stream_of(qkv),
-                           alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr);
+                           alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr,
+                           doc_start.has_value() ? doc_start->data_ptr<int>() : nullptr);
   g_launches += 1;
 }
 void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, const Tensor& lse, Tensor& dqkv, Tensor& delta,
-                   int n_heads, double scale, bool causal, const c10::optional<Tensor>& alibi_slopes) {
+                   int n_heads, double scale, bool causal, const c10::optional<Tensor>& alibi_slopes,
+                   const c10::optional<Tensor>& doc_start, const c10::optional<Tensor>& doc_end) {
   check_bf16(qkv, "qkv");
   check_bf16(out, "out");
   check_bf16(dout, "dout");
@@ -303,6 +320,8 @@ void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, con
   check_f32(lse, "lse");
   check_f32(delta, "delta");
   check_attention_args(qkv, out, lse, n_heads, causal, alibi_slopes);
+  check_doc_args(qkv, causal, doc_start, doc_end);
+  TORCH_CHECK(doc_start.has_value() == doc_end.has_value(), "attention_bwd: doc_start needs doc_end");
   TORCH_CHECK(dout.is_contiguous() && dout.sizes() == out.sizes(), "dout must be contiguous [B,S,d]");
   TORCH_CHECK(delta.is_contiguous() && delta.sizes() == lse.sizes(), "delta must be contiguous float32 [B,H,S]");
   TORCH_CHECK(dqkv.is_contiguous() && dqkv.sizes() == qkv.sizes(), "dqkv must be contiguous and shaped like qkv");
@@ -314,8 +333,27 @@ void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, con
   const int launched = pb::attention_bwd_launch(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr<float>(), dqkv.data_ptr(),
                                                 delta.data_ptr<float>(), dq_acc.data_ptr<float>(), B, S, n_heads, d / n_heads, float(scale), causal,
                                                 at::cuda::getCurrentDeviceProperties()->multiProcessorCount, stream_of(qkv),
-                                                alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr);
+                                                alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr,
+                                                doc_start.has_value() ? doc_start->data_ptr<int>() : nullptr,
+                                                doc_end.has_value() ? doc_end->data_ptr<int>() : nullptr);
   g_launches += launched;
+}
+// sequence_id int64 [B,S] -> doc_start / doc_end int32 [B*S] (first / last row of each row's document)
+void doc_bounds(const Tensor& sequence_id, Tensor& doc_start, Tensor& doc_end) {
+  check_cuda(sequence_id, "sequence_id");
+  TORCH_CHECK(sequence_id.scalar_type() == at::kLong && sequence_id.dim() == 2 && sequence_id.is_contiguous(),
+              "sequence_id must be contiguous int64 [B,S]");
+  const int64_t B = sequence_id.size(0), S = sequence_id.size(1);
+  for (const Tensor* t : {&doc_start, &doc_end}) {
+    check_cuda(*t, "doc bounds");
+    TORCH_CHECK(t->scalar_type() == at::kInt && t->is_contiguous() && t->numel() == B * S && t->device() == sequence_id.device(),
+                "doc_start / doc_end must be contiguous int32 with B*S elements on the device of sequence_id");
+  }
+  c10::cuda::CUDAGuard guard(sequence_id.device());
+  if (B == 0 || S == 0) return;
+  pb::doc_bounds_launch(reinterpret_cast<const long long*>(sequence_id.data_ptr<int64_t>()), doc_start.data_ptr<int>(),
+                        doc_end.data_ptr<int>(), int(B), int(S), stream_of(sequence_id));
+  g_launches += 1;
 }
 void rope(Tensor& qkv, const Tensor& cos_t, const Tensor& sin_t, int n_heads, bool inverse) {
   check_bf16(qkv, "qkv");
@@ -850,9 +888,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fp8_quantize_segments", &fp8_quantize_segments);
   m.def("fp8_update_scales", &fp8_update_scales);
   m.def("attention_fwd", &attention_fwd, py::arg("qkv"), py::arg("out"), py::arg("lse"), py::arg("n_heads"), py::arg("scale"),
-        py::arg("causal"), py::arg("alibi_slopes") = py::none());
+        py::arg("causal"), py::arg("alibi_slopes") = py::none(), py::arg("doc_start") = py::none());
   m.def("attention_bwd", &attention_bwd, py::arg("qkv"), py::arg("out"), py::arg("dout"), py::arg("lse"), py::arg("dqkv"), py::arg("delta"),
-        py::arg("n_heads"), py::arg("scale"), py::arg("causal"), py::arg("alibi_slopes") = py::none());
+        py::arg("n_heads"), py::arg("scale"), py::arg("causal"), py::arg("alibi_slopes") = py::none(), py::arg("doc_start") = py::none(),
+        py::arg("doc_end") = py::none());
+  m.def("doc_bounds", &doc_bounds, py::arg("sequence_id"), py::arg("doc_start"), py::arg("doc_end"));
   m.def("rope", &rope);
   m.def("embed_fwd", &embed_fwd);
   m.def("skinny_gemm", &skinny_gemm, py::arg("x"), py::arg("w"), py::arg("y"), py::arg("bias") = py::none(), py::arg("residual") = py::none(),

@@ -178,14 +178,34 @@ class StreamingTokenDataset:
         self.sample_in_epoch = pos * old_w // self.world_size  # elastic resume across world sizes
 
 
+def sequence_ids(ids: torch.Tensor, eos_token_id: int | None = None, bos_token_id: int | None = None) -> torch.Tensor | None:
+    """llm-foundry's ``sequence_id`` of a packed batch ``[B, S]``: the document index of every token, counted from 0 in each
+    row. EOS mode: ``cumsum(ids == eos)`` shifted right by one, so the EOS token belongs to the document it ends. BOS mode:
+    ``cumsum(ids == bos)``, so the BOS token opens its document. None when neither id is given."""
+    if eos_token_id is not None and bos_token_id is not None:
+        raise ValueError("Cannot use both eos_token_id and bos_token_id to detect document boundaries")
+    if bos_token_id is not None:
+        return torch.cumsum(ids == int(bos_token_id), dim=1).to(ids.dtype)
+    if eos_token_id is None:
+        return None
+    cs = torch.cumsum(ids == int(eos_token_id), dim=1).to(ids.dtype)
+    return torch.cat([cs.new_zeros(cs.shape[0], 1), cs[:, :-1]], dim=1)
+
+
 class TokenLoader:
     """Batches a :class:`StreamingTokenDataset` into pinned ``[B,S]`` int64 tensors.
     ``num_workers>0`` turns on a background prefetch thread (host side only; the H2D
     copy belongs to the trainer's copy stream)."""
 
     def __init__(self, dataset: StreamingTokenDataset, batch_size: int, drop_last: bool = True,
-                 num_workers: int = 0, prefetch: int = 4, pin_memory: bool | None = None) -> None:
+                 num_workers: int = 0, prefetch: int = 4, pin_memory: bool | None = None,
+                 eos_token_id: int | None = None, bos_token_id: int | None = None) -> None:
+        """``eos_token_id`` / ``bos_token_id`` (at most one; llm-foundry's ``dataset`` keys): add a per-token ``sequence_id``
+        to every batch that numbers the documents of each packed row (see :func:`sequence_ids`)."""
+        if eos_token_id is not None and bos_token_id is not None:
+            raise ValueError("Cannot use both eos_token_id and bos_token_id to detect document boundaries")
         self.dataset, self.batch_size, self.drop_last = dataset, int(batch_size), bool(drop_last)
+        self.eos_token_id, self.bos_token_id = eos_token_id, bos_token_id
         self.num_workers, self.prefetch = int(num_workers), int(prefetch)
         self.pin = torch.cuda.is_available() if pin_memory is None else pin_memory
         # position of the CONSUMER (the trainer), not of the producer: the prefetch thread runs ahead of what has been
@@ -200,9 +220,14 @@ class TokenLoader:
 
     def _collate(self, rows: list[np.ndarray]) -> dict[str, torch.Tensor]:
         ids = torch.from_numpy(np.stack(rows).astype(np.int64))
+        sid = sequence_ids(ids, self.eos_token_id, self.bos_token_id)
         if self.pin:
             ids = ids.pin_memory()
-        return {"input_ids": ids, "labels": ids}  # labels == inputs; the shift happens in the loss
+            sid = sid.pin_memory() if sid is not None else None
+        batch = {"input_ids": ids, "labels": ids}  # labels == inputs; the shift happens in the loss
+        if sid is not None:
+            batch["sequence_id"] = sid
+        return batch
 
     def _gen(self) -> Iterator[dict[str, torch.Tensor]]:
         rows: list[np.ndarray] = []
@@ -285,6 +310,10 @@ def build_text_loader(loader_cfg: dict[str, Any], batch_size: int, rank: int = 0
     split = ds_cfg.pop("split", None)
     root_local = ds_cfg.pop("root_local", None) or ds_cfg.pop("local", None)
     ds_cfg.pop("root_remote", None)
+    # llm-foundry's text collator keys: either one makes every batch carry a per-token sequence_id
+    eos_token_id, bos_token_id = ds_cfg.pop("eos_token_id", None), ds_cfg.pop("bos_token_id", None)
+    if eos_token_id is not None and bos_token_id is not None:
+        raise ValueError("dataset: set at most one of eos_token_id and bos_token_id")
     streams: list[Stream] = []
     if isinstance(streams_cfg, dict):
         for name, sc in streams_cfg.items():
@@ -306,4 +335,5 @@ def build_text_loader(loader_cfg: dict[str, Any], batch_size: int, rank: int = 0
                                synthetic_seed=seed, synthetic_vocab=vocab_size,
                                **{k: v for k, v in ds_cfg.items() if k in ("synthetic_samples", "allow_synthetic")})
     return TokenLoader(ds, batch_size=batch_size, drop_last=bool(loader_cfg.get("drop_last", True)),
-                       num_workers=0 if nw in (None, "auto") else min(int(nw), 1))
+                       num_workers=0 if nw in (None, "auto") else min(int(nw), 1),
+                       eos_token_id=eos_token_id, bos_token_id=bos_token_id)

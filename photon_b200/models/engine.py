@@ -33,7 +33,7 @@ import torch
 import torch.nn.functional as F
 
 from photon_b200 import ops
-from photon_b200.models.mpt import MPTConfig, MPTForCausalLM, shift_labels
+from photon_b200.models.mpt import MPTConfig, MPTForCausalLM, check_sequence_id, shift_labels
 from photon_b200.train.backend import apply_freeze
 from photon_b200.utils.flat import FlatLayout, FlatParams
 
@@ -409,45 +409,57 @@ class B200Engine:
                   logits=bf(min(self.lm_head_chunk, T), c.vocab_size))
         if self.fp8:   # E5M2 copy of the gradient currently flowing backward (one buffer, viewed at the width in use)
             ws["g8"] = torch.empty(T * max(c.expansion_ratio, 3) * d, dtype=torch.uint8, device=dev)
+        if c.attn_uses_sequence_id:   # first / last row of each row's document, shared by every layer and both directions
+            ws.update(doc_start=torch.empty(T, dtype=torch.int32, device=dev), doc_end=torch.empty(T, dtype=torch.int32, device=dev))
+        ws["sequence_id"] = None      # this microbatch's document ids (set by _forward), None: plain causal
         self._ws[key] = ws
         return ws
 
     # ------------------------------------------------------------------ forward
-    def _attention_fwd(self, lw: dict[str, Any], b: int, S: int) -> None:
+    def _kernel_attention(self, S: int) -> bool:
+        return self.attn_mode == "b200" and S % 128 == 0
+
+    def _attention_fwd(self, lw: dict[str, Any], ws: dict[str, Any], b: int, S: int) -> None:
         c = self.cfg
         scale = 1.0 / math.sqrt(c.d_head)
-        if self.attn_mode == "b200" and S % 128 == 0:
+        doc = ws["sequence_id"] is not None
+        if self._kernel_attention(S):
             ops.attention_fwd(lw["qkv"].view(b, S, 3 * c.d_model), lw["attn"].view(b, S, c.d_model), lw["lse"], c.n_heads, scale, True,
-                              self.alibi)
+                              self.alibi, ws["doc_start"] if doc else None)
             return
         # library attention: kernels.attention=torch, an unsupported d_head, or a sequence length that is not a multiple
         # of the 128-row tiles (the shipped configs use 2048)
         q, k, v = lw["qkv"].view(b, S, 3, c.n_heads, c.d_head).permute(2, 0, 3, 1, 4)
-        o = F.scaled_dot_product_attention(q, k, v, scale=scale, **self._sdpa_mask(S, q.dtype))
+        o = F.scaled_dot_product_attention(q, k, v, scale=scale, **self._sdpa_mask(S, q.dtype, ws["sequence_id"]))
         lw["attn"].view(b, S, c.n_heads, c.d_head).copy_(o.transpose(1, 2))
 
-    def _sdpa_mask(self, S: int, dtype: torch.dtype) -> dict[str, Any]:
-        if self.alibi is None:
+    def _sdpa_mask(self, S: int, dtype: torch.dtype, sequence_id: torch.Tensor | None = None) -> dict[str, Any]:
+        if self.alibi is None and sequence_id is None:
             return {"is_causal": True}
+        keep = torch.ones(S, S, dtype=torch.bool, device=self.device).tril()
+        if sequence_id is not None:   # the same equality mask as the torch module: [b, 1, S, S]
+            keep = keep & (sequence_id[:, :, None] == sequence_id[:, None, :])[:, None]
+        if self.alibi is None:
+            return {"attn_mask": keep}
         pos = torch.arange(S, device=self.device)
         bias = self.alibi[:, None, None] * (pos[None, :] - pos[:, None]).clamp(max=0).float()[None]
-        keep = torch.ones(S, S, dtype=torch.bool, device=self.device).tril()
-        return {"attn_mask": bias.masked_fill(~keep, float("-inf")).to(dtype)[None]}
+        return {"attn_mask": bias[None].masked_fill(~keep, float("-inf")).to(dtype)}
 
     def _attention_bwd(self, lw: dict[str, Any], ws: dict[str, Any], b: int, S: int) -> None:
         c = self.cfg
         scale = 1.0 / math.sqrt(c.d_head)
-        if self.attn_mode == "b200" and S % 128 == 0:
+        doc = ws["sequence_id"] is not None
+        if self._kernel_attention(S):
             ops.attention_bwd(lw["qkv"].view(b, S, 3 * c.d_model), lw["attn"].view(b, S, c.d_model),
                               ws["dattn"].view(b, S, c.d_model), lw["lse"], ws["dqkv"].view(b, S, 3 * c.d_model), ws["delta"],
-                              c.n_heads, scale, True, self.alibi)
+                              c.n_heads, scale, True, self.alibi, ws["doc_start"] if doc else None, ws["doc_end"] if doc else None)
             if self.rope is not None:   # gradients w.r.t. the un-rotated q, k
                 ops.rope_(ws["dqkv"].view(b, S, 3 * c.d_model), self.rope[0], self.rope[1], c.n_heads, inverse=True)
             return
         with torch.enable_grad():
             qkv = lw["qkv"].view(b, S, 3, c.n_heads, c.d_head).detach().requires_grad_(True)
             q, k, v = qkv.permute(2, 0, 3, 1, 4)
-            o = F.scaled_dot_product_attention(q, k, v, scale=scale, **self._sdpa_mask(S, q.dtype))
+            o = F.scaled_dot_product_attention(q, k, v, scale=scale, **self._sdpa_mask(S, q.dtype, ws["sequence_id"]))
             (g,) = torch.autograd.grad(o, qkv, ws["dattn"].view(b, S, c.n_heads, c.d_head).transpose(1, 2))
         ws["dqkv"].view(b, S, 3, c.n_heads, c.d_head).copy_(g)
         if self.rope is not None:
@@ -474,7 +486,7 @@ class B200Engine:
                 qkv3[:, j].copy_(ws["qk_tmp"])
         if self.rope is not None:
             ops.rope_(lw["qkv"].view(b, S, 3 * c.d_model), self.rope[0], self.rope[1], c.n_heads)
-        self._attention_fwd(lw, b, S)
+        self._attention_fwd(lw, ws, b, S)
         if self.fp8:
             ops.colsum_quant(lw["attn"], None, lw["attn8"], ops.E4M3, M, R("x_attn", i))
             ops.gemm_fp8(lw["attn8"], w8["wo"], lw["hmid"], M, R("x_attn", i), R("wo", i), epi=ops.EPI_RESIDUAL, bias=w.bo, aux=h[i])
@@ -489,11 +501,16 @@ class B200Engine:
         ops.linear_gelu_grad_fwd(lw["ln2"], w.wup, w.bup, lw["z"], lw["u"])   # lw["z"] holds gelu'(pre-activation)
         ops.linear_fwd(lw["u"], w.wdown, w.bdown, h[i + 1], residual=lw["hmid"])
 
-    def _forward(self, ids: torch.Tensor, ws: dict[str, Any]) -> None:
+    def _forward(self, ids: torch.Tensor, ws: dict[str, Any], sequence_id: torch.Tensor | None = None) -> None:
+        """``sequence_id``: document ids of the rows (already checked by :func:`check_sequence_id`), None: plain causal. The
+        kernels' document bounds are computed once here for every layer, the backward and its recompute."""
         c = self.cfg
         b, S = ids.shape
         h = ws["h"]
         z = self.zero3
+        ws["sequence_id"] = sequence_id
+        if sequence_id is not None and self._kernel_attention(S):
+            ops.doc_bounds(sequence_id, ws["doc_start"], ws["doc_end"])
         if z is not None:
             z.ensure_resident()
         ops.embed_fwd(ids.reshape(-1), self.wte16, self.wpe16, h[0], S)
@@ -615,7 +632,7 @@ class B200Engine:
         ops.layernorm_bwd(dln, h[i], w.g1, lw["m1"], lw["r1"], dhmid, dh, w.d_g1, w.d_b1)
 
     # ---------------------------------------------------------------- protocol
-    def _fwd_bwd_eager(self, ids: torch.Tensor, grad_scale: float) -> None:
+    def _fwd_bwd_eager(self, ids: torch.Tensor, grad_scale: float, sequence_id: torch.Tensor | None = None) -> None:
         b, S = ids.shape
         ws = self._workspace(b, S)
         targets = shift_labels(ids).reshape(-1)
@@ -624,68 +641,80 @@ class B200Engine:
             self._fp8_prologue(train=True)
         if self.zero3 is not None:
             self.zero3.zero_stage(self.zero3.plan.rest)   # embeddings + final norm collect gradients over the whole backward
-        self._forward(ids, ws)
+        self._forward(ids, ws, sequence_id)
         self._head(ws, targets, grad_scale, train=True)
         self._backward(ids, ws)
 
-    def fwd_bwd(self, ids: torch.Tensor, denom: float, scale: float = 1.0) -> tuple[torch.Tensor, torch.Tensor]:
-        """Accumulate d(Σ token-loss · scale / denom) into ``flat.grads``; returns (loss_sum, n_tokens)."""
+    def fwd_bwd(self, ids: torch.Tensor, denom: float, scale: float = 1.0,
+                sequence_id: torch.Tensor | None = None) -> tuple[torch.Tensor, torch.Tensor]:
+        """Accumulate d(Σ token-loss · scale / denom) into ``flat.grads``; returns (loss_sum, n_tokens). ``sequence_id`` [b, S]
+        (int64, ids non-decreasing along each row): document ids, applied when ``attn_uses_sequence_id`` is on."""
         b, S = ids.shape
+        sequence_id = check_sequence_id(self.cfg, sequence_id, train=True)
+        if sequence_id is not None:
+            sequence_id = sequence_id.to(self.device, torch.int64, non_blocking=True).contiguous()
         grad_scale = scale / denom
         if self.fp8 and not self._fp8_calibrated:
             # delayed scaling has no history yet: one discarded pass at scale 1 records every role's amax (gradients would
             # underflow E5M2 unscaled), the next prologue turns them into scales
             saved = self.flat.grads.clone()
-            self._fwd_bwd_eager(ids, grad_scale)
+            self._fwd_bwd_eager(ids, grad_scale, sequence_id)
             self.flat.grads.copy_(saved)
             self._fp8_calibrated = True
         graphable = self.use_graph and self.attn_mode == "b200" and S % 128 == 0 and not self.collect_activation_stats
         if not graphable:
             n0 = ops.launch_count()
-            self._fwd_bwd_eager(ids, grad_scale)
+            self._fwd_bwd_eager(ids, grad_scale, sequence_id)
             self.launches_per_microbatch = ops.launch_count() - n0
         else:
-            key = (b, S, float(grad_scale))
+            # a graph with the document mask reads a static sequence_id input of its own
+            key = (b, S, float(grad_scale)) if sequence_id is None else (b, S, float(grad_scale), "doc")
             g = self._graphs.get(key)
             if g is None:
-                g = self._capture(ids, grad_scale, key)
+                g = self._capture(ids, grad_scale, key, sequence_id)
             g["ids"].copy_(ids, non_blocking=True)
+            if sequence_id is not None:
+                g["sequence_id"].copy_(sequence_id, non_blocking=True)
             g["graph"].replay()
             ops.add_launch_count(self.launches_per_microbatch)   # replayed launches are still our kernels
         st = self._stats.clone()
         return st[0], st[1]
 
-    def _capture(self, ids: torch.Tensor, grad_scale: float, key: tuple) -> dict[str, Any]:
+    def _capture(self, ids: torch.Tensor, grad_scale: float, key: tuple, sequence_id: torch.Tensor | None = None) -> dict[str, Any]:
         """Warm up eagerly on a side stream (lazy allocations, kernel attributes), then capture one microbatch.
         Gradients accumulate into ``flat.grads`` — they are saved around the warm-up / capture passes."""
         if len(self._graphs) >= 4:      # shapes changed (auto microbatch, eval): drop old graphs with their static inputs
             self._graphs.clear()
         static_ids = ids.clone()
+        static_sid = sequence_id.clone() if sequence_id is not None else None
         saved = self.flat.grads.clone()
         side = torch.cuda.Stream(self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(side):
             n0 = ops.launch_count()
-            self._fwd_bwd_eager(static_ids, grad_scale)
+            self._fwd_bwd_eager(static_ids, grad_scale, static_sid)
             self.launches_per_microbatch = ops.launch_count() - n0
         torch.cuda.current_stream(self.device).wait_stream(side)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
-            self._fwd_bwd_eager(static_ids, grad_scale)
+            self._fwd_bwd_eager(static_ids, grad_scale, static_sid)
         self.flat.grads.copy_(saved)
-        g = {"graph": graph, "ids": static_ids}
+        g = {"graph": graph, "ids": static_ids, "sequence_id": static_sid}
         self._graphs[key] = g
         return g
 
     @torch.no_grad()
-    def eval_stats(self, ids: torch.Tensor) -> dict[str, torch.Tensor]:
+    def eval_stats(self, ids: torch.Tensor, sequence_id: torch.Tensor | None = None) -> dict[str, torch.Tensor]:
         b, S = ids.shape
+        sequence_id = check_sequence_id(self.cfg, sequence_id, train=False)
+        if sequence_id is not None:
+            sequence_id = sequence_id.to(self.device, torch.int64).contiguous()
         ws = self._workspace(b, S)
         targets = shift_labels(ids).reshape(-1)
         self._stats.zero_()
         if self.fp8:
             self._fp8_prologue(train=False)
-        self._forward(ids, ws)
+        self._forward(ids, ws, sequence_id)
         self._head(ws, targets, 0.0, train=False)
         st = self._stats.clone()
         out = {"loss_sum": st[0], "n_tokens": st[1], "n_correct": st[2]}

@@ -40,6 +40,8 @@ class MPTConfig:
     no_bias: bool = False
     learned_pos_emb: bool = True
     norm_eps: float = 1e-5
+    # attn_config.attn_uses_sequence_id: attention stays inside each document of a packed row (the collator's sequence_id)
+    attn_uses_sequence_id: bool = False
     init_std: float | None = None  # None -> kaiming_normal_ (llm-foundry default)
     extra: dict[str, Any] = field(default_factory=dict)
 
@@ -60,6 +62,7 @@ class MPTConfig:
             alibi=bool(attn.pop("alibi", False)), alibi_bias_max=attn.pop("alibi_bias_max", 8),
             rope=bool(attn.pop("rope", False)), rope_theta=float(attn.pop("rope_theta", 10000.0)),
             qk_ln=bool(attn.pop("qk_ln", False)), clip_qkv=attn.pop("clip_qkv", None),
+            attn_uses_sequence_id=bool(attn.pop("attn_uses_sequence_id", False)),
             no_bias=bool(m.pop("no_bias", False)), learned_pos_emb=bool(m.pop("learned_pos_emb", True)),
         )
         for k in ("name", "init_device"):
@@ -121,7 +124,8 @@ class MPTAttention(nn.Module):
             self.k_ln = nn.LayerNorm(d, eps=cfg.norm_eps)
 
     def forward(self, x: torch.Tensor, rope: tuple[torch.Tensor, torch.Tensor] | None,
-                alibi: torch.Tensor | None) -> torch.Tensor:
+                alibi: torch.Tensor | None, doc_keep: torch.Tensor | None = None) -> torch.Tensor:
+        """``doc_keep``: optional bool [B, 1, S, S], True where query and key belong to the same document."""
         cfg = self.cfg
         B, S, d = x.shape
         qkv = self.Wqkv(x)
@@ -140,13 +144,17 @@ class MPTAttention(nn.Module):
             if alibi is not None:
                 att = att + alibi[:, :, :S, :S].to(att.dtype)
             mask = torch.ones(S, S, dtype=torch.bool, device=x.device).tril()
+            if doc_keep is not None:
+                mask = mask & doc_keep
             att = att.masked_fill(~mask, float("-inf"))
             o = torch.softmax(att.float(), dim=-1).to(v.dtype) @ v
         else:
             bias = None
-            if alibi is not None:
+            if alibi is not None or doc_keep is not None:
                 mask = torch.ones(S, S, dtype=torch.bool, device=x.device).tril()
-                bias = alibi[:, :, :S, :S].to(q.dtype).masked_fill(~mask, float("-inf"))
+                if doc_keep is not None:
+                    mask = mask & doc_keep
+                bias = mask if alibi is None else alibi[:, :, :S, :S].to(q.dtype).masked_fill(~mask, float("-inf"))
             o = F.scaled_dot_product_attention(q, k, v, attn_mask=bias, is_causal=bias is None, scale=scale)
         return self.out_proj(o.transpose(1, 2).reshape(B, S, d))
 
@@ -170,8 +178,8 @@ class MPTBlock(nn.Module):
         self.norm_2 = nn.LayerNorm(cfg.d_model, eps=cfg.norm_eps, bias=not cfg.no_bias)
         self.ffn = MPTMLP(cfg)
 
-    def forward(self, x: torch.Tensor, rope: Any, alibi: Any) -> torch.Tensor:
-        x = x + self.attn(self.norm_1(x).to(x.dtype), rope, alibi)
+    def forward(self, x: torch.Tensor, rope: Any, alibi: Any, doc_keep: Any = None) -> torch.Tensor:
+        x = x + self.attn(self.norm_1(x).to(x.dtype), rope, alibi, doc_keep)
         return x + self.ffn(self.norm_2(x).to(x.dtype))
 
 
@@ -249,7 +257,14 @@ class MPTForCausalLM(nn.Module):
             alibi = self._alibi_cache
         return rope, alibi
 
-    def hidden_states(self, input_ids: torch.Tensor) -> torch.Tensor:
+    def doc_keep(self, sequence_id: torch.Tensor | None) -> torch.Tensor | None:
+        """llm-foundry's document mask: bool [B, 1, S, S], True where query and key share a ``sequence_id``; None when
+        ``attn_uses_sequence_id`` is off (a given ``sequence_id`` is then ignored) or no ids are given (plain causal)."""
+        if not self.cfg.attn_uses_sequence_id or sequence_id is None:
+            return None
+        return (sequence_id[:, :, None] == sequence_id[:, None, :])[:, None]
+
+    def hidden_states(self, input_ids: torch.Tensor, sequence_id: torch.Tensor | None = None) -> torch.Tensor:
         t = self.transformer
         B, S = input_ids.shape
         if S > self.cfg.max_seq_len:
@@ -258,23 +273,25 @@ class MPTForCausalLM(nn.Module):
         if self.cfg.learned_pos_emb:
             x = x + t.wpe(torch.arange(S, device=input_ids.device))[None]
         rope, alibi = self._aux(S, input_ids.device)
+        keep = self.doc_keep(sequence_id)
         for blk in t.blocks:
             if self.activation_checkpointing and self.training and torch.is_grad_enabled():
                 from torch.utils.checkpoint import checkpoint
 
-                x = checkpoint(blk, x, rope, alibi, use_reentrant=False)   # keep only block inputs, recompute in backward
+                x = checkpoint(blk, x, rope, alibi, keep, use_reentrant=False)   # keep only block inputs, recompute in backward
             else:
-                x = blk(x, rope, alibi)
+                x = blk(x, rope, alibi, keep)
         return t.norm_f(x).to(x.dtype)
 
-    def forward(self, input_ids: torch.Tensor) -> torch.Tensor:
-        h = self.hidden_states(input_ids)
+    def forward(self, input_ids: torch.Tensor, sequence_id: torch.Tensor | None = None) -> torch.Tensor:
+        h = self.hidden_states(input_ids, sequence_id)
         return F.linear(h, self.transformer.wte.weight.to(h.dtype))
 
     def loss(self, input_ids: torch.Tensor, labels: torch.Tensor | None = None,
-             reduction: str = "mean") -> tuple[torch.Tensor, torch.Tensor]:
-        """Returns (loss, n_valid_tokens). Targets are shifted *inside* (ref semantics)."""
-        logits = self.forward(input_ids)
+             reduction: str = "mean", sequence_id: torch.Tensor | None = None) -> tuple[torch.Tensor, torch.Tensor]:
+        """Returns (loss, n_valid_tokens). Targets are shifted *inside* (ref semantics); the target that crosses a document
+        boundary stays in the loss."""
+        logits = self.forward(input_ids, sequence_id)
         targets = shift_labels(input_ids if labels is None else labels)
         flat = F.cross_entropy(logits.float().view(-1, logits.shape[-1]), targets.view(-1),
                                ignore_index=-100, reduction="sum")
@@ -287,6 +304,17 @@ def shift_labels(labels: torch.Tensor) -> torch.Tensor:
     t = torch.roll(labels, shifts=-1, dims=1).clone()
     t[:, -1] = -100
     return t
+
+
+def check_sequence_id(cfg: MPTConfig, sequence_id: torch.Tensor | None, train: bool) -> torch.Tensor | None:
+    """The ``sequence_id`` a backend should apply: None when ``attn_uses_sequence_id`` is off (ids are ignored). With it on, a
+    training batch must carry ids (llm-foundry raises the same in train mode); an eval batch without them is plain causal."""
+    if not cfg.attn_uses_sequence_id:
+        return None
+    if sequence_id is None and train:
+        raise ValueError("sequence_id is required to train with attn_config.attn_uses_sequence_id=true "
+                         "(set dataset.eos_token_id or dataset.bos_token_id so the collator emits it)")
+    return sequence_id
 
 
 def build_model(model_cfg: dict[str, Any] | MPTConfig, device: Any = None, seed: int | None = None,

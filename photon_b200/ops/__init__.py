@@ -255,15 +255,25 @@ def fused_optimizer_step(opt: Any, lr: float, grad_mult: torch.Tensor | float | 
 
 # ---------------------------------------------------------------------------- attention
 def attention_fwd(qkv: torch.Tensor, out: torch.Tensor, lse: torch.Tensor, n_heads: int, scale: float, causal: bool = True,
-                  alibi_slopes: torch.Tensor | None = None) -> None:
-    """``alibi_slopes``: optional fp32 [n_heads]; adds ``slope_h * (key - query)`` to the scores (MPT ``attn_config.alibi``)."""
-    ext().attention_fwd(qkv, out, lse, int(n_heads), float(scale), bool(causal), alibi_slopes)
+                  alibi_slopes: torch.Tensor | None = None, doc_start: torch.Tensor | None = None) -> None:
+    """``alibi_slopes``: optional fp32 [n_heads]; adds ``slope_h * (key - query)`` to the scores (MPT ``attn_config.alibi``).
+    ``doc_start``: optional int32 [B*S] from :func:`doc_bounds` (causal only); query ``q`` then sees key ``k`` iff
+    ``doc_start[q] <= k <= q``, and key tiles before a query tile's first document are skipped."""
+    ext().attention_fwd(qkv, out, lse, int(n_heads), float(scale), bool(causal), alibi_slopes, doc_start)
 
 
 def attention_bwd(qkv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor, dqkv: torch.Tensor,
                   delta: torch.Tensor, n_heads: int, scale: float, causal: bool = True,
-                  alibi_slopes: torch.Tensor | None = None) -> None:
-    ext().attention_bwd(qkv, out, dout, lse, dqkv, delta, int(n_heads), float(scale), bool(causal), alibi_slopes)
+                  alibi_slopes: torch.Tensor | None = None, doc_start: torch.Tensor | None = None,
+                  doc_end: torch.Tensor | None = None) -> None:
+    """``doc_start`` / ``doc_end`` (both or neither): the document mask of :func:`attention_fwd`."""
+    ext().attention_bwd(qkv, out, dout, lse, dqkv, delta, int(n_heads), float(scale), bool(causal), alibi_slopes, doc_start, doc_end)
+
+
+def doc_bounds(sequence_id: torch.Tensor, doc_start: torch.Tensor, doc_end: torch.Tensor) -> None:
+    """``sequence_id`` int64 [B, S] -> ``doc_start`` / ``doc_end`` int32 [B*S]: the first / last row (within its sequence) of
+    each row's document. Documents are maximal runs of equal ids."""
+    ext().doc_bounds(sequence_id, doc_start, doc_end)
 
 
 def rope_(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_heads: int, inverse: bool = False) -> torch.Tensor:

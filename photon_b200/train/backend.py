@@ -12,9 +12,11 @@ Trainer does not care which one it drives.
 Protocol
 --------
 ``flat``                      :class:`FlatParams` (fp32 master params + grads)
-``fwd_bwd(ids, denom, scale)``  accumulate d(Σ token-loss · scale / denom) into ``flat.grads``;
+``fwd_bwd(ids, denom, scale[, sequence_id])``  accumulate d(Σ token-loss · scale / denom) into ``flat.grads``;
                               returns device scalars ``(loss_sum, n_tokens)``
-``eval_stats(ids)``           ``{"loss_sum","n_tokens","n_correct"[, "unigram_loss_sum"]}``
+``eval_stats(ids[, sequence_id])``  ``{"loss_sum","n_tokens","n_correct"[, "unigram_loss_sum"]}``
+                              (``sequence_id``: the collator's per-token document ids, applied when the model's
+                              ``attn_uses_sequence_id`` is on)
 ``params_updated()``          hook after optimizer / parameter load (refresh shadows)
 """
 from __future__ import annotations
@@ -25,7 +27,7 @@ from typing import Any
 import torch
 import torch.nn.functional as F
 
-from photon_b200.models.mpt import MPTConfig, MPTForCausalLM, shift_labels
+from photon_b200.models.mpt import MPTConfig, MPTForCausalLM, check_sequence_id, shift_labels
 from photon_b200.utils.flat import FlatParams
 
 
@@ -89,9 +91,11 @@ class TorchBackend:
         self.launches_per_microbatch = 0  # stock torch ops are not "our" kernels
 
     # -- training ---------------------------------------------------------------------
-    def fwd_bwd(self, ids: torch.Tensor, denom: float, scale: float = 1.0) -> tuple[torch.Tensor, torch.Tensor]:
+    def fwd_bwd(self, ids: torch.Tensor, denom: float, scale: float = 1.0,
+                sequence_id: torch.Tensor | None = None) -> tuple[torch.Tensor, torch.Tensor]:
+        sequence_id = check_sequence_id(self.cfg, sequence_id, train=True)
         with autocast_ctx(self.device, self.precision):
-            loss_sum, n = self.model.loss(ids, reduction="sum")
+            loss_sum, n = self.model.loss(ids, reduction="sum", sequence_id=sequence_id)
         (loss_sum * (scale / denom)).backward()
         if self.collect_activation_stats:
             self._act_stats(ids)
@@ -111,9 +115,9 @@ class TorchBackend:
 
     # -- evaluation -------------------------------------------------------------------
     @torch.no_grad()
-    def eval_stats(self, ids: torch.Tensor) -> dict[str, torch.Tensor]:
+    def eval_stats(self, ids: torch.Tensor, sequence_id: torch.Tensor | None = None) -> dict[str, torch.Tensor]:
         with autocast_ctx(self.device, self.precision):
-            logits = self.model(ids)
+            logits = self.model(ids, check_sequence_id(self.cfg, sequence_id, train=False))
         targets = shift_labels(ids)
         lf = logits.float().view(-1, logits.shape[-1])
         tf = targets.view(-1)

@@ -95,6 +95,16 @@ def shard_bounds(total: int, world_size: int, align: int = 256) -> list[tuple[in
     return [(min(total, r * per), min(total, (r + 1) * per)) for r in range(world_size)]
 
 
+def check_sequence_id_runs(sequence_id: torch.Tensor) -> None:
+    """The document-masked attention kernels take documents as maximal runs of equal ids; the collator's ids are
+    non-decreasing along each row, so a host batch whose ids decrease anywhere did not come from it and is rejected."""
+    if sequence_id.dim() != 2:
+        raise ValueError(f"sequence_id must be [batch, seq_len], got shape {tuple(sequence_id.shape)}")
+    if sequence_id.shape[1] > 1 and bool((sequence_id[:, 1:] < sequence_id[:, :-1]).any()):
+        raise ValueError("sequence_id must be non-decreasing along each row (documents as runs of equal ids, as the "
+                         "text collator emits them)")
+
+
 def _is_oom(e: BaseException) -> bool:
     return isinstance(e, torch.cuda.OutOfMemoryError) or "out of memory" in str(e).lower()
 
@@ -259,9 +269,15 @@ class Trainer:
         return v
 
     # ------------------------------------------------------------------ training
+    def _uses_sequence_id(self) -> bool:
+        return bool(getattr(self.model_cfg, "attn_uses_sequence_id", False))
+
     def _train_batch(self, batch: dict[str, torch.Tensor]) -> None:
         st = self.state
         ids_host = batch["input_ids"]
+        sid_host = batch.get("sequence_id")
+        if sid_host is not None and self._uses_sequence_id():
+            check_sequence_id_runs(sid_host)
         B, S = ids_host.shape
         n_tok_target = float(B * (S - 1))  # packed sequences: only the last position is ignored
         scale = self.scaler.scale if self.scaler else 1.0
@@ -276,7 +292,8 @@ class Trainer:
                 uni_sum = torch.zeros((), device=self.device, dtype=torch.float32) if uni_logp is not None else None
                 for lo in range(0, B, mb):
                     ids = self._to_device(ids_host[lo:lo + mb])
-                    ls, n = st.backend.fwd_bwd(ids, n_tok_target, scale)
+                    kw = {} if sid_host is None else {"sequence_id": self._to_device(sid_host[lo:lo + mb])}
+                    ls, n = st.backend.fwd_bwd(ids, n_tok_target, scale, **kw)
                     loss_sum += ls.float()
                     n_tok += n.float() if torch.is_tensor(n) else float(n)
                     if uni_sum is not None:  # CE of the unigram model needs the targets only (K15: no second pass over logits)
@@ -420,7 +437,10 @@ class Trainer:
                 if 0 <= limit <= i:
                     break
                 ids = self._to_device(batch["input_ids"])
-                stats = self._eval_batch_stats(ids)
+                sid = batch.get("sequence_id")
+                if sid is not None and self._uses_sequence_id():
+                    check_sequence_id_runs(sid)
+                stats = self._eval_batch_stats(ids, None if sid is None else self._to_device(sid))
                 for m in metrics.values():
                     m.update(stats)
                 st.eval_timestamp.advance_batch(samples=ids.shape[0] * self.world_size,
@@ -454,9 +474,10 @@ class Trainer:
         finally:
             decoder.close()
 
-    def _eval_batch_stats(self, ids: torch.Tensor) -> dict[str, float]:
+    def _eval_batch_stats(self, ids: torch.Tensor, sequence_id: torch.Tensor | None = None) -> dict[str, float]:
         """Sum-type statistics of one eval batch, computed in ``device_eval_microbatch_size`` slices (``auto`` halves the
-        slice on an out-of-memory error and remembers the size that worked — same policy as the train microbatch)."""
+        slice on an out-of-memory error and remembers the size that worked — same policy as the train microbatch).
+        ``sequence_id`` (the collator's document ids) is sliced with ``ids`` and passed on only when given."""
         B = ids.shape[0]
         while True:
             mb = self.eval_microbatch
@@ -464,7 +485,8 @@ class Trainer:
             try:
                 total: dict[str, float] = {}
                 for lo in range(0, B, mb):
-                    for k, v in self.state.backend.eval_stats(ids[lo:lo + mb]).items():
+                    kw = {} if sequence_id is None else {"sequence_id": sequence_id[lo:lo + mb]}
+                    for k, v in self.state.backend.eval_stats(ids[lo:lo + mb], **kw).items():
                         total[k] = total.get(k, 0.0) + float(v)
                 return total
             except RuntimeError as e:
