@@ -41,6 +41,17 @@ inline void check_f32(const Tensor& t, const char* name) {
   TORCH_CHECK(t.scalar_type() == at::kFloat, name, " must be float32");
 }
 inline const void* opt_ptr(const c10::optional<Tensor>& t) { return t.has_value() ? t->data_ptr() : nullptr; }
+// The fused memory-bound kernels read and write rows as `bytes`-wide vectors (16: uint4 / float4, 8: four fp8 bytes as uint2):
+// the base pointer and, for a 2-D operand, the row stride must be multiples of that width. Checked before any launch, since a
+// misaligned vector access faults the device instead of raising.
+inline void check_vec(const Tensor& t, const char* op, const char* name, int bytes = 16) {
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(t.data_ptr()) % bytes) == 0, op, ": ", name, " must start on a ", bytes, "-byte boundary");
+  TORCH_CHECK(t.dim() < 2 || (t.stride(0) * t.element_size()) % bytes == 0, op, ": the row stride of ", name, " must be a multiple of ",
+              bytes, " bytes");
+}
+inline void check_numel(const Tensor& t, int64_t n, const char* op, const char* name) {
+  TORCH_CHECK(t.numel() == n, op, ": ", name, " must have ", n, " elements, not ", t.numel());
+}
 
 #define CUDA_OK(expr)                                                                        \
   do {                                                                                       \
@@ -205,8 +216,22 @@ void layernorm_fwd_q8(const Tensor& x, const Tensor& gamma, const c10::optional<
   TORCH_CHECK(x.is_contiguous() && y8.is_contiguous() && is_byte(y8) && y8.numel() == x.numel(), "layernorm_fwd_q8: y8 must be a contiguous 1-byte tensor shaped like x");
   const int64_t nr = meta.size(1);
   TORCH_CHECK(meta.dim() == 2 && meta.size(0) == 3 && role >= 0 && role < nr, "bad meta / role");
-  c10::cuda::CUDAGuard guard(x.device());
   const int d = int(x.size(-1));
+  const int64_t T = x.numel() / d;
+  check_f32(mean, "mean");
+  check_f32(rstd, "rstd");
+  check_numel(gamma, d, "layernorm_fwd_q8", "gamma");
+  check_numel(mean, T, "layernorm_fwd_q8", "mean");
+  check_numel(rstd, T, "layernorm_fwd_q8", "rstd");
+  check_vec(x, "layernorm_fwd_q8", "x");
+  check_vec(gamma, "layernorm_fwd_q8", "gamma");
+  check_vec(y8, "layernorm_fwd_q8", "y8", 8);
+  if (beta.has_value()) {
+    check_f32(*beta, "beta");
+    check_numel(*beta, d, "layernorm_fwd_q8", "beta");
+    check_vec(*beta, "layernorm_fwd_q8", "beta");
+  }
+  c10::cuda::CUDAGuard guard(x.device());
   float* m = meta.data_ptr<float>();
   pb::layernorm_fwd_q8(x.data_ptr(), gamma.data_ptr<float>(), beta.has_value() ? beta->data_ptr<float>() : nullptr, y8.data_ptr(),
                        mean.data_ptr<float>(), rstd.data_ptr<float>(), x.numel() / d, d, float(eps), m + role, m + 2 * nr + role, stream_of(x));
@@ -216,6 +241,12 @@ void layernorm_fwd_q8(const Tensor& x, const Tensor& gamma, const c10::optional<
 void colsum_quant(const Tensor& dy, c10::optional<Tensor> out_sum, c10::optional<Tensor> y8, int fmt, c10::optional<Tensor> meta, int role) {
   check_bf16(dy, "dy");
   TORCH_CHECK(dy.dim() == 2 && dy.stride(1) == 1, "colsum_quant expects [T,N] with unit inner stride");
+  check_vec(dy, "colsum_quant", "dy");
+  if (y8.has_value()) check_vec(*y8, "colsum_quant", "y8", 8);
+  if (out_sum.has_value()) {
+    check_f32(*out_sum, "out_sum");
+    check_numel(*out_sum, dy.size(1), "colsum_quant", "out_sum");
+  }
   c10::cuda::CUDAGuard guard(dy.device());
   const float* scale = nullptr;
   float* amax = nullptr;
@@ -232,7 +263,6 @@ void colsum_quant(const Tensor& dy, c10::optional<Tensor> out_sum, c10::optional
     amax = meta->data_ptr<float>() + 2 * nr + role;
     y = y8->data_ptr(), ld8 = y8->stride(0);
   }
-  if (out_sum.has_value()) check_f32(*out_sum, "out_sum");
   pb::colsum_quant(dy.data_ptr(), dy.stride(0), out_sum.has_value() ? out_sum->data_ptr<float>() : nullptr, y, ld8, fmt, scale, amax,
                    dy.size(0), int(dy.size(1)), stream_of(dy));
   g_launches += 1;
@@ -539,9 +569,19 @@ void embed_fwd(const Tensor& ids, const Tensor& wte, const c10::optional<Tensor>
   TORCH_CHECK(ids.scalar_type() == at::kLong && ids.is_contiguous(), "ids must be contiguous int64");
   check_bf16(wte, "wte");
   check_bf16(out, "out");
+  TORCH_CHECK(wte.dim() == 2 && wte.is_contiguous() && wte.size(1) % 8 == 0, "embed_fwd: wte must be contiguous [V,d], d % 8 == 0");
+  const int d = int(wte.size(1));
+  TORCH_CHECK(out.is_contiguous() && out.numel() == ids.numel() * d, "embed_fwd: out must be contiguous [T,d]");
+  TORCH_CHECK(S > 0, "embed_fwd: seq_len must be positive");
+  check_vec(wte, "embed_fwd", "wte");
+  check_vec(out, "embed_fwd", "out");
+  if (wpe.has_value()) {
+    check_bf16(*wpe, "wpe");
+    TORCH_CHECK(wpe->dim() == 2 && wpe->size(1) == d && wpe->size(0) >= S && wpe->is_contiguous(), "embed_fwd: wpe must be contiguous [>=S,d]");
+    check_vec(*wpe, "embed_fwd", "wpe");
+  }
   c10::cuda::CUDAGuard guard(ids.device());
-  pb::embed_fwd(ids.data_ptr<int64_t>(), wte.data_ptr(), opt_ptr(wpe), out.data_ptr(), ids.numel(), S, int(wte.size(1)),
-                int(wte.size(0)), stream_of(ids));
+  pb::embed_fwd(ids.data_ptr<int64_t>(), wte.data_ptr(), opt_ptr(wpe), out.data_ptr(), ids.numel(), S, d, int(wte.size(0)), stream_of(ids));
   g_launches += 1;
 }
 // dwte / dwpe: either may be None (a frozen embedding); the kernel of a missing one is not launched
@@ -551,14 +591,17 @@ void embed_bwd(const Tensor& ids, const Tensor& dh, c10::optional<Tensor> dwte, 
   check_bf16(dh, "dh");
   TORCH_CHECK(dh.dim() == 2 && dh.is_contiguous() && dh.size(0) == ids.numel() && dh.size(1) % 8 == 0, "dh must be contiguous [T,d], d % 8 == 0");
   TORCH_CHECK(S > 0 && ids.numel() % S == 0, "the token count must be a multiple of seq_len");
+  check_vec(dh, "embed_bwd", "dh");
   const int d = int(dh.size(1));
   if (dwte.has_value()) {
     check_f32(*dwte, "dwte");
     TORCH_CHECK(dwte->dim() == 2 && dwte->size(1) == d && dwte->is_contiguous(), "dwte must be contiguous [V,d]");
+    check_vec(*dwte, "embed_bwd", "dwte");
   }
   if (dwpe.has_value()) {
     check_f32(*dwpe, "dwpe");
     TORCH_CHECK(dwpe->dim() == 2 && dwpe->size(1) == d && dwpe->size(0) >= S && dwpe->is_contiguous(), "dwpe must be contiguous [>=S,d]");
+    check_vec(*dwpe, "embed_bwd", "dwpe");
   }
   c10::cuda::CUDAGuard guard(ids.device());
   pb::embed_bwd(ids.data_ptr<int64_t>(), dh.data_ptr(), dwte.has_value() ? dwte->data_ptr<float>() : nullptr,
@@ -575,11 +618,39 @@ void transpose_u8(const Tensor& src, Tensor& dst) {
   pb::transpose_u8(src.data_ptr(), src.stride(0), dst.data_ptr(), int(src.size(0)), int(src.size(1)), stream_of(src));
   g_launches += 1;
 }
-void layernorm_fwd(const Tensor& x, const Tensor& gamma, const c10::optional<Tensor>& beta, Tensor& y, Tensor& mean, Tensor& rstd,
-                   double eps) {
+// gamma / beta: fp32 [d]; mean / rstd: fp32 [T] with T = x.numel() / d; y / dx / dres shaped like x
+void check_layernorm(const char* op, const Tensor& x, const Tensor& gamma, const c10::optional<Tensor>& beta, const Tensor& mean,
+                     const Tensor& rstd) {
   check_bf16(x, "x");
   check_f32(gamma, "gamma");
-  TORCH_CHECK(x.is_contiguous() && y.is_contiguous(), "layernorm tensors must be contiguous");
+  check_f32(mean, "mean");
+  check_f32(rstd, "rstd");
+  TORCH_CHECK(x.dim() >= 1 && x.is_contiguous(), op, ": x must be contiguous");
+  const int64_t d = x.size(-1);
+  TORCH_CHECK(d > 0, op, ": empty rows");
+  const int64_t T = x.numel() / d;
+  check_numel(gamma, d, op, "gamma");
+  check_numel(mean, T, op, "mean");
+  check_numel(rstd, T, op, "rstd");
+  TORCH_CHECK(gamma.is_contiguous() && mean.is_contiguous() && rstd.is_contiguous(), op, ": gamma, mean and rstd must be contiguous");
+  check_vec(x, op, "x");
+  check_vec(gamma, op, "gamma");
+  if (beta.has_value()) {
+    check_f32(*beta, "beta");
+    check_numel(*beta, d, op, "beta");
+    TORCH_CHECK(beta->is_contiguous(), op, ": beta must be contiguous");
+    check_vec(*beta, op, "beta");
+  }
+}
+void check_like_x(const char* op, const Tensor& t, const Tensor& x, const char* name) {
+  check_bf16(t, name);
+  TORCH_CHECK(t.is_contiguous() && t.numel() == x.numel() && t.size(-1) == x.size(-1), op, ": ", name, " must be contiguous and shaped like x");
+  check_vec(t, op, name);
+}
+void layernorm_fwd(const Tensor& x, const Tensor& gamma, const c10::optional<Tensor>& beta, Tensor& y, Tensor& mean, Tensor& rstd,
+                   double eps) {
+  check_layernorm("layernorm_fwd", x, gamma, beta, mean, rstd);
+  check_like_x("layernorm_fwd", y, x, "y");
   c10::cuda::CUDAGuard guard(x.device());
   const int d = int(x.size(-1));
   pb::layernorm_fwd(x.data_ptr(), gamma.data_ptr<float>(), beta.has_value() ? beta->data_ptr<float>() : nullptr, y.data_ptr(),
@@ -588,11 +659,18 @@ void layernorm_fwd(const Tensor& x, const Tensor& gamma, const c10::optional<Ten
 }
 void layernorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& gamma, const Tensor& mean, const Tensor& rstd,
                    const c10::optional<Tensor>& dres, Tensor& dx, c10::optional<Tensor> dgamma, c10::optional<Tensor> dbeta) {
-  check_bf16(dy, "dy");
-  check_bf16(x, "x");
-  TORCH_CHECK(dy.is_contiguous() && x.is_contiguous() && dx.is_contiguous(), "layernorm tensors must be contiguous");
-  c10::cuda::CUDAGuard guard(x.device());
+  check_layernorm("layernorm_bwd", x, gamma, c10::nullopt, mean, rstd);
+  check_like_x("layernorm_bwd", dy, x, "dy");
+  check_like_x("layernorm_bwd", dx, x, "dx");
+  if (dres.has_value()) check_like_x("layernorm_bwd", *dres, x, "dres");
   const int d = int(x.size(-1));
+  for (const auto* t : {&dgamma, &dbeta}) {
+    if (!t->has_value()) continue;
+    check_f32(**t, "dgamma / dbeta");
+    check_numel(**t, d, "layernorm_bwd", "dgamma / dbeta");
+    TORCH_CHECK((*t)->is_contiguous(), "layernorm_bwd: dgamma / dbeta must be contiguous");
+  }
+  c10::cuda::CUDAGuard guard(x.device());
   pb::layernorm_bwd(dy.data_ptr(), x.data_ptr(), gamma.data_ptr<float>(), mean.data_ptr<float>(), rstd.data_ptr<float>(), opt_ptr(dres),
                     dx.data_ptr(), dgamma.has_value() ? dgamma->data_ptr<float>() : nullptr,
                     dbeta.has_value() ? dbeta->data_ptr<float>() : nullptr, x.numel() / d, d, stream_of(x));
@@ -602,6 +680,10 @@ void col_sum(const Tensor& dy, Tensor& out) {
   check_bf16(dy, "dy");
   check_f32(out, "out");
   TORCH_CHECK(dy.dim() == 2 && dy.stride(1) == 1, "col_sum expects [T,N] with unit inner stride");
+  TORCH_CHECK(dy.size(1) % 8 == 0, "col_sum: the row length must be a multiple of 8");
+  TORCH_CHECK(out.is_contiguous(), "col_sum: out must be contiguous");
+  check_numel(out, dy.size(1), "col_sum", "out");
+  check_vec(dy, "col_sum", "dy");
   c10::cuda::CUDAGuard guard(dy.device());
   pb::col_reduce(dy.data_ptr(), dy.stride(0), nullptr, nullptr, nullptr, out.data_ptr<float>(), nullptr, dy.size(0), int(dy.size(1)),
                  stream_of(dy));
@@ -612,15 +694,30 @@ void cross_entropy(Tensor& logits, const Tensor& targets, double grad_scale, boo
   check_bf16(logits, "logits");
   TORCH_CHECK(logits.dim() == 2 && logits.stride(1) == 1, "logits must be [rows,V]");
   TORCH_CHECK(targets.scalar_type() == at::kLong && targets.is_contiguous(), "targets must be contiguous int64");
+  TORCH_CHECK(targets.numel() == logits.size(0), "cross_entropy: one target per row of logits");
   TORCH_CHECK(stats.scalar_type() == at::kDouble && stats.numel() >= 4, "stats must be float64[>=4]");
+  check_cuda(targets, "targets");
+  check_cuda(stats, "stats");
+  check_vec(logits, "cross_entropy", "logits");
+  if (row_lse.has_value()) {
+    check_f32(*row_lse, "row_lse");
+    TORCH_CHECK(row_lse->is_contiguous() && row_lse->numel() >= logits.size(0), "cross_entropy: row_lse must be contiguous [>=rows]");
+  }
+  if (unigram_logp.has_value()) {
+    check_f32(*unigram_logp, "unigram_logp");
+    TORCH_CHECK(unigram_logp->is_contiguous() && unigram_logp->numel() >= logits.size(1), "cross_entropy: unigram_logp must be contiguous [>=V]");
+  }
   c10::cuda::CUDAGuard guard(logits.device());
   pb::cross_entropy(logits.data_ptr(), logits.stride(0), targets.data_ptr<int64_t>(), logits.size(0), int(logits.size(1)), float(grad_scale),
                     write_grad, stats.data_ptr<double>(), row_lse.has_value() ? row_lse->data_ptr<float>() : nullptr,
                     unigram_logp.has_value() ? unigram_logp->data_ptr<float>() : nullptr, stream_of(logits));
   g_launches += 1;
 }
+// any length: the kernel reads float4s and then the last numel % 4 elements
 void flat_l2_norm(const Tensor& x, Tensor& scratch_f64, Tensor& out_f32) {
   check_f32(x, "x");
+  TORCH_CHECK(x.is_contiguous(), "flat_l2_norm: x must be contiguous");
+  check_vec(x, "flat_l2_norm", "x");
   c10::cuda::CUDAGuard guard(x.device());
   cudaStream_t st = stream_of(x);
   CUDA_OK(cudaMemsetAsync(scratch_f64.data_ptr(), 0, sizeof(double), st));
@@ -650,13 +747,29 @@ void fused_optimizer(Tensor& p, const Tensor& g, Tensor& m, Tensor& v, c10::opti
   check_f32(p, "p");
   check_f32(g, "g");
   TORCH_CHECK(p.numel() % 4 == 0, "flat buffers must be multiples of 4 elements");
+  // every plane the kernel touches is read / written as float4 (the shadow as 4 bf16) at the same index as p
+  std::vector<std::pair<const Tensor*, const char*>> planes{{&p, "p"}, {&g, "g"}};
+  if (kind != 2) planes.push_back({&m, "m"}), planes.push_back({&v, "v"});   // SGD keeps no moments
+  for (auto& [t, name] : planes) {
+    if (t != &p) check_f32(*t, name);
+    TORCH_CHECK(t->is_contiguous(), "fused_optimizer: ", name, " must be contiguous");
+    check_numel(*t, p.numel(), "fused_optimizer", name);
+    check_vec(*t, "fused_optimizer", name);
+  }
+  if (shadow.has_value()) {
+    check_bf16(*shadow, "shadow");
+    TORCH_CHECK(shadow->is_contiguous(), "fused_optimizer: shadow must be contiguous");
+    check_numel(*shadow, p.numel(), "fused_optimizer", "shadow");
+    check_vec(*shadow, "fused_optimizer", "shadow", 8);
+  }
+  if (grad_mult.has_value()) check_f32(*grad_mult, "grad_mult");
   c10::cuda::CUDAGuard guard(p.device());
   pb::OptimHyper h;
   h.kind = kind, h.first_step = first_step ? 1 : 0;
   h.lr = float(lr), h.beta1 = float(beta1), h.beta2 = float(beta2), h.eps = float(eps), h.decay = float(decay);
   h.clip = std::isfinite(clip) ? float(clip) : std::numeric_limits<float>::infinity();
   h.step_size = float(step_size), h.inv_sqrt_bc2 = float(inv_sqrt_bc2);
-  pb::fused_optimizer(p.data_ptr<float>(), g.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
+  pb::fused_optimizer(p.data_ptr<float>(), g.data_ptr<float>(), kind != 2 ? m.data_ptr<float>() : nullptr, kind != 2 ? v.data_ptr<float>() : nullptr,
                       shadow.has_value() ? shadow->data_ptr() : nullptr, p.numel(), h,
                       grad_mult.has_value() ? grad_mult->data_ptr<float>() : nullptr, stream_of(p));
   g_launches += 1;

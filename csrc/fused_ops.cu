@@ -9,6 +9,7 @@
 #include <stdint.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cstdlib>
 #include <stdexcept>
 #include <string>
@@ -582,6 +583,7 @@ __global__ void __launch_bounds__(512) ce_smem_kernel(__nv_bfloat16* __restrict_
 }
 
 // ------------------------------------------------------------------ flat helpers
+// sum x[i]^2 over all n elements: float4 body, and the last n % 4 elements (a slice of a padded buffer) by block 0
 __global__ void sqnorm_kernel(const float* __restrict__ x, long long n, double* __restrict__ out) {
   __shared__ float sh[32];
   float acc = 0.f;
@@ -589,6 +591,10 @@ __global__ void sqnorm_kernel(const float* __restrict__ x, long long n, double* 
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     const float4 v = reinterpret_cast<const float4*>(x)[i];
     acc += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
+  }
+  if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
+    const float t = x[n4 * 4 + threadIdx.x];
+    acc += t * t;
   }
   acc = warp_sum(acc);
   if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = acc;
@@ -738,13 +744,20 @@ void cross_entropy(void* logits, long long ld, const int64_t* targets, long long
   if (V % 8) throw std::runtime_error("cross_entropy: V must be a multiple of 8");
   const size_t row_bytes = size_t(V) * 2;
   static const bool smem_path = [] { const char* e = std::getenv("PB_CE_SMEM"); return !(e && e[0] == '0'); }();
-  if (smem_path && row_bytes <= 200 * 1024 && (ld * 2) % 16 == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0) {
-    // the row lives in shared memory between the two passes: one HBM read of the logits instead of two
-    static bool configured = false;
-    if (!configured) {
-      cudaError_t e = cudaFuncSetAttribute(ce_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  // Both kernels move the row in 16-byte pieces, so the binding has already required a 16-byte aligned base and a row stride
+  // that is a multiple of 8. ce_kernel (two reads of the row from HBM) therefore runs only for rows over 200 KiB (V > 102400)
+  // or under PB_CE_SMEM=0.
+  if (smem_path && row_bytes <= 200 * 1024) {
+    // the row lives in shared memory between the two passes: one HBM read of the logits instead of two. The opt-in to more
+    // than 48 KiB of dynamic shared memory is a per-device attribute of the kernel, so it is set once on each device.
+    static std::atomic<bool> configured[64];
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess || dev < 0 || dev >= 64) throw std::runtime_error("cross_entropy: no usable current device");
+    if (!configured[dev].load()) {
+      e = cudaFuncSetAttribute(ce_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
       if (e != cudaSuccess) throw std::runtime_error(std::string("cross_entropy smem attr: ") + cudaGetErrorString(e));
-      configured = true;
+      configured[dev].store(true);
     }
     ce_smem_kernel<<<int(rows), 512, row_bytes, st>>>((__nv_bfloat16*)logits, ld, targets, V, grad_scale, write_grad ? 1 : 0, stats, row_lse,
                                                       unigram_logp);

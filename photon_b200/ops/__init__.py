@@ -197,7 +197,10 @@ _NORM_SCRATCH: dict[int, tuple[torch.Tensor, torch.Tensor]] = {}
 
 
 def flat_l2_norm(x: torch.Tensor) -> torch.Tensor:
-    """‖x‖₂ of a flat fp32 buffer as a 0-dim device tensor (no host sync)."""
+    """‖x‖₂ of a flat fp32 buffer as a 0-dim device tensor (no host sync).
+
+    Any length: the kernel reads float4s and then the last ``numel % 4`` elements. ``x`` must be contiguous and start on a
+    16-byte boundary (a slice of a padded flat buffer at a multiple of 4 elements); anything else raises."""
     key = x.device.index or 0
     if key not in _NORM_SCRATCH:
         _NORM_SCRATCH[key] = (torch.zeros(1, dtype=torch.float64, device=x.device), torch.zeros(1, dtype=torch.float32, device=x.device))
@@ -212,6 +215,8 @@ def axpby_(acc: torch.Tensor, x: torch.Tensor, a: float, b: float) -> torch.Tens
 
 
 def cast_bf16(src: torch.Tensor, dst: torch.Tensor) -> torch.Tensor:
+    """``dst = bf16(src)``, round to nearest even, the same bits as ``src.to(torch.bfloat16)`` (fp32 subnormals are kept, not
+    flushed); the length must be a multiple of 4."""
     ext().cast_bf16(src, dst)
     return dst
 
