@@ -1,14 +1,18 @@
 // Causal flash attention for sm_90a on wgmma tensor cores, accumulators in registers.
 //
-// Forward (attn_fwd_kernel<DH>): one CTA = one (batch, head, 128-query tile), three warpgroups.
-//   warpgroup 0 : TMA producer (one thread) — Q once, then a 2-stage ring of K / V tiles straight out of the fused
-//                 [B*S, 3*d] QKV projection output (no head split / transpose copies); gives its registers away (setmaxnreg)
+// The fused QKV projection output is [B*S, (H + 2*HKV)*DH]: H query heads, then HKV key heads, then HKV value heads. With
+// grouped-query attention (HKV < H) query head h uses kv head h / G, G = H / HKV; HKV = H is multi-head attention.
+//
+// Forward (attn_fwd_kernel<DH>): one CTA = one (batch, query head, 128-query tile), three warpgroups.
+//   warpgroup 0 : TMA producer (one thread) — Q once, then a 2-stage ring of K / V tiles of the head's kv head straight out of
+//                 the fused QKV buffer (no head split / transpose copies); gives its registers away (setmaxnreg)
 //   warpgroups 1, 2: 64 query rows each — S = Q K^T (wgmma, both operands from shared memory, K-major), online softmax in
 //                 registers (log2 domain, quad shuffles for the row max), O += P V with P taken from REGISTERS as the A operand
 //                 (the S accumulator layout converts to the A fragment layout in place) and V consumed MN-major as stored.
 //
-// Backward (attn_bwd_kernel<DH>): one CTA = one (batch, head, 128-key tile) holding K_j, V_j in shared memory; warpgroups 1, 2
-// own 64 key rows each and walk the 64-row query tiles i (causal: those that see the key tile): S^T = K Q^T and dP^T = V dO^T
+// Backward (attn_bwd_kernel<DH>): one CTA = one (batch, kv head, 128-key tile) holding K_j, V_j in shared memory; warpgroups 1, 2
+// own 64 key rows each and walk the 64-row query tiles i (causal: those that see the key tile) of each of the G query heads
+// of the group in turn, so dK / dV of the whole group accumulate in registers (no atomics): S^T = K Q^T and dP^T = V dO^T
 // (shared-memory operands), P^T and dS^T in registers, dV += P^T dO and dK += dS^T Q with the register A operand; dS^T is also
 // staged in shared memory, where it reads as an MN-major dS for dQ = dS K (each warpgroup one half of the head dimension);
 // dQ partial tiles leave through fp32 red.global.add into an accumulator that a last kernel converts to bf16.
@@ -54,10 +58,11 @@ __device__ __forceinline__ void wgmma_pv(float (&o)[DH / 2], const uint32_t (&a)
 
 // DOC (document mask): doc_start [B*S] holds the first row of each row's document (rows of one sequence). Query q sees key k
 // iff doc_start[q] <= k <= q. Key tiles that end before the document of the tile's first row are never loaded.
-template <int DH, bool ALIBI, bool DOC>
+// GQA: HKV < H (grouped-query attention); false compiles the multi-head kernel (HKV == H, the kv head is the query head).
+template <int DH, bool ALIBI, bool DOC, bool GQA>
 __global__ void __launch_bounds__(384, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __restrict__ out, float* __restrict__ lse, int S, int H,
-                float scale, int causal, const float* __restrict__ alibi_slopes, const int* __restrict__ doc_start) {
+                float scale, int causal, const float* __restrict__ alibi_slopes, const int* __restrict__ doc_start, int HKV) {
   using C = FwdCfg<DH>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -75,6 +80,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __rest
   const int qt = n_qt - 1 - int(blockIdx.x);      // heaviest (causal) tiles first
   const int bh = blockIdx.y, b = bh / H, h = bh - b * H;
   const int d_model = H * DH;
+  // the kv head's K / V columns; the multi-head instances keep the multi-head expressions (and so the multi-head code)
+  const int k_col = GQA ? d_model + h / (H / HKV) * DH : d_model + h * DH;
+  const int v_col = GQA ? k_col + HKV * DH : 2 * d_model + h * DH;
   const int n_kv = causal ? qt + 1 : S / BKV;
   const int j0 = DOC ? doc_start[b * S + qt * BQ] / BKV : 0;   // first key tile any row of this query tile sees
   const int wg = threadIdx.x >> 7;
@@ -107,12 +115,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __rest
         mbar_expect_tx(&k_full[st], C::TILE);
 #pragma unroll
         for (int c = 0; c < C::CH; ++c)
-          tma_load_2d(sK + st * C::TILE + c * 16384, &tmQKV, &k_full[st], d_model + h * DH + c * 64, b * S + j * BKV);
+          tma_load_2d(sK + st * C::TILE + c * 16384, &tmQKV, &k_full[st], k_col + c * 64, b * S + j * BKV);
         mbar_wait(&v_empty[st], ph);
         mbar_expect_tx(&v_full[st], C::TILE);
 #pragma unroll
         for (int c = 0; c < C::CH; ++c)
-          tma_load_2d(sV + st * C::TILE + c * 16384, &tmQKV, &v_full[st], 2 * d_model + h * DH + c * 64, b * S + j * BKV);
+          tma_load_2d(sV + st * C::TILE + c * 16384, &tmQKV, &v_full[st], v_col + c * 64, b * S + j * BKV);
       }
     }
     return;
@@ -267,15 +275,16 @@ __global__ void __launch_bounds__(256) attn_bwd_delta_kernel(const __nv_bfloat16
   }
 }
 
-// dq_acc (fp32, [B*S, H*DH]) * scale -> bf16 into the q third of dqkv
-__global__ void attn_bwd_dq_convert_kernel(const float* __restrict__ dq_acc, __nv_bfloat16* __restrict__ dqkv, long long rows, int d, float scale) {
+// dq_acc (fp32, [B*S, H*DH]) * scale -> bf16 into the q columns of dqkv (rows of width w)
+__global__ void attn_bwd_dq_convert_kernel(const float* __restrict__ dq_acc, __nv_bfloat16* __restrict__ dqkv, long long rows, int d, int w,
+                                           float scale) {
   const long long n4 = rows * d / 4;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     const float4 v = reinterpret_cast<const float4*>(dq_acc)[i];
     const long long e = i * 4, r = e / d, c = e % d;
     uint2 o;
     o.x = pack_bf16(v.x * scale, v.y * scale), o.y = pack_bf16(v.z * scale, v.w * scale);
-    *reinterpret_cast<uint2*>(dqkv + r * 3 * d + c) = o;
+    *reinterpret_cast<uint2*>(dqkv + r * w + c) = o;
   }
 }
 
@@ -296,13 +305,13 @@ __device__ __forceinline__ void wgmma_acc_rs(float (&d)[DH / 2], const uint32_t 
 }
 
 // DOC: as in the forward; doc_end [B*S] holds the last row of each row's document, so the query walk of a key tile stops at
-// the 64-row tile holding the end of its last key's document.
-template <int DH, bool ALIBI, bool DOC>
+// the 64-row tile holding the end of its last key's document. GQA: as in the forward.
+template <int DH, bool ALIBI, bool DOC, bool GQA>
 __global__ void __launch_bounds__(384, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
                 const float* __restrict__ lse, const float* __restrict__ delta, __nv_bfloat16* __restrict__ dqkv, int S, int H, float scale,
                 int causal, float* __restrict__ dq_acc, const float* __restrict__ alibi_slopes, const int* __restrict__ doc_start,
-                const int* __restrict__ doc_end) {
+                const int* __restrict__ doc_end, int HKV) {
   using C = BwdCfg<DH>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -317,8 +326,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
   uint64_t* q_empty = bars + 3;          // [2]
 
   const int jt = int(gridDim.x) - 1 - int(blockIdx.x);   // causal: small key tiles see the most query tiles - start them first
-  const int bh = blockIdx.y, b = bh / H, h = bh - b * H;
+  const int hkv = GQA ? HKV : H;                          // the multi-head instances keep the multi-head expressions
+  const int bk = blockIdx.y, b = bk / hkv, hk = bk - b * hkv;
+  const int G = GQA ? H / hkv : 1, h0 = hk * G;           // query heads h0 .. h0 + G - 1 read this kv head
   const int d_model = H * DH;
+  const int k_col = d_model + hk * DH, v_col = GQA ? k_col + HKV * DH : 2 * d_model + hk * DH;
   const int i0 = causal ? jt * 2 : 0;                      // 64-row query tiles
   const int n_q = DOC ? doc_end[b * S + jt * 128 + 127] / 64 + 1 : S / 64;
   const int wg = threadIdx.x >> 7;
@@ -343,17 +355,19 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
       mbar_expect_tx(kv_full, 2 * C::KT);
 #pragma unroll
       for (int c = 0; c < C::CH; ++c) {
-        tma_load_2d(sK + c * 16384, &tmKV, kv_full, d_model + h * DH + c * 64, b * S + jt * 128);
-        tma_load_2d(sV + c * 16384, &tmKV, kv_full, 2 * d_model + h * DH + c * 64, b * S + jt * 128);
+        tma_load_2d(sK + c * 16384, &tmKV, kv_full, k_col + c * 64, b * S + jt * 128);
+        tma_load_2d(sV + c * 16384, &tmKV, kv_full, v_col + c * 64, b * S + jt * 128);
       }
-      for (int i = i0; i < n_q; ++i) {
-        const int n = i - i0, st = n & 1;
-        mbar_wait(&q_empty[st], ((n >> 1) & 1) ^ 1);
-        mbar_expect_tx(&q_full[st], 2 * C::QT);
+      for (int h = h0; h < h0 + G; ++h) {
+        for (int i = i0; i < n_q; ++i) {
+          const int n = (h - h0) * (n_q - i0) + i - i0, st = n & 1;   // (query head, query tile) items in walk order
+          mbar_wait(&q_empty[st], ((n >> 1) & 1) ^ 1);
+          mbar_expect_tx(&q_full[st], 2 * C::QT);
 #pragma unroll
-        for (int c = 0; c < C::CH; ++c) {
-          tma_load_2d(sQ + st * C::QT + c * 8192, &tmQ, &q_full[st], h * DH + c * 64, b * S + i * 64);
-          tma_load_2d(sDO + st * C::QT + c * 8192, &tmDO, &q_full[st], h * DH + c * 64, b * S + i * 64);
+          for (int c = 0; c < C::CH; ++c) {
+            tma_load_2d(sQ + st * C::QT + c * 8192, &tmQ, &q_full[st], h * DH + c * 64, b * S + i * 64);
+            tma_load_2d(sDO + st * C::QT + c * 8192, &tmDO, &q_full[st], h * DH + c * 64, b * S + i * 64);
+          }
         }
       }
     }
@@ -366,119 +380,131 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
   const int kl0 = cw * 64 + wq * 16 + g;          // this thread's key rows inside the tile: kl0, kl0 + 8
   const int key0 = jt * 128 + kl0;
   const float sc = scale * LOG2E;
-  const float slope2 = ALIBI ? alibi_slopes[h] * LOG2E : 0.f;
-  const float* lse_bh = lse + (long long)bh * S;
-  const float* delta_bh = delta + (long long)bh * S;
+  // the multi-head instances read their head's row statistics here, where the multi-head kernel always has
+  const float slope2_mh = ALIBI && !GQA ? alibi_slopes[h0] * LOG2E : 0.f;
+  const float* lse_mh = lse + (long long)bk * S;
+  const float* delta_mh = delta + (long long)bk * S;
   const int* dstart_b = DOC ? doc_start + (long long)b * S : nullptr;
   float dv[DH / 2], dk[DH / 2];
 #pragma unroll
   for (int i = 0; i < DH / 2; ++i) dv[i] = 0.f, dk[i] = 0.f;
   mbar_wait(kv_full, 0);
-  for (int i = i0; i < n_q; ++i) {
-    const int n = i - i0, st = n & 1;
-    const int q0 = i * 64;
-    uint8_t* q_st = sQ + st * C::QT;
-    uint8_t* do_st = sDO + st * C::QT;
-    float s[32], dp[32];
-    mbar_wait(&q_full[st], (n >> 1) & 1);
-    wgmma_fence();
+  // the query tiles of query head h; n0: the walk position of its first tile (the group's heads come one after the other)
+  auto walk = [&](const int h, const int n0) {
+    const float slope2 = !GQA ? slope2_mh : ALIBI ? alibi_slopes[h] * LOG2E : 0.f;
+    const float* lse_bh = GQA ? lse + ((long long)b * H + h) * S : lse_mh;
+    const float* delta_bh = GQA ? delta + ((long long)b * H + h) * S : delta_mh;
+    for (int i = i0; i < n_q; ++i) {
+      const int n = n0 + i - i0, st = n & 1;
+      const int q0 = i * 64;
+      uint8_t* q_st = sQ + st * C::QT;
+      uint8_t* do_st = sDO + st * C::QT;
+      float s[32], dp[32];
+      mbar_wait(&q_full[st], (n >> 1) & 1);
+      wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < DH / 16; ++kk) {   // S^T = K Q^T
-      const int c = kk >> 2, off = (kk & 3) * 32;
-      wgmma_bf16_ss_n64<0, 0>(s, desc_add(desc_sw128(sK + c * 16384 + cw * 8192, 16), off), desc_add(desc_sw128(q_st + c * 8192, 16), off),
-                              kk > 0 ? 1u : 0u);
-    }
-#pragma unroll
-    for (int kk = 0; kk < DH / 16; ++kk) {   // dP^T = V dO^T
-      const int c = kk >> 2, off = (kk & 3) * 32;
-      wgmma_bf16_ss_n64<0, 0>(dp, desc_add(desc_sw128(sV + c * 16384 + cw * 8192, 16), off), desc_add(desc_sw128(do_st + c * 8192, 16), off),
-                              kk > 0 ? 1u : 0u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(s);
-    wgmma_fence_regs(dp);
-    // P^T = exp(S^T * scale + alibi - lse[q]) (masked where query < key), dS^T = P^T * (dP^T - delta[q])
-    uint32_t pa[4][4], da[4][4];
-#pragma unroll
-    for (int j8 = 0; j8 < 8; ++j8) {
-      const int qa = q0 + 8 * j8 + 2 * t4;
-      const float2 L = *reinterpret_cast<const float2*>(lse_bh + qa);
-      const float2 D = *reinterpret_cast<const float2*>(delta_bh + qa);
-      int2 DS = make_int2(0, 0);
-      if (DOC) DS = *reinterpret_cast<const int2*>(dstart_b + qa);   // through L1, like lse / delta
-      float pv[4], dsv[4];
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int q = qa + (e & 1), key = key0 + 8 * (e >> 1);
-        float x = fmaf(s[4 * j8 + e], sc, -((e & 1) ? L.y : L.x) * LOG2E);
-        if (ALIBI) x = fmaf(slope2, float(key - q), x);
-        float pr = exp2f(x);
-        if (causal && q < key) pr = 0.f;
-        if (DOC && ((e & 1) ? DS.y : DS.x) > key) pr = 0.f;
-        pv[e] = pr;
-        dsv[e] = pr * (dp[4 * j8 + e] - ((e & 1) ? D.y : D.x));
-        // a masked query of another document may carry a non-finite delta (its own keys' fault): keep it out of dK
-        if (DOC && pr == 0.f) dsv[e] = 0.f;
+      for (int kk = 0; kk < DH / 16; ++kk) {   // S^T = K Q^T
+        const int c = kk >> 2, off = (kk & 3) * 32;
+        wgmma_bf16_ss_n64<0, 0>(s, desc_add(desc_sw128(sK + c * 16384 + cw * 8192, 16), off), desc_add(desc_sw128(q_st + c * 8192, 16), off),
+                                kk > 0 ? 1u : 0u);
       }
-      // accumulator columns 16 kc .. 16 kc + 15 (queries) are the A fragment of k-step kc
-      const int kc = j8 >> 1, hi = (j8 & 1) * 2;
-      pa[kc][hi] = pack_bf16(pv[0], pv[1]);
-      pa[kc][hi + 1] = pack_bf16(pv[2], pv[3]);
-      da[kc][hi] = pack_bf16(dsv[0], dsv[1]);
-      da[kc][hi + 1] = pack_bf16(dsv[2], dsv[3]);
-    }
-    wgmma_fence();
 #pragma unroll
-    for (int kc = 0; kc < 4; ++kc) {   // dV += P^T dO, dK += dS^T Q (B operands MN-major: 16 query rows per k-step)
-      wgmma_acc_rs<DH>(dv, pa[kc], desc_add(desc_sw128(do_st, 8192), kc * 2048));
-      wgmma_acc_rs<DH>(dk, da[kc], desc_add(desc_sw128(q_st, 8192), kc * 2048));
-    }
-    wgmma_commit();
-    // dS^T -> shared memory (row = key, 64 queries = 128 bytes, 128-byte swizzle); both warpgroups' previous dQ MMAs are done
-    named_bar_sync(1, 256);
+      for (int kk = 0; kk < DH / 16; ++kk) {   // dP^T = V dO^T
+        const int c = kk >> 2, off = (kk & 3) * 32;
+        wgmma_bf16_ss_n64<0, 0>(dp, desc_add(desc_sw128(sV + c * 16384 + cw * 8192, 16), off), desc_add(desc_sw128(do_st + c * 8192, 16), off),
+                                kk > 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(s);
+      wgmma_fence_regs(dp);
+      // P^T = exp(S^T * scale + alibi - lse[q]) (masked where query < key), dS^T = P^T * (dP^T - delta[q])
+      uint32_t pa[4][4], da[4][4];
 #pragma unroll
-    for (int j8 = 0; j8 < 8; ++j8) {
-      const int kc = j8 >> 1, hi = (j8 & 1) * 2;
+      for (int j8 = 0; j8 < 8; ++j8) {
+        const int qa = q0 + 8 * j8 + 2 * t4;
+        const float2 L = *reinterpret_cast<const float2*>(lse_bh + qa);
+        const float2 D = *reinterpret_cast<const float2*>(delta_bh + qa);
+        int2 DS = make_int2(0, 0);
+        if (DOC) DS = *reinterpret_cast<const int2*>(dstart_b + qa);   // through L1, like lse / delta
+        float pv[4], dsv[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int q = qa + (e & 1), key = key0 + 8 * (e >> 1);
+          float x = fmaf(s[4 * j8 + e], sc, -((e & 1) ? L.y : L.x) * LOG2E);
+          if (ALIBI) x = fmaf(slope2, float(key - q), x);
+          float pr = exp2f(x);
+          if (causal && q < key) pr = 0.f;
+          if (DOC && ((e & 1) ? DS.y : DS.x) > key) pr = 0.f;
+          pv[e] = pr;
+          dsv[e] = pr * (dp[4 * j8 + e] - ((e & 1) ? D.y : D.x));
+          // a masked query of another document may carry a non-finite delta (its own keys' fault): keep it out of dK
+          if (DOC && pr == 0.f) dsv[e] = 0.f;
+        }
+        // accumulator columns 16 kc .. 16 kc + 15 (queries) are the A fragment of k-step kc
+        const int kc = j8 >> 1, hi = (j8 & 1) * 2;
+        pa[kc][hi] = pack_bf16(pv[0], pv[1]);
+        pa[kc][hi + 1] = pack_bf16(pv[2], pv[3]);
+        da[kc][hi] = pack_bf16(dsv[0], dsv[1]);
+        da[kc][hi + 1] = pack_bf16(dsv[2], dsv[3]);
+      }
+      wgmma_fence();
+#pragma unroll
+      for (int kc = 0; kc < 4; ++kc) {   // dV += P^T dO, dK += dS^T Q (B operands MN-major: 16 query rows per k-step)
+        wgmma_acc_rs<DH>(dv, pa[kc], desc_add(desc_sw128(do_st, 8192), kc * 2048));
+        wgmma_acc_rs<DH>(dk, da[kc], desc_add(desc_sw128(q_st, 8192), kc * 2048));
+      }
+      wgmma_commit();
+      // dS^T -> shared memory (row = key, 64 queries = 128 bytes, 128-byte swizzle); both warpgroups' previous dQ MMAs are done
+      named_bar_sync(1, 256);
+#pragma unroll
+      for (int j8 = 0; j8 < 8; ++j8) {
+        const int kc = j8 >> 1, hi = (j8 & 1) * 2;
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int kl = kl0 + 8 * hh;
+          *reinterpret_cast<uint32_t*>(sDS + kl * 128 + ((j8 ^ (kl & 7)) << 4) + 4 * t4) = da[kc][hi + hh];
+        }
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(1, 256);
+      // dQ[64 queries, this warpgroup's half of the head] = dS K: A = dS (MN-major: queries contiguous), B = K (MN-major)
+      float dq[DH / 4];
+      wgmma_fence();
+#pragma unroll
+      for (int kc = 0; kc < 8; ++kc) {
+        const uint64_t ad = desc_add(desc_sw128(sDS, 16384), kc * 2048);
+        if constexpr (DH == 128) {
+          wgmma_bf16_ss_n64<1, 1>(dq, ad, desc_add(desc_sw128(sK + cw * 16384, 16384), kc * 2048), kc > 0 ? 1u : 0u);
+        } else {
+          wgmma_bf16_ss_n32<1, 1>(dq, ad, desc_add(desc_sw128(sK + cw * 64, 16384), kc * 2048), kc > 0 ? 1u : 0u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(dq);
+      wgmma_fence_regs(dv);
+      wgmma_fence_regs(dk);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&q_empty[st]);
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
-        const int kl = kl0 + 8 * hh;
-        *reinterpret_cast<uint32_t*>(sDS + kl * 128 + ((j8 ^ (kl & 7)) << 4) + 4 * t4) = da[kc][hi + hh];
+        float* dst = dq_acc + (long long)(b * S + q0 + wq * 16 + g + 8 * hh) * d_model + h * DH + cw * (DH / 2) + 2 * t4;
+#pragma unroll
+        for (int j = 0; j < DH / 16; ++j) red_add_f32x2(dst + 8 * j, dq[4 * j + 2 * hh], dq[4 * j + 2 * hh + 1]);
       }
     }
-    fence_proxy_async_smem();
-    named_bar_sync(1, 256);
-    // dQ[64 queries, this warpgroup's half of the head] = dS K: A = dS (MN-major: queries contiguous), B = K (MN-major)
-    float dq[DH / 4];
-    wgmma_fence();
-#pragma unroll
-    for (int kc = 0; kc < 8; ++kc) {
-      const uint64_t ad = desc_add(desc_sw128(sDS, 16384), kc * 2048);
-      if constexpr (DH == 128) {
-        wgmma_bf16_ss_n64<1, 1>(dq, ad, desc_add(desc_sw128(sK + cw * 16384, 16384), kc * 2048), kc > 0 ? 1u : 0u);
-      } else {
-        wgmma_bf16_ss_n32<1, 1>(dq, ad, desc_add(desc_sw128(sK + cw * 64, 16384), kc * 2048), kc > 0 ? 1u : 0u);
-      }
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(dq);
-    wgmma_fence_regs(dv);
-    wgmma_fence_regs(dk);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&q_empty[st]);
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      float* dst = dq_acc + (long long)(b * S + q0 + wq * 16 + g + 8 * hh) * d_model + h * DH + cw * (DH / 2) + 2 * t4;
-#pragma unroll
-      for (int j = 0; j < DH / 16; ++j) red_add_f32x2(dst + 8 * j, dq[4 * j + 2 * hh], dq[4 * j + 2 * hh + 1]);
-    }
+  };
+  if constexpr (GQA) {
+    for (int h = h0; h < h0 + G; ++h) walk(h, (h - h0) * (n_q - i0));
+  } else {
+    walk(h0, 0);
   }
-  // dK (x scale), dV -> bf16 -> dqkv
+  // dK (x scale), dV of the kv head (summed over its query heads) -> bf16 -> dqkv
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
-    __nv_bfloat16* krow = dqkv + (long long)(b * S + key0 + 8 * hh) * (3 * d_model) + d_model + h * DH;
-    __nv_bfloat16* vrow = krow + d_model;
+    __nv_bfloat16* krow = dqkv + (long long)(b * S + key0 + 8 * hh) * (GQA ? d_model + 2 * HKV * DH : 3 * d_model) + k_col;
+    __nv_bfloat16* vrow = krow + (GQA ? HKV * DH : d_model);
 #pragma unroll
     for (int j = 0; j < DH / 8; ++j) {
       *reinterpret_cast<uint32_t*>(krow + 8 * j + 2 * t4) = pack_bf16(dk[4 * j + 2 * hh] * scale, dk[4 * j + 2 * hh + 1] * scale);
@@ -542,21 +568,28 @@ void set_smem(K kern, int bytes) {
 
 }  // namespace
 
-void attention_fwd_launch(const void* qkv, void* out, float* lse, int B, int S, int H, int dh, float scale, bool causal, int num_sms,
-                          cudaStream_t st, const float* alibi_slopes, const int* doc_start) {
+void attention_fwd_launch(const void* qkv, void* out, float* lse, int B, int S, int H, int Hkv, int dh, float scale, bool causal,
+                          int num_sms, cudaStream_t st, const float* alibi_slopes, const int* doc_start) {
   (void)num_sms;
   if (S % 128) throw std::runtime_error("photon_b200 attention: sequence length must be a multiple of 128");
   if (dh != 64 && dh != 128) throw std::runtime_error("photon_b200 attention: d_head must be 64 or 128");
   if (doc_start && !causal) throw std::runtime_error("photon_b200 attention: the document mask needs the causal mask");
-  const int d = H * dh;
-  CUtensorMap tm = make_tmap_2d(qkv, 2, false, uint64_t(3) * d, uint64_t(B) * S, uint64_t(3) * d * 2, 64, 128);
+  if (Hkv < 1 || H % Hkv) throw std::runtime_error("photon_b200 attention: the kv head count must divide the head count");
+  const uint64_t w = uint64_t(H + 2 * Hkv) * dh;   // fused qkv row width
+  CUtensorMap tm = make_tmap_2d(qkv, 2, false, w, uint64_t(B) * S, w * 2, 64, 128);
   const dim3 grid(S / 128, B * H);
+#define PB_FWD_G(DHV, AL, DOC, GQA)                                                                                  \
+  {                                                                                                                  \
+    static bool once = (set_smem(attn_fwd_kernel<DHV, AL, DOC, GQA>, FwdCfg<DHV>::SMEM), true);                      \
+    (void)once;                                                                                                      \
+    attn_fwd_kernel<DHV, AL, DOC, GQA><<<grid, 384, FwdCfg<DHV>::SMEM, st>>>(tm, (__nv_bfloat16*)out, lse, S, H, scale, \
+                                                                            causal ? 1 : 0, alibi_slopes, doc_start, \
+                                                                            Hkv);                                    \
+  }
 #define PB_FWD(DHV, AL, DOC)                                                                                         \
   {                                                                                                                  \
-    static bool once = (set_smem(attn_fwd_kernel<DHV, AL, DOC>, FwdCfg<DHV>::SMEM), true);                           \
-    (void)once;                                                                                                      \
-    attn_fwd_kernel<DHV, AL, DOC><<<grid, 384, FwdCfg<DHV>::SMEM, st>>>(tm, (__nv_bfloat16*)out, lse, S, H, scale,   \
-                                                                       causal ? 1 : 0, alibi_slopes, doc_start);    \
+    if (Hkv == H) PB_FWD_G(DHV, AL, DOC, false)                                                                      \
+    else PB_FWD_G(DHV, AL, DOC, true)                                                                                \
   }
   if (!doc_start) {
     if (dh == 64 && !alibi_slopes) PB_FWD(64, false, false)
@@ -570,19 +603,22 @@ void attention_fwd_launch(const void* qkv, void* out, float* lse, int B, int S, 
     else PB_FWD(128, true, true)
   }
 #undef PB_FWD
+#undef PB_FWD_G
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) throw std::runtime_error(std::string("attention fwd launch: ") + cudaGetErrorString(e));
 }
 
 int attention_bwd_launch(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta, float* dq_acc,
-                         int B, int S, int H, int dh, float scale, bool causal, int num_sms, cudaStream_t st, const float* alibi_slopes,
+                         int B, int S, int H, int Hkv, int dh, float scale, bool causal, int num_sms, cudaStream_t st, const float* alibi_slopes,
                          const int* doc_start, const int* doc_end) {
   if (S % 128) throw std::runtime_error("photon_b200 attention: sequence length must be a multiple of 128");
   if (dh != 64 && dh != 128) throw std::runtime_error("photon_b200 attention backward: d_head must be 64 or 128");
   if (bool(doc_start) != bool(doc_end)) throw std::runtime_error("photon_b200 attention backward: doc_start and doc_end go together");
   if (doc_start && !causal) throw std::runtime_error("photon_b200 attention: the document mask needs the causal mask");
+  if (Hkv < 1 || H % Hkv) throw std::runtime_error("photon_b200 attention: the kv head count must divide the head count");
   const int sms = num_sms > 0 ? num_sms : 132;
   const int d = H * dh;
+  const uint64_t w = uint64_t(H + 2 * Hkv) * dh;   // fused qkv row width
   const long long rows = (long long)B * S;
   cudaMemsetAsync(dq_acc, 0, size_t(rows) * d * sizeof(float), st);
   {
@@ -590,17 +626,22 @@ int attention_bwd_launch(const void* qkv, const void* out, const void* dout, con
     const int blocks = int(std::min<long long>((n8 + 255) / 256, sms * 16));
     attn_bwd_delta_kernel<<<blocks, 256, 0, st>>>((const __nv_bfloat16*)out, (const __nv_bfloat16*)dout, delta, S, H, dh, rows);
   }
-  CUtensorMap tmKV = make_tmap_2d(qkv, 2, false, uint64_t(3) * d, uint64_t(rows), uint64_t(3) * d * 2, 64, 128);
-  CUtensorMap tmQ = make_tmap_2d(qkv, 2, false, uint64_t(3) * d, uint64_t(rows), uint64_t(3) * d * 2, 64, 64);
+  CUtensorMap tmKV = make_tmap_2d(qkv, 2, false, w, uint64_t(rows), w * 2, 64, 128);
+  CUtensorMap tmQ = make_tmap_2d(qkv, 2, false, w, uint64_t(rows), w * 2, 64, 64);
   CUtensorMap tmDO = make_tmap_2d(dout, 2, false, uint64_t(d), uint64_t(rows), uint64_t(d) * 2, 64, 64);
-  const dim3 grid(S / 128, B * H);
+  const dim3 grid(S / 128, B * Hkv);
+#define PB_BWD_G(DHV, AL, DOC, GQA)                                                                                  \
+  {                                                                                                                  \
+    static bool once = (set_smem(attn_bwd_kernel<DHV, AL, DOC, GQA>, BwdCfg<DHV>::SMEM), true);                      \
+    (void)once;                                                                                                      \
+    attn_bwd_kernel<DHV, AL, DOC, GQA><<<grid, 384, BwdCfg<DHV>::SMEM, st>>>(tmKV, tmQ, tmDO, lse, delta, (__nv_bfloat16*)dqkv, \
+                                                                            S, H, scale, causal ? 1 : 0, dq_acc,        \
+                                                                            alibi_slopes, doc_start, doc_end, Hkv);     \
+  }
 #define PB_BWD(DHV, AL, DOC)                                                                                         \
   {                                                                                                                  \
-    static bool once = (set_smem(attn_bwd_kernel<DHV, AL, DOC>, BwdCfg<DHV>::SMEM), true);                           \
-    (void)once;                                                                                                      \
-    attn_bwd_kernel<DHV, AL, DOC><<<grid, 384, BwdCfg<DHV>::SMEM, st>>>(tmKV, tmQ, tmDO, lse, delta, (__nv_bfloat16*)dqkv, S, H, \
-                                                                       scale, causal ? 1 : 0, dq_acc, alibi_slopes,  \
-                                                                       doc_start, doc_end);                          \
+    if (Hkv == H) PB_BWD_G(DHV, AL, DOC, false)                                                                      \
+    else PB_BWD_G(DHV, AL, DOC, true)                                                                                \
   }
   if (!doc_start) {
     if (dh == 64 && !alibi_slopes) PB_BWD(64, false, false)
@@ -614,7 +655,8 @@ int attention_bwd_launch(const void* qkv, const void* out, const void* dout, con
     else PB_BWD(128, true, true)
   }
 #undef PB_BWD
-  attn_bwd_dq_convert_kernel<<<sms * 8, 256, 0, st>>>(dq_acc, (__nv_bfloat16*)dqkv, rows, d, scale);
+#undef PB_BWD_G
+  attn_bwd_dq_convert_kernel<<<sms * 8, 256, 0, st>>>(dq_acc, (__nv_bfloat16*)dqkv, rows, d, int(w), scale);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) throw std::runtime_error(std::string("attention bwd launch: ") + cudaGetErrorString(e));
   return 3;
@@ -627,22 +669,22 @@ void doc_bounds_launch(const long long* sequence_id, int* doc_start, int* doc_en
 }
 
 // ---------------------------------------------------------------------------------------------- RoPE
-// In-place rotary embedding (rotate-half / GPT-NeoX convention) on the q and k thirds of a fused qkv buffer
-// [T, 3*H*dh] bf16; cos / sin: fp32 [S, dh/2]. inverse = 1 applies the transposed rotation (gradients of q, k).
+// In-place rotary embedding (rotate-half / GPT-NeoX convention) on the H q heads and the Hkv k heads of a fused qkv buffer
+// [T, (H + 2*Hkv)*dh] bf16 (the k heads follow the q heads, so together they are H + Hkv consecutive heads of each row);
+// cos / sin: fp32 [S, dh/2]. inverse = 1 applies the transposed rotation (gradients of q, k).
 namespace {
 __global__ void __launch_bounds__(256) rope_kernel(__nv_bfloat16* __restrict__ qkv, const float* __restrict__ cosT, const float* __restrict__ sinT,
-                                                   long long T, int S, int H, int dh, int inverse) {
+                                                   long long T, int S, int H, int Hkv, int dh, int inverse) {
   const int half = dh / 2, groups = half / 8;                 // 8 pairs (16 bytes of each half) per thread
-  const long long n = T * 2 * H * groups;                     // (token, q|k, head, group)
+  const int nh = H + Hkv;                                     // rotated heads per row: q heads, then k heads
+  const long long n = T * nh * groups;                        // (token, head, group)
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const int g = int(i % groups);
-    long long r = i / groups;
-    const int h = int(r % H);
-    r /= H;
-    const int which = int(r % 2);
-    const long long t = r / 2;
+    const long long r = i / groups;
+    const int h = int(r % nh);
+    const long long t = r / nh;
     const int pos = int(t % S);
-    __nv_bfloat16* base = qkv + t * (3LL * H * dh) + (long long)which * H * dh + h * dh + g * 8;
+    __nv_bfloat16* base = qkv + t * ((long long)(H + 2 * Hkv) * dh) + (long long)h * dh + g * 8;
     const uint4 a = *reinterpret_cast<const uint4*>(base);
     const uint4 b = *reinterpret_cast<const uint4*>(base + half);
     const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w};
@@ -663,11 +705,13 @@ __global__ void __launch_bounds__(256) rope_kernel(__nv_bfloat16* __restrict__ q
 }
 }  // namespace
 
-void rope_launch(void* qkv, const float* cosT, const float* sinT, long long T, int S, int H, int dh, bool inverse, cudaStream_t st) {
+void rope_launch(void* qkv, const float* cosT, const float* sinT, long long T, int S, int H, int Hkv, int dh, bool inverse,
+                 cudaStream_t st) {
   if (dh % 16) throw std::runtime_error("photon_b200 rope: d_head must be a multiple of 16");
-  const long long n = T * 2 * H * (dh / 16);
+  if (Hkv < 1 || H % Hkv) throw std::runtime_error("photon_b200 rope: the kv head count must divide the head count");
+  const long long n = T * (H + Hkv) * (dh / 16);
   const int blocks = int(std::min<long long>((n + 255) / 256, 132 * 16));
-  rope_kernel<<<blocks, 256, 0, st>>>((__nv_bfloat16*)qkv, cosT, sinT, T, S, H, dh, inverse ? 1 : 0);
+  rope_kernel<<<blocks, 256, 0, st>>>((__nv_bfloat16*)qkv, cosT, sinT, T, S, H, Hkv, dh, inverse ? 1 : 0);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) throw std::runtime_error(std::string("rope launch: ") + cudaGetErrorString(e));
 }

@@ -297,12 +297,20 @@ void fp8_update_scales(Tensor& meta, Tensor& hist, const Tensor& fmax, Tensor& p
 }
 
 // ---------------------------------------------------------------------------------- attention
-// shapes shared by the forward and the backward: qkv [B,S,3d]; o-like tensors [B,S,d]; row statistics fp32 [B,H,S]
-void check_attention_args(const Tensor& qkv, const Tensor& out, const Tensor& lse, int n_heads, bool causal,
+// head counts of a fused qkv row of `width` elements: H q heads, then Hkv k heads and Hkv v heads of d_head each; returns d_head
+int64_t check_qkv_heads(int64_t width, int n_heads, int n_kv_heads, const char* what) {
+  TORCH_CHECK(n_heads > 0 && n_kv_heads > 0 && n_heads % n_kv_heads == 0, what, ": n_kv_heads = ", n_kv_heads,
+              " must be positive and divide n_heads = ", n_heads);
+  const int64_t units = int64_t(n_heads) + 2 * int64_t(n_kv_heads);
+  TORCH_CHECK(width % units == 0, what, ": a qkv row of ", width, " elements is not (n_heads + 2 * n_kv_heads) = ", units,
+              " heads of equal size");
+  return width / units;
+}
+// shapes shared by the forward and the backward: qkv [B,S,(H+2*Hkv)*dh]; o-like tensors [B,S,H*dh]; row statistics fp32 [B,H,S]
+void check_attention_args(const Tensor& qkv, const Tensor& out, const Tensor& lse, int n_heads, int n_kv_heads, bool causal,
                           const c10::optional<Tensor>& alibi_slopes) {
-  TORCH_CHECK(qkv.dim() == 3 && qkv.is_contiguous() && qkv.size(2) % 3 == 0, "qkv must be contiguous [B,S,3*d]");
-  const int64_t B = qkv.size(0), S = qkv.size(1), d = qkv.size(2) / 3;
-  TORCH_CHECK(n_heads > 0 && d % n_heads == 0, "attention: d = ", d, " is not a multiple of n_heads = ", n_heads);
+  TORCH_CHECK(qkv.dim() == 3 && qkv.is_contiguous(), "qkv must be contiguous [B,S,(n_heads+2*n_kv_heads)*d_head]");
+  const int64_t B = qkv.size(0), S = qkv.size(1), d = check_qkv_heads(qkv.size(2), n_heads, n_kv_heads, "attention") * n_heads;
   TORCH_CHECK(out.is_contiguous() && out.sizes() == at::IntArrayRef({B, S, d}), "out must be contiguous [B,S,d]");
   TORCH_CHECK(lse.is_contiguous() && lse.sizes() == at::IntArrayRef({B, int64_t(n_heads), S}), "lse must be contiguous float32 [B,H,S]");
   if (alibi_slopes.has_value()) {
@@ -326,15 +334,16 @@ void check_doc_args(const Tensor& qkv, bool causal, const c10::optional<Tensor>&
   check_doc_bound(doc_end, "doc_end", qkv);
 }
 void attention_fwd(const Tensor& qkv, Tensor& out, Tensor& lse, int n_heads, double scale, bool causal,
-                   const c10::optional<Tensor>& alibi_slopes, const c10::optional<Tensor>& doc_start) {
+                   const c10::optional<Tensor>& alibi_slopes, const c10::optional<Tensor>& doc_start, int n_kv_heads) {
   check_bf16(qkv, "qkv");
   check_bf16(out, "out");
   check_f32(lse, "lse");
-  check_attention_args(qkv, out, lse, n_heads, causal, alibi_slopes);
+  n_kv_heads = n_kv_heads == -1 ? n_heads : n_kv_heads;   // -1: multi-head attention
+  check_attention_args(qkv, out, lse, n_heads, n_kv_heads, causal, alibi_slopes);
   check_doc_args(qkv, causal, doc_start, c10::nullopt);
   c10::cuda::CUDAGuard guard(qkv.device());
-  const int B = int(qkv.size(0)), S = int(qkv.size(1)), d = int(qkv.size(2) / 3);
-  pb::attention_fwd_launch(qkv.data_ptr(), out.data_ptr(), lse.data_ptr<float>(), B, S, n_heads, d / n_heads, float(scale), causal,
+  const int B = int(qkv.size(0)), S = int(qkv.size(1)), dh = int(qkv.size(2) / (n_heads + 2 * n_kv_heads));
+  pb::attention_fwd_launch(qkv.data_ptr(), out.data_ptr(), lse.data_ptr<float>(), B, S, n_heads, n_kv_heads, dh, float(scale), causal,
                            at::cuda::getCurrentDeviceProperties()->multiProcessorCount, stream_of(qkv),
                            alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr,
                            doc_start.has_value() ? doc_start->data_ptr<int>() : nullptr);
@@ -342,26 +351,27 @@ void attention_fwd(const Tensor& qkv, Tensor& out, Tensor& lse, int n_heads, dou
 }
 void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, const Tensor& lse, Tensor& dqkv, Tensor& delta,
                    int n_heads, double scale, bool causal, const c10::optional<Tensor>& alibi_slopes,
-                   const c10::optional<Tensor>& doc_start, const c10::optional<Tensor>& doc_end) {
+                   const c10::optional<Tensor>& doc_start, const c10::optional<Tensor>& doc_end, int n_kv_heads) {
   check_bf16(qkv, "qkv");
   check_bf16(out, "out");
   check_bf16(dout, "dout");
   check_bf16(dqkv, "dqkv");
   check_f32(lse, "lse");
   check_f32(delta, "delta");
-  check_attention_args(qkv, out, lse, n_heads, causal, alibi_slopes);
+  n_kv_heads = n_kv_heads == -1 ? n_heads : n_kv_heads;   // -1: multi-head attention
+  check_attention_args(qkv, out, lse, n_heads, n_kv_heads, causal, alibi_slopes);
   check_doc_args(qkv, causal, doc_start, doc_end);
   TORCH_CHECK(doc_start.has_value() == doc_end.has_value(), "attention_bwd: doc_start needs doc_end");
   TORCH_CHECK(dout.is_contiguous() && dout.sizes() == out.sizes(), "dout must be contiguous [B,S,d]");
   TORCH_CHECK(delta.is_contiguous() && delta.sizes() == lse.sizes(), "delta must be contiguous float32 [B,H,S]");
   TORCH_CHECK(dqkv.is_contiguous() && dqkv.sizes() == qkv.sizes(), "dqkv must be contiguous and shaped like qkv");
   c10::cuda::CUDAGuard guard(qkv.device());
-  const int B = int(qkv.size(0)), S = int(qkv.size(1)), d = int(qkv.size(2) / 3);
+  const int B = int(qkv.size(0)), S = int(qkv.size(1)), dh = int(qkv.size(2) / (n_heads + 2 * n_kv_heads)), d = n_heads * dh;
   // the fp32 dQ accumulator comes from the caching allocator on this stream: eagerly it is recycled in stream order, under
   // CUDA-graph capture it comes from the graph's private pool and lives as long as the graph
   Tensor dq_acc = at::empty({(int64_t)B * S, d}, qkv.options().dtype(at::kFloat));
   const int launched = pb::attention_bwd_launch(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr<float>(), dqkv.data_ptr(),
-                                                delta.data_ptr<float>(), dq_acc.data_ptr<float>(), B, S, n_heads, d / n_heads, float(scale), causal,
+                                                delta.data_ptr<float>(), dq_acc.data_ptr<float>(), B, S, n_heads, n_kv_heads, dh, float(scale), causal,
                                                 at::cuda::getCurrentDeviceProperties()->multiProcessorCount, stream_of(qkv),
                                                 alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr,
                                                 doc_start.has_value() ? doc_start->data_ptr<int>() : nullptr,
@@ -385,15 +395,17 @@ void doc_bounds(const Tensor& sequence_id, Tensor& doc_start, Tensor& doc_end) {
                         doc_end.data_ptr<int>(), int(B), int(S), stream_of(sequence_id));
   g_launches += 1;
 }
-void rope(Tensor& qkv, const Tensor& cos_t, const Tensor& sin_t, int n_heads, bool inverse) {
+void rope(Tensor& qkv, const Tensor& cos_t, const Tensor& sin_t, int n_heads, bool inverse, int n_kv_heads) {
   check_bf16(qkv, "qkv");
   check_f32(cos_t, "cos");
   check_f32(sin_t, "sin");
-  TORCH_CHECK(qkv.dim() == 3 && qkv.is_contiguous(), "qkv must be contiguous [B,S,3*d]");
+  TORCH_CHECK(qkv.dim() == 3 && qkv.is_contiguous(), "qkv must be contiguous [B,S,(n_heads+2*n_kv_heads)*d_head]");
+  n_kv_heads = n_kv_heads == -1 ? n_heads : n_kv_heads;   // -1: multi-head attention
+  const int dh = int(check_qkv_heads(qkv.size(2), n_heads, n_kv_heads, "rope"));
   c10::cuda::CUDAGuard guard(qkv.device());
-  const int S = int(qkv.size(1)), d = int(qkv.size(2) / 3), dh = d / n_heads;
+  const int S = int(qkv.size(1));
   TORCH_CHECK(cos_t.is_contiguous() && sin_t.is_contiguous() && cos_t.size(0) >= S && cos_t.size(1) == dh / 2, "cos/sin must be [>=S, dh/2]");
-  pb::rope_launch(qkv.data_ptr(), cos_t.data_ptr<float>(), sin_t.data_ptr<float>(), (long long)qkv.size(0) * S, S, n_heads, dh, inverse,
+  pb::rope_launch(qkv.data_ptr(), cos_t.data_ptr<float>(), sin_t.data_ptr<float>(), (long long)qkv.size(0) * S, S, n_heads, n_kv_heads, dh, inverse,
                   stream_of(qkv));
   g_launches += 1;
 }
@@ -447,17 +459,19 @@ void skinny_gemm(const Tensor& x, const Tensor& w, Tensor& y, const c10::optiona
   pb::skinny_gemm_launch(a, splits > 1 ? part.data_ptr<float>() : nullptr, stream_of(x));
   g_launches += splits > 1 ? 2 : 1;
 }
-// kc / vc: one layer of the cache, [B_max, H, S_max, dh]; q: rows of [B, >= H*dh] (the q third of the fused qkv)
+// kc / vc: one layer of the cache, [B_max, Hkv, S_max, dh]; q: rows of [B, >= H*dh] (the q heads of the fused qkv)
 void decode_attention(const Tensor& q, const Tensor& kc, const Tensor& vc, const Tensor& pos, Tensor& out, int n_heads, double scale,
-                      const c10::optional<Tensor>& alibi_slopes) {
+                      const c10::optional<Tensor>& alibi_slopes, int n_kv_heads) {
   check_bf16(q, "q");
   check_bf16(kc, "k_cache");
   check_bf16(vc, "v_cache");
   check_bf16(out, "out");
   check_i32(pos, "pos");
-  TORCH_CHECK(kc.dim() == 4 && kc.is_contiguous() && vc.sizes() == kc.sizes() && vc.is_contiguous(), "k/v cache must be contiguous [B_max, H, S_max, dh]");
-  const int B = int(q.size(0)), H = int(kc.size(1)), S = int(kc.size(2)), dh = int(kc.size(3));
-  TORCH_CHECK(H == n_heads && (dh == 64 || dh == 128), "decode_attention: cache heads must equal n_heads and d_head be 64 or 128");
+  TORCH_CHECK(kc.dim() == 4 && kc.is_contiguous() && vc.sizes() == kc.sizes() && vc.is_contiguous(), "k/v cache must be contiguous [B_max, Hkv, S_max, dh]");
+  n_kv_heads = n_kv_heads == -1 ? n_heads : n_kv_heads;   // -1: multi-head attention
+  const int B = int(q.size(0)), Hkv = int(kc.size(1)), H = n_heads, S = int(kc.size(2)), dh = int(kc.size(3));
+  TORCH_CHECK(n_heads > 0 && n_kv_heads > 0 && Hkv == n_kv_heads && n_heads % n_kv_heads == 0 && (dh == 64 || dh == 128),
+              "decode_attention: cache heads must equal n_kv_heads, n_kv_heads divide n_heads and d_head be 64 or 128");
   TORCH_CHECK(B <= kc.size(0) && pos.numel() >= B, "decode_attention: batch larger than the cache or the position vector");
   TORCH_CHECK(q.dim() == 2 && q.stride(1) == 1 && q.size(1) >= H * dh, "q must be [B, >= H*dh] with unit inner stride");
   TORCH_CHECK(out.dim() == 2 && out.size(0) == B && out.size(1) == H * dh && out.stride(1) == 1, "out must be [B, H*dh]");
@@ -470,19 +484,21 @@ void decode_attention(const Tensor& q, const Tensor& kc, const Tensor& vc, const
   Tensor po = torch::empty({(long long)B * H * splits * dh}, q.options().dtype(at::kFloat));
   Tensor pml = torch::empty({(long long)B * H * splits * 2}, q.options().dtype(at::kFloat));
   pb::decode_attention_launch(q.data_ptr(), q.stride(0), kc.data_ptr(), vc.data_ptr(), pos.data_ptr<int>(), out.data_ptr(), out.stride(0),
-                              po.data_ptr<float>(), pml.data_ptr<float>(), B, H, dh, S, float(scale),
+                              po.data_ptr<float>(), pml.data_ptr<float>(), B, H, Hkv, dh, S, float(scale),
                               alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr, stream_of(q));
   g_launches += 2;
 }
 void decode_append(Tensor& qkv, const Tensor& pos, Tensor& kc, Tensor& vc, const c10::optional<Tensor>& cos_t,
-                   const c10::optional<Tensor>& sin_t, int n_heads, const c10::optional<Tensor>& slot) {
+                   const c10::optional<Tensor>& sin_t, int n_heads, const c10::optional<Tensor>& slot, int n_kv_heads) {
   check_bf16(qkv, "qkv");
   check_bf16(kc, "k_cache");
   check_bf16(vc, "v_cache");
   check_i32(pos, "pos");
-  TORCH_CHECK(kc.dim() == 4 && kc.is_contiguous() && vc.sizes() == kc.sizes() && vc.is_contiguous(), "k/v cache must be contiguous [B_max, H, S_max, dh]");
-  const int B = int(qkv.size(0)), H = int(kc.size(1)), S = int(kc.size(2)), dh = int(kc.size(3));
-  TORCH_CHECK(H == n_heads && qkv.dim() == 2 && qkv.size(1) == 3 * H * dh && qkv.stride(1) == 1, "qkv must be [B, 3*H*dh]");
+  TORCH_CHECK(kc.dim() == 4 && kc.is_contiguous() && vc.sizes() == kc.sizes() && vc.is_contiguous(), "k/v cache must be contiguous [B_max, Hkv, S_max, dh]");
+  n_kv_heads = n_kv_heads == -1 ? n_heads : n_kv_heads;   // -1: multi-head attention
+  const int B = int(qkv.size(0)), Hkv = int(kc.size(1)), H = n_heads, S = int(kc.size(2)), dh = int(kc.size(3));
+  TORCH_CHECK(n_heads > 0 && n_kv_heads > 0 && Hkv == n_kv_heads && n_heads % n_kv_heads == 0, "decode_append: cache heads must equal n_kv_heads and divide n_heads");
+  TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == (H + 2 * Hkv) * dh && qkv.stride(1) == 1, "qkv must be [B, (n_heads+2*n_kv_heads)*d_head]");
   check_aligned16(qkv, "qkv");
   TORCH_CHECK(pos.numel() >= B, "decode_append: position vector shorter than the batch");
   if (slot.has_value()) {
@@ -501,21 +517,24 @@ void decode_append(Tensor& qkv, const Tensor& pos, Tensor& kc, Tensor& vc, const
   c10::cuda::CUDAGuard guard(qkv.device());
   pb::decode_append_launch(qkv.data_ptr(), qkv.stride(0), pos.data_ptr<int>(), kc.data_ptr(), vc.data_ptr(),
                            cos_t.has_value() ? cos_t->data_ptr<float>() : nullptr, sin_t.has_value() ? sin_t->data_ptr<float>() : nullptr,
-                           B, H, dh, S, slot.has_value() ? slot->data_ptr<int>() : nullptr, stream_of(qkv));
+                           B, H, Hkv, dh, S, slot.has_value() ? slot->data_ptr<int>() : nullptr, stream_of(qkv));
   g_launches += 1;
 }
-// query rows of qkv [N, 3*H*dh] in tiles (int32 [T, 4]: slot, first_row, n_rows <= 64, first_pos) against one cache layer
+// query rows of qkv [N, (H+2*Hkv)*dh] in tiles (int32 [T, 4]: slot, first_row, n_rows <= 64, first_pos) against one cache layer
 void cache_attention(const Tensor& qkv, const Tensor& kc, const Tensor& vc, const Tensor& tiles, Tensor& out, int n_heads, double scale,
-                     const c10::optional<Tensor>& alibi_slopes) {
+                     const c10::optional<Tensor>& alibi_slopes, int n_kv_heads) {
   check_bf16(qkv, "qkv");
   check_bf16(kc, "k_cache");
   check_bf16(vc, "v_cache");
   check_bf16(out, "out");
   check_i32(tiles, "tiles");
-  TORCH_CHECK(kc.dim() == 4 && kc.is_contiguous() && vc.sizes() == kc.sizes() && vc.is_contiguous(), "k/v cache must be contiguous [B_max, H, S_max, dh]");
-  const int Bm = int(kc.size(0)), H = int(kc.size(1)), S = int(kc.size(2)), dh = int(kc.size(3));
-  TORCH_CHECK(H == n_heads && (dh == 64 || dh == 128), "cache_attention: cache heads must equal n_heads and d_head be 64 or 128");
-  TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == 3 * H * dh && qkv.stride(1) == 1, "qkv must be [N, 3*H*dh] with unit inner stride");
+  TORCH_CHECK(kc.dim() == 4 && kc.is_contiguous() && vc.sizes() == kc.sizes() && vc.is_contiguous(), "k/v cache must be contiguous [B_max, Hkv, S_max, dh]");
+  n_kv_heads = n_kv_heads == -1 ? n_heads : n_kv_heads;   // -1: multi-head attention
+  const int Bm = int(kc.size(0)), Hkv = int(kc.size(1)), H = n_heads, S = int(kc.size(2)), dh = int(kc.size(3));
+  TORCH_CHECK(n_heads > 0 && n_kv_heads > 0 && Hkv == n_kv_heads && n_heads % n_kv_heads == 0 && (dh == 64 || dh == 128),
+              "cache_attention: cache heads must equal n_kv_heads, n_kv_heads divide n_heads and d_head be 64 or 128");
+  TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == (H + 2 * Hkv) * dh && qkv.stride(1) == 1,
+              "qkv must be [N, (n_heads+2*n_kv_heads)*d_head] with unit inner stride");
   check_aligned16(qkv, "qkv");
   TORCH_CHECK(out.dim() == 2 && out.size(0) == qkv.size(0) && out.size(1) == H * dh && out.stride(1) == 1, "out must be [N, H*dh]");
   check_aligned16(out, "out");
@@ -526,7 +545,7 @@ void cache_attention(const Tensor& qkv, const Tensor& kc, const Tensor& vc, cons
   }
   c10::cuda::CUDAGuard guard(qkv.device());
   pb::cache_attention_launch(qkv.data_ptr(), qkv.stride(0), qkv.size(0), kc.data_ptr(), vc.data_ptr(), tiles.data_ptr<int>(),
-                             int(tiles.size(0)), out.data_ptr(), out.stride(0), Bm, H, dh, S, float(scale),
+                             int(tiles.size(0)), out.data_ptr(), out.stride(0), Bm, H, Hkv, dh, S, float(scale),
                              alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr, stream_of(qkv));
   g_launches += 1;
 }
@@ -1001,21 +1020,21 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fp8_quantize_segments", &fp8_quantize_segments);
   m.def("fp8_update_scales", &fp8_update_scales);
   m.def("attention_fwd", &attention_fwd, py::arg("qkv"), py::arg("out"), py::arg("lse"), py::arg("n_heads"), py::arg("scale"),
-        py::arg("causal"), py::arg("alibi_slopes") = py::none(), py::arg("doc_start") = py::none());
+        py::arg("causal"), py::arg("alibi_slopes") = py::none(), py::arg("doc_start") = py::none(), py::arg("n_kv_heads") = -1);
   m.def("attention_bwd", &attention_bwd, py::arg("qkv"), py::arg("out"), py::arg("dout"), py::arg("lse"), py::arg("dqkv"), py::arg("delta"),
         py::arg("n_heads"), py::arg("scale"), py::arg("causal"), py::arg("alibi_slopes") = py::none(), py::arg("doc_start") = py::none(),
-        py::arg("doc_end") = py::none());
+        py::arg("doc_end") = py::none(), py::arg("n_kv_heads") = -1);
   m.def("doc_bounds", &doc_bounds, py::arg("sequence_id"), py::arg("doc_start"), py::arg("doc_end"));
-  m.def("rope", &rope);
+  m.def("rope", &rope, py::arg("qkv"), py::arg("cos"), py::arg("sin"), py::arg("n_heads"), py::arg("inverse"), py::arg("n_kv_heads") = -1);
   m.def("embed_fwd", &embed_fwd);
   m.def("skinny_gemm", &skinny_gemm, py::arg("x"), py::arg("w"), py::arg("y"), py::arg("bias") = py::none(), py::arg("residual") = py::none(),
         py::arg("epi") = 0);
   m.def("decode_attention", &decode_attention, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("pos"), py::arg("out"),
-        py::arg("n_heads"), py::arg("scale"), py::arg("alibi_slopes") = py::none());
+        py::arg("n_heads"), py::arg("scale"), py::arg("alibi_slopes") = py::none(), py::arg("n_kv_heads") = -1);
   m.def("decode_append", &decode_append, py::arg("qkv"), py::arg("pos"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cos") = py::none(),
-        py::arg("sin") = py::none(), py::arg("n_heads") = 1, py::arg("slot") = py::none());
+        py::arg("sin") = py::none(), py::arg("n_heads") = 1, py::arg("slot") = py::none(), py::arg("n_kv_heads") = -1);
   m.def("cache_attention", &cache_attention, py::arg("qkv"), py::arg("k_cache"), py::arg("v_cache"), py::arg("tiles"), py::arg("out"),
-        py::arg("n_heads"), py::arg("scale"), py::arg("alibi_slopes") = py::none());
+        py::arg("n_heads"), py::arg("scale"), py::arg("alibi_slopes") = py::none(), py::arg("n_kv_heads") = -1);
   m.def("embed_pos", &embed_pos, py::arg("ids"), py::arg("pos"), py::arg("wte"), py::arg("wpe"), py::arg("out"));
   m.def("argmax_advance", &argmax_advance, py::arg("logits"), py::arg("ids"), py::arg("pos") = py::none());
   m.def("embed_bwd", &embed_bwd);

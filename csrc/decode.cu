@@ -6,8 +6,9 @@
 //     ring; one warpgroup issues the wgmmas. Every CTA owns 64 output columns and one K range; when the column tiles alone
 //     cannot fill the GPU, K is split and the fp32 partials are summed in split order by a second kernel (no float atomics,
 //     so the result does not depend on scheduling).
-//   * decode attention: one query per (sequence, head) against the cache, split over 256-key chunks (flash-decoding); the
-//     chunk results (unnormalised o, running max, sum) are combined in chunk order.
+//   * decode attention: one query per (sequence, head) against the cache, split over 256-key chunks (flash-decoding); one CTA
+//     serves the query heads of one kv head (grouped-query attention), so each cached row it loads is scored / weighed for
+//     all of them; the chunk results (unnormalised o, running max, sum) of every query head are combined in chunk order.
 //   * cache attention (scoring): tiles of up to 64 consecutive query rows of one cache slot against the slot's keys on wgmma,
 //     with the causal mask at each row's own position.
 //   * append (RoPE at each row's own position + cache write into the row's slot), embedding at per-row positions, argmax +
@@ -209,87 +210,143 @@ __device__ __forceinline__ float da_warp_sum(float v) {
   return v;
 }
 
-template <int DH, bool ALIBI>
+// One CTA = one (chunk, kv head, sequence). The G = H / HKV query heads of the kv head are taken NG at a time: each pass loads
+// the chunk's key rows once and scores them against the pass's NG queries, then its value rows once for the NG weighted sums
+// (G <= NG: every cached row of the chunk is read once). Per query head the arithmetic is that of one head alone.
+template <int DH, bool ALIBI, int NG>
 __global__ void __launch_bounds__(DA_THREADS)
 decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __nv_bfloat16* __restrict__ kc,
                    const __nv_bfloat16* __restrict__ vc, const int* __restrict__ pos, float* __restrict__ po, float* __restrict__ pml,
-                   int H, int s_max, int n_split, float sc, const float* __restrict__ slopes) {
-  __shared__ float qs[DH];
-  __shared__ float ps[DA_CHUNK];
-  __shared__ float red[2][4];
-  __shared__ float os[4][DH];
-  const int s = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+                   int H, int HKV, int s_max, int n_split, float sc, const float* __restrict__ slopes) {
+  __shared__ float qs[NG][DH];
+  __shared__ float ps[NG][DA_CHUNK];
+  __shared__ float red[2][NG][4];
+  __shared__ float os[4][NG][DH];
+  const int s = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int len = pos[b] + 1;
   const int j0 = s * DA_CHUNK, j1 = min(len, j0 + DA_CHUNK);
   if (j0 >= j1) return;   // chunk past the sequence: the combine kernel reads only the chunks below pos[b] + 1
-  const long long slot = (long long)(b * H + h) * n_split + s;
-  for (int i = tid; i < DH; i += DA_THREADS) qs[i] = __bfloat162float(q[b * ldq + h * DH + i]) * sc;
-  __syncthreads();
-  const long long head = (long long)(b * H + h) * s_max * DH;
-  const float slope2 = ALIBI ? slopes[h] * LOG2E : 0.f;
-  // scores (log2 domain): one key per thread and pass, 16-byte loads of the key row, q broadcast from shared memory
-  float mx = -INFINITY;
-  for (int jj = tid; jj < DA_CHUNK; jj += DA_THREADS) {
-    const int j = j0 + jj;
-    float x = -INFINITY;
-    if (j < j1) {
-      const uint4* kr = reinterpret_cast<const uint4*>(kc + head + (long long)j * DH);
-      float acc = 0.f;
+  const int G = H / HKV;
+  const long long head = (long long)(b * HKV + hk) * s_max * DH;
+  constexpr int PER = DH / 32;
+  for (int h0 = hk * G; h0 < (hk + 1) * G; h0 += NG) {
+    const int ng = min(NG, (hk + 1) * G - h0);   // query heads h0 .. h0 + ng - 1 in this pass
+    for (int i = tid; i < NG * DH; i += DA_THREADS) {
+      const int g = i / DH, e = i - g * DH;
+      qs[g][e] = g < ng ? __bfloat162float(q[b * ldq + (h0 + g) * DH + e]) * sc : 0.f;
+    }
+    __syncthreads();
+    float slope2[NG];
 #pragma unroll
-      for (int c = 0; c < DH / 8; ++c) {
-        const uint4 u = kr[c];
-        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+    for (int g = 0; g < NG; ++g) slope2[g] = ALIBI && g < ng ? slopes[h0 + g] * LOG2E : 0.f;
+    // scores (log2 domain): one key per thread and pass, 16-byte loads of the key row, q broadcast from shared memory
+    float mx[NG];
 #pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          const float2 f = unpack_bf16(w[t]);
-          acc = fmaf(qs[c * 8 + 2 * t], f.x, acc);
-          acc = fmaf(qs[c * 8 + 2 * t + 1], f.y, acc);
+    for (int g = 0; g < NG; ++g) mx[g] = -INFINITY;
+    for (int jj = tid; jj < DA_CHUNK; jj += DA_THREADS) {
+      const int j = j0 + jj;
+      float x[NG];
+#pragma unroll
+      for (int g = 0; g < NG; ++g) x[g] = -INFINITY;
+      if (j < j1) {
+        const uint4* kr = reinterpret_cast<const uint4*>(kc + head + (long long)j * DH);
+        float acc[NG];
+#pragma unroll
+        for (int g = 0; g < NG; ++g) acc[g] = 0.f;
+        // one head: the whole row in flight; several: a 16-byte piece at a time (their queries' registers would spill)
+#pragma unroll(NG == 1 ? DH / 8 : 1)
+        for (int c = 0; c < DH / 8; ++c) {
+          const uint4 u = kr[c];
+          const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+          for (int t = 0; t < 4; ++t) {
+            const float2 f = unpack_bf16(w[t]);
+#pragma unroll
+            for (int g = 0; g < NG; ++g) {
+              acc[g] = fmaf(qs[g][c * 8 + 2 * t], f.x, acc[g]);
+              acc[g] = fmaf(qs[g][c * 8 + 2 * t + 1], f.y, acc[g]);
+            }
+          }
+        }
+#pragma unroll
+        for (int g = 0; g < NG; ++g) {
+          x[g] = acc[g];
+          if (ALIBI) x[g] = fmaf(slope2[g], float(j - (len - 1)), x[g]);   // slope * (key - query)
         }
       }
-      x = acc;
-      if (ALIBI) x = fmaf(slope2, float(j - (len - 1)), x);   // slope * (key - query)
-    }
-    ps[jj] = x;
-    mx = fmaxf(mx, x);
-  }
-  mx = warp_max_f(mx);
-  if (lane == 0) red[0][warp] = mx;
-  __syncthreads();
-  const float m = fmaxf(fmaxf(red[0][0], red[0][1]), fmaxf(red[0][2], red[0][3]));
-  float l = 0.f;
-  for (int jj = tid; jj < DA_CHUNK; jj += DA_THREADS) {
-    const float pv = (j0 + jj < j1) ? exp2f(ps[jj] - m) : 0.f;
-    ps[jj] = pv;
-    l += pv;
-  }
-  l = da_warp_sum(l);
-  if (lane == 0) red[1][warp] = l;
-  __syncthreads();
-  // P.V: warp w takes keys w, w+4, ...; each lane owns DH/32 consecutive output dims (coalesced value rows)
-  constexpr int PER = DH / 32;
-  float o[PER];
 #pragma unroll
-  for (int i = 0; i < PER; ++i) o[i] = 0.f;
-  for (int jj = warp; jj < j1 - j0; jj += 4) {
-    const float pv = ps[jj];
-    const __nv_bfloat16* vr = vc + head + (long long)(j0 + jj) * DH + lane * PER;
-    if constexpr (PER == 2) {
-      const float2 f = unpack_bf16(*reinterpret_cast<const uint32_t*>(vr));
-      o[0] = fmaf(pv, f.x, o[0]), o[1] = fmaf(pv, f.y, o[1]);
-    } else {
-      const uint2 u = *reinterpret_cast<const uint2*>(vr);
-      const float2 f0 = unpack_bf16(u.x), f1 = unpack_bf16(u.y);
-      o[0] = fmaf(pv, f0.x, o[0]), o[1] = fmaf(pv, f0.y, o[1]), o[2] = fmaf(pv, f1.x, o[2]), o[3] = fmaf(pv, f1.y, o[3]);
+      for (int g = 0; g < NG; ++g) {
+        ps[g][jj] = x[g];
+        mx[g] = fmaxf(mx[g], x[g]);
+      }
     }
-  }
 #pragma unroll
-  for (int i = 0; i < PER; ++i) os[warp][lane * PER + i] = o[i];
-  __syncthreads();
-  for (int i = tid; i < DH; i += DA_THREADS) po[slot * DH + i] = ((os[0][i] + os[1][i]) + os[2][i]) + os[3][i];
-  if (tid == 0) {
-    pml[2 * slot] = m;
-    pml[2 * slot + 1] = ((red[1][0] + red[1][1]) + red[1][2]) + red[1][3];
+    for (int g = 0; g < NG; ++g) {
+      mx[g] = warp_max_f(mx[g]);
+      if (lane == 0) red[0][g][warp] = mx[g];
+    }
+    __syncthreads();
+    float m[NG], l[NG];
+#pragma unroll
+    for (int g = 0; g < NG; ++g) {
+      m[g] = fmaxf(fmaxf(red[0][g][0], red[0][g][1]), fmaxf(red[0][g][2], red[0][g][3]));
+      l[g] = 0.f;
+    }
+    for (int jj = tid; jj < DA_CHUNK; jj += DA_THREADS) {
+#pragma unroll
+      for (int g = 0; g < NG; ++g) {
+        const float pv = (j0 + jj < j1) ? exp2f(ps[g][jj] - m[g]) : 0.f;
+        ps[g][jj] = pv;
+        l[g] += pv;
+      }
+    }
+#pragma unroll
+    for (int g = 0; g < NG; ++g) {
+      l[g] = da_warp_sum(l[g]);
+      if (lane == 0) red[1][g][warp] = l[g];
+    }
+    __syncthreads();
+    // P.V: warp w takes keys w, w+4, ...; each lane owns DH/32 consecutive output dims (coalesced value rows)
+    float o[NG][PER];
+#pragma unroll
+    for (int g = 0; g < NG; ++g)
+#pragma unroll
+      for (int i = 0; i < PER; ++i) o[g][i] = 0.f;
+    for (int jj = warp; jj < j1 - j0; jj += 4) {
+      const __nv_bfloat16* vr = vc + head + (long long)(j0 + jj) * DH + lane * PER;
+      float f[PER];
+      if constexpr (PER == 2) {
+        const float2 f0 = unpack_bf16(*reinterpret_cast<const uint32_t*>(vr));
+        f[0] = f0.x, f[1] = f0.y;
+      } else {
+        const uint2 u = *reinterpret_cast<const uint2*>(vr);
+        const float2 f0 = unpack_bf16(u.x), f1 = unpack_bf16(u.y);
+        f[0] = f0.x, f[1] = f0.y, f[2] = f1.x, f[3] = f1.y;
+      }
+#pragma unroll
+      for (int g = 0; g < NG; ++g) {
+        const float pv = ps[g][jj];
+#pragma unroll
+        for (int i = 0; i < PER; ++i) o[g][i] = fmaf(pv, f[i], o[g][i]);
+      }
+    }
+#pragma unroll
+    for (int g = 0; g < NG; ++g)
+#pragma unroll
+      for (int i = 0; i < PER; ++i) os[warp][g][lane * PER + i] = o[g][i];
+    __syncthreads();
+    for (int i = tid; i < ng * DH; i += DA_THREADS) {
+      const int g = i / DH, e = i - g * DH;
+      const long long slot = (long long)(b * H + h0 + g) * n_split + s;
+      po[slot * DH + e] = ((os[0][g][e] + os[1][g][e]) + os[2][g][e]) + os[3][g][e];
+    }
+    if (tid < ng) {
+      const long long slot = (long long)(b * H + h0 + tid) * n_split + s;
+      pml[2 * slot] = fmaxf(fmaxf(red[0][tid][0], red[0][tid][1]), fmaxf(red[0][tid][2], red[0][tid][3]));
+      pml[2 * slot + 1] = ((red[1][tid][0] + red[1][tid][1]) + red[1][tid][2]) + red[1][tid][3];
+    }
+    __syncthreads();   // the next pass reuses the shared buffers
   }
 }
 
@@ -315,8 +372,8 @@ __global__ void __launch_bounds__(DH) decode_combine_kernel(const float* __restr
 // One CTA = one (tile, head): up to 64 query rows of one cache slot, at consecutive positions, against that slot's keys.
 // Warps 0-3 (one warpgroup) own the 64 rows: S = Q K^T on wgmma (both operands in shared memory, K-major), online softmax in
 // registers (log2 domain), O += P V with P as the register A operand and V read MN-major as the cache stores it. Warp 4 is
-// the TMA producer: Q once from the fused qkv, then 128-key K / V tiles through a 2-stage ring from the cache viewed as
-// [B_max * H * S_max, dh] rows. Every row is reduced by one thread quad in a fixed order: no atomics, bitwise repeatable.
+// the TMA producer: Q once from the fused qkv, then 128-key K / V tiles of the head's kv head through a 2-stage ring from the
+// cache viewed as [B_max * HKV * S_max, dh] rows. Every row is reduced by one thread quad in a fixed order: no atomics, bitwise repeatable.
 constexpr int CA_BQ = 64, CA_BKV = 128;
 constexpr int CA_THREADS = 160;
 
@@ -332,7 +389,8 @@ struct CaCfg {
 template <int DH, bool ALIBI>
 __global__ void __launch_bounds__(CA_THREADS)
 cache_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                  const int4* __restrict__ tiles, __nv_bfloat16* __restrict__ out, long long ldo, long long n_q, int H, int s_max, float sc,
+                  const int4* __restrict__ tiles, __nv_bfloat16* __restrict__ out, long long ldo, long long n_q, int H, int HKV, int s_max,
+                  float sc,
                   const float* __restrict__ slopes) {
   using C = CaCfg<DH>;
   extern __shared__ uint8_t smem_raw[];
@@ -367,7 +425,7 @@ cache_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
       prefetch_tmap(&tmQ);
       prefetch_tmap(&tmK);
       prefetch_tmap(&tmV);
-      const int kv_row0 = (tile.x * H + h) * s_max;
+      const int kv_row0 = (tile.x * HKV + h / (H / HKV)) * s_max;
       mbar_expect_tx(q_full, C::Q_BYTES);   // rows past the last qkv row arrive as zeros
 #pragma unroll
       for (int c = 0; c < C::CH; ++c) tma_load_2d(sQ + c * 8192, &tmQ, q_full, h * DH + c * 64, tile.y);
@@ -490,17 +548,18 @@ cache_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
 __global__ void __launch_bounds__(128) decode_append_kernel(__nv_bfloat16* __restrict__ qkv, long long ld, const int* __restrict__ pos,
                                                             const int* __restrict__ slot, __nv_bfloat16* __restrict__ kc,
                                                             __nv_bfloat16* __restrict__ vc, const float* __restrict__ cosT,
-                                                            const float* __restrict__ sinT, int H, int dh, int s_max) {
+                                                            const float* __restrict__ sinT, int H, int HKV, int dh, int s_max) {
   const int b = blockIdx.x, p = pos[b];
   const int sb = slot ? slot[b] : b;   // the cache slot this row writes
-  const int d = H * dh, half = dh / 2, groups = half / 8, vec = dh / 8;
+  const int d = H * dh, kvd = HKV * dh, half = dh / 2, groups = half / 8, vec = dh / 8;
   __nv_bfloat16* row = qkv + b * ld;
-  const long long cache_row = ((long long)sb * H) * s_max + p;   // + h * s_max: row of head h
+  const long long cache_row = ((long long)sb * HKV) * s_max + p;   // + h * s_max: row of kv head h
   if (cosT != nullptr) {
-    // rotate-half RoPE at position p, the arithmetic of rope_kernel: q in place, k straight into the cache
-    for (int i = threadIdx.x; i < 2 * H * groups; i += blockDim.x) {
-      const int g = i % groups, h = (i / groups) % H, which = i / (groups * H);
-      __nv_bfloat16* src = row + which * d + h * dh + g * 8;
+    // rotate-half RoPE at position p, the arithmetic of rope_kernel: the H q heads in place, the HKV k heads (which follow
+    // them in the row) straight into the cache
+    for (int i = threadIdx.x; i < (H + HKV) * groups; i += blockDim.x) {
+      const int g = i % groups, h = i / groups;
+      __nv_bfloat16* src = row + h * dh + g * 8;
       const uint4 a = *reinterpret_cast<const uint4*>(src);
       const uint4 bb = *reinterpret_cast<const uint4*>(src + half);
       const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {bb.x, bb.y, bb.z, bb.w};
@@ -514,21 +573,21 @@ __global__ void __launch_bounds__(128) decode_append_kernel(__nv_bfloat16* __res
         oa[k] = pack_bf16(x1.x * c0 - x2.x * s0, x1.y * c1 - x2.y * s1);
         ob[k] = pack_bf16(x2.x * c0 + x1.x * s0, x2.y * c1 + x1.y * s1);
       }
-      __nv_bfloat16* dst = which == 0 ? src : kc + (cache_row + (long long)h * s_max) * dh + g * 8;
+      __nv_bfloat16* dst = h < H ? src : kc + (cache_row + (long long)(h - H) * s_max) * dh + g * 8;
       *reinterpret_cast<uint4*>(dst) = make_uint4(oa[0], oa[1], oa[2], oa[3]);
       *reinterpret_cast<uint4*>(dst + half) = make_uint4(ob[0], ob[1], ob[2], ob[3]);
     }
   } else {
-    for (int i = threadIdx.x; i < H * vec; i += blockDim.x) {
+    for (int i = threadIdx.x; i < HKV * vec; i += blockDim.x) {
       const int h = i / vec, c = i % vec;
       *reinterpret_cast<uint4*>(kc + (cache_row + (long long)h * s_max) * dh + c * 8) =
           *reinterpret_cast<const uint4*>(row + d + h * dh + c * 8);
     }
   }
-  for (int i = threadIdx.x; i < H * vec; i += blockDim.x) {
+  for (int i = threadIdx.x; i < HKV * vec; i += blockDim.x) {
     const int h = i / vec, c = i % vec;
     *reinterpret_cast<uint4*>(vc + (cache_row + (long long)h * s_max) * dh + c * 8) =
-        *reinterpret_cast<const uint4*>(row + 2 * d + h * dh + c * 8);
+        *reinterpret_cast<const uint4*>(row + d + kvd + h * dh + c * 8);
   }
 }
 
@@ -630,48 +689,58 @@ void skinny_gemm_launch(const SkinnyArgs& a, float* partials, cudaStream_t st) {
 int decode_attention_splits(int s_max) { return (s_max + DA_CHUNK - 1) / DA_CHUNK; }
 
 void decode_attention_launch(const void* q, long long ldq, const void* kc, const void* vc, const int* pos, void* out, long long ldo,
-                             float* partial_o, float* partial_ml, int B, int H, int dh, int s_max, float scale, const float* alibi_slopes,
-                             cudaStream_t st) {
+                             float* partial_o, float* partial_ml, int B, int H, int Hkv, int dh, int s_max, float scale,
+                             const float* alibi_slopes, cudaStream_t st) {
   if (B < 1) return;
+  if (Hkv < 1 || H % Hkv) throw std::runtime_error("photon_b200 decode attention: the kv head count must divide the head count");
   const int n_split = decode_attention_splits(s_max);
-  const dim3 grid(n_split, H, B);
+  const dim3 grid(n_split, Hkv, B);
+  const int G = H / Hkv;
   const auto* qq = (const __nv_bfloat16*)q;
   const auto* kk = (const __nv_bfloat16*)kc;
   const auto* vv = (const __nv_bfloat16*)vc;
   const float sc = scale * LOG2E;
 #define PB_DA(D, A)                                                                                                         \
   {                                                                                                                         \
-    decode_attn_kernel<D, A><<<grid, DA_THREADS, 0, st>>>(qq, ldq, kk, vv, pos, partial_o, partial_ml, H, s_max, n_split, sc, \
-                                                         alibi_slopes);                                                     \
+    if (G == 1) PB_DA_NG(D, A, 1)                                                                                           \
+    else if (G == 2) PB_DA_NG(D, A, 2)                                                                                      \
+    else if (G <= 4) PB_DA_NG(D, A, 4)                                                                                      \
+    else PB_DA_NG(D, A, 8)                                                                                                  \
     PB_DECODE_CHECK("decode attention");                                                                                    \
     decode_combine_kernel<D><<<dim3(H, B), D, 0, st>>>(partial_o, partial_ml, pos, (__nv_bfloat16*)out, ldo, H, n_split);   \
     PB_DECODE_CHECK("decode attention combine");                                                                            \
     return;                                                                                                                 \
   }
+#define PB_DA_NG(D, A, NG)                                                                                                   \
+  decode_attn_kernel<D, A, NG><<<grid, DA_THREADS, 0, st>>>(qq, ldq, kk, vv, pos, partial_o, partial_ml, H, Hkv, s_max, n_split, sc, \
+                                                           alibi_slopes);
   if (dh == 64 && !alibi_slopes) PB_DA(64, false)
   if (dh == 64) PB_DA(64, true)
   if (dh == 128 && !alibi_slopes) PB_DA(128, false)
   if (dh == 128) PB_DA(128, true)
+#undef PB_DA_NG
 #undef PB_DA
   throw std::runtime_error("photon_b200 decode attention: d_head must be 64 or 128");
 }
 
 void decode_append_launch(void* qkv, long long ldqkv, const int* pos, void* kc, void* vc, const float* cosT, const float* sinT, int B,
-                          int H, int dh, int s_max, const int* slot, cudaStream_t st) {
+                          int H, int Hkv, int dh, int s_max, const int* slot, cudaStream_t st) {
   if (B < 1) return;
   if (dh % 16) throw std::runtime_error("photon_b200 decode append: d_head must be a multiple of 16");
+  if (Hkv < 1 || H % Hkv) throw std::runtime_error("photon_b200 decode append: the kv head count must divide the head count");
   decode_append_kernel<<<B, 128, 0, st>>>((__nv_bfloat16*)qkv, ldqkv, pos, slot, (__nv_bfloat16*)kc, (__nv_bfloat16*)vc, cosT, sinT, H,
-                                          dh, s_max);
+                                          Hkv, dh, s_max);
   PB_DECODE_CHECK("decode append");
 }
 
 void cache_attention_launch(const void* qkv, long long ldq, long long n_q, const void* kc, const void* vc, const int* tiles, int n_tiles,
-                            void* out, long long ldo, int B_max, int H, int dh, int s_max, float scale, const float* alibi_slopes,
-                            cudaStream_t st) {
+                            void* out, long long ldo, int B_max, int H, int Hkv, int dh, int s_max, float scale,
+                            const float* alibi_slopes, cudaStream_t st) {
   if (n_tiles < 1 || n_q < 1) return;
-  const long long kv_rows = (long long)B_max * H * s_max;
+  if (Hkv < 1 || H % Hkv) throw std::runtime_error("photon_b200 cache attention: the kv head count must divide the head count");
+  const long long kv_rows = (long long)B_max * Hkv * s_max;
   if (kv_rows >= (1LL << 31)) throw std::runtime_error("photon_b200 cache attention: the cache has more than 2^31 rows per layer");
-  const CUtensorMap tq = make_tmap_2d(qkv, 2, false, uint64_t(3) * H * dh, uint64_t(n_q), uint64_t(ldq) * 2, 64, CA_BQ);
+  const CUtensorMap tq = make_tmap_2d(qkv, 2, false, uint64_t(H + 2 * Hkv) * dh, uint64_t(n_q), uint64_t(ldq) * 2, 64, CA_BQ);
   const CUtensorMap tk = make_tmap_2d(kc, 2, false, dh, kv_rows, uint64_t(dh) * 2, 64, CA_BKV);
   const CUtensorMap tv = make_tmap_2d(vc, 2, false, dh, kv_rows, uint64_t(dh) * 2, 64, CA_BKV);
   const dim3 grid(n_tiles, H);
@@ -686,7 +755,8 @@ void cache_attention_launch(const void* qkv, long long ldq, long long n_q, const
       if (e != cudaSuccess) throw std::runtime_error(std::string("cache attention smem attr: ") + cudaGetErrorString(e));       \
       configured = true;                                                                                                         \
     }                                                                                                                            \
-    kern<<<grid, CA_THREADS, CaCfg<D>::SMEM, st>>>(tq, tk, tv, tt, (__nv_bfloat16*)out, ldo, n_q, H, s_max, sc, alibi_slopes);  \
+    kern<<<grid, CA_THREADS, CaCfg<D>::SMEM, st>>>(tq, tk, tv, tt, (__nv_bfloat16*)out, ldo, n_q, H, Hkv, s_max, sc,        \
+                                                   alibi_slopes);                                                               \
     PB_DECODE_CHECK("cache attention");                                                                                          \
     return;                                                                                                                      \
   }

@@ -1,7 +1,9 @@
 // Kernels of the KV-cached greedy decoder (sm_90a): one query row per sequence and step.
 //
-// KV cache layout (one layer): k and v are each bf16 [B_max, H, S_max, dh], row-major, so the keys of one (sequence, head)
-// are S_max contiguous rows of dh elements. The decoder keeps all layers in one tensor [L, 2, B_max, H, S_max, dh]
+// KV cache layout (one layer): k and v are each bf16 [B_max, Hkv, S_max, dh], row-major, so the keys of one (sequence, kv head)
+// are S_max contiguous rows of dh elements. Hkv is the kv head count: H for multi-head attention, fewer with grouped-query
+// attention, where query head h reads kv head h / (H / Hkv). The fused qkv rows are [(H + 2*Hkv)*dh]: q heads, k heads, v heads.
+// The decoder keeps all layers in one tensor [L, 2, B_max, Hkv, S_max, dh]
 // (index 0 = k, 1 = v). Position p of sequence b holds the key / value of token p; positions >= the sequence length are
 // never read.
 //
@@ -38,28 +40,28 @@ int skinny_gemm_splits(int M, int N, int K, int num_sms);
 // skinny_gemm_splits() == 1); the split partials are summed in split order, so the result is bitwise reproducible.
 void skinny_gemm_launch(const SkinnyArgs& a, float* partials, cudaStream_t st);
 
-// Number of KV chunks (one CTA each per sequence and head) for a cache of s_max positions.
+// Number of KV chunks (one CTA each per sequence and kv head) for a cache of s_max positions.
 int decode_attention_splits(int s_max);
 // out[b, h*dh:(h+1)*dh] = softmax(q k^T * scale + alibi) v over keys 0..pos[b] of the cache.
 // q: row b at q + b*ldq (head h at +h*dh); partial_o: fp32 [B, H, splits, dh]; partial_ml: fp32 [B, H, splits, 2].
 void decode_attention_launch(const void* q, long long ldq, const void* kc, const void* vc, const int* pos, void* out, long long ldo,
-                             float* partial_o, float* partial_ml, int B, int H, int dh, int s_max, float scale, const float* alibi_slopes,
-                             cudaStream_t st);
+                             float* partial_o, float* partial_ml, int B, int H, int Hkv, int dh, int s_max, float scale,
+                             const float* alibi_slopes, cudaStream_t st);
 
-// For each row b of the fused qkv [B, 3*H*dh]: rotate q and k (rotate-half tables cos / sin [>= s_max, dh/2], nullptr = no RoPE)
+// For each row b of the fused qkv [B, (H + 2*Hkv)*dh]: rotate q and k (rotate-half tables cos / sin [>= s_max, dh/2], nullptr = no RoPE)
 // at position pos[b] (q in place), and write k, v into the cache at position pos[b] of slot slot[b] (slot == nullptr: slot b).
 void decode_append_launch(void* qkv, long long ldqkv, const int* pos, void* kc, void* vc, const float* cosT, const float* sinT, int B,
-                          int H, int dh, int s_max, const int* slot, cudaStream_t st);
+                          int H, int Hkv, int dh, int s_max, const int* slot, cudaStream_t st);
 
 // Several query rows per cache slot (log-likelihood scoring). tiles: int32 [n_tiles, 4] on the device, each
-// (slot, first_row, n_rows <= 64, first_pos): query rows first_row .. first_row + n_rows - 1 of qkv [n_q, 3*H*dh] (q third, after
+// (slot, first_row, n_rows <= 64, first_pos): query rows first_row .. first_row + n_rows - 1 of qkv [n_q, (H + 2*Hkv)*dh] (q, after
 // RoPE) sit at positions first_pos + i of that slot, and row i attends to keys 0 .. first_pos + i of the slot:
 //   out[first_row + i, h*dh:(h+1)*dh] = softmax(q k^T * scale + alibi) v.
 // Rows outside every tile are not written. The keys of all tile rows must already be in the cache (decode_append first).
 // qkv and out rows must be 16-byte aligned (TMA); d_head 64 or 128.
 void cache_attention_launch(const void* qkv, long long ldq, long long n_q, const void* kc, const void* vc, const int* tiles, int n_tiles,
-                            void* out, long long ldo, int B_max, int H, int dh, int s_max, float scale, const float* alibi_slopes,
-                            cudaStream_t st);
+                            void* out, long long ldo, int B_max, int H, int Hkv, int dh, int s_max, float scale,
+                            const float* alibi_slopes, cudaStream_t st);
 
 // h[b,:] = wte[ids[b],:] + wpe[pos[b],:] (wpe may be nullptr)
 void embed_pos_launch(const int* ids, const int* pos, const void* wte, const void* wpe, void* out, int B, int d, int V, cudaStream_t st);

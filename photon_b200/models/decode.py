@@ -12,7 +12,8 @@ The step is captured as one CUDA graph per batch size and replayed; token ids, p
 buffers, and the host reads back one int32 per sequence. The GEMMs of a step use the weight-streaming skinny GEMM up to
 ``SKINNY_MAX_M`` rows and the training GEMM above.
 
-Cache layout: bf16 ``[L, 2, B, H, max_seq_len, d_head]`` (k = index 0, v = 1), see ``csrc/decode.h``. It is allocated for the
+Cache layout: bf16 ``[L, 2, B, H_kv, max_seq_len, d_head]`` (k = index 0, v = 1; ``H_kv`` = ``kv_n_heads``, fewer than the query
+heads with grouped-query attention), see ``csrc/decode.h``. It is allocated for the
 largest batch the decoder has been asked to run (at most ``max_batch``). The weights are the engine's bf16 compute shadow,
 also under ``amp_fp8``; the decoder never touches the training workspace or its captured graphs.
 
@@ -60,7 +61,7 @@ class KVDecoder:
         c, dev = self.cfg, self.dev
         self._graphs.clear()   # graphs point into the old buffers
         self.cache = None
-        self.cache = torch.zeros(c.n_layers, 2, b, c.n_heads, self.max_seq_len, c.d_head, dtype=torch.bfloat16, device=dev)
+        self.cache = torch.zeros(c.n_layers, 2, b, c.kv_n_heads, self.max_seq_len, c.d_head, dtype=torch.bfloat16, device=dev)
         self.tok = torch.zeros(b, dtype=torch.int32, device=dev)
         self.pos = torch.zeros(b, dtype=torch.int32, device=dev)
         self.buf = self._row_buffers(b)
@@ -73,7 +74,7 @@ class KVDecoder:
         bf = lambda *s: torch.empty(*s, dtype=torch.bfloat16, device=dev)  # noqa: E731
         f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
         d, dff = c.d_model, c.expansion_ratio * c.d_model
-        x = {"h": bf(n, d) if h is None else h, "ln": bf(n, d), "m": f32(n), "r": f32(n), "qkv": bf(n, 3 * d), "attn": bf(n, d),
+        x = {"h": bf(n, d) if h is None else h, "ln": bf(n, d), "m": f32(n), "r": f32(n), "qkv": bf(n, c.qkv_dim), "attn": bf(n, d),
              "hmid": bf(n, d), "u": bf(n, dff), "z": bf(n, dff)}
         if c.qk_ln:
             x.update(qk_pre=bf(n, d), qk_tmp=bf(n, d))
@@ -100,11 +101,13 @@ class KVDecoder:
         if c.clip_qkv:
             qkv.clamp_(-c.clip_qkv, c.clip_qkv)
         if c.qk_ln:
-            qkv3 = qkv.view(-1, 3, c.d_model)
-            for j in range(2):
-                pre.copy_(qkv3[:, j])
-                ops.layernorm_fwd(pre, w.qk_g[j], w.qk_b[j], tmp, m, r, c.norm_eps)
-                qkv3[:, j].copy_(tmp)
+            T = qkv.shape[0]
+            for j, (lo, n) in enumerate(self.e._qk_parts()):  # noqa: SLF001
+                part = qkv[:, lo:lo + n]
+                p, t = (x.view(-1)[: T * n].view(T, n) for x in (pre, tmp))
+                p.copy_(part)
+                ops.layernorm_fwd(p, w.qk_g[j], w.qk_b[j], t, m, r, c.norm_eps)
+                part.copy_(t)
 
     # ------------------------------------------------------------------ prefill
     def _prefill(self, prompts: list[list[int]], slots: list[int]) -> torch.Tensor:
@@ -114,7 +117,7 @@ class KVDecoder:
         b = len(prompts)
         lens = [len(p) for p in prompts]
         S = -(-max(lens) // 128) * 128
-        d, H, dh, T = c.d_model, c.n_heads, c.d_head, b * S
+        d, H, Hkv, dh, T, W = c.d_model, c.n_heads, c.kv_n_heads, c.d_head, b * S, c.qkv_dim
         ids = torch.zeros(b, S, dtype=torch.long)
         for i, p in enumerate(prompts):
             ids[i, : len(p)] = torch.tensor(p, dtype=torch.long)
@@ -122,7 +125,7 @@ class KVDecoder:
         dst = torch.tensor(slots, dtype=torch.long).to(self.dev, non_blocking=True)
         bf = lambda *s: torch.empty(*s, dtype=torch.bfloat16, device=self.dev)  # noqa: E731
         f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=self.dev)  # noqa: E731
-        h, hmid, ln, qkv, attn = bf(T, d), bf(T, d), bf(T, d), bf(T, 3 * d), bf(T, d)
+        h, hmid, ln, qkv, attn = bf(T, d), bf(T, d), bf(T, d), bf(T, W), bf(T, d)
         m, r, lse = f32(T), f32(T), f32(b, H, S)
         u, z = bf(T, c.expansion_ratio * d), bf(T, c.expansion_ratio * d)
         pre, tmp = (bf(T, d), bf(T, d)) if c.qk_ln else (None, None)
@@ -132,11 +135,11 @@ class KVDecoder:
             ops.linear_fwd(ln, w.wqkv, w.bqkv, qkv)
             self._qkv_post(w, qkv, pre, tmp, m, r)
             if e.rope is not None:
-                ops.rope_(qkv.view(b, S, 3 * d), e.rope[0], e.rope[1], H)
-            ops.attention_fwd(qkv.view(b, S, 3 * d), attn.view(b, S, d), lse, H, self.scale, True, e.alibi)
-            kv = qkv.view(b, S, 3, H, dh)
-            self.cache[i, 0, :, :, :S].index_copy_(0, dst, kv[:, :, 1].transpose(1, 2))   # k / v after clip, qk_ln and RoPE
-            self.cache[i, 1, :, :, :S].index_copy_(0, dst, kv[:, :, 2].transpose(1, 2))
+                ops.rope_(qkv.view(b, S, W), e.rope[0], e.rope[1], H, n_kv_heads=Hkv)
+            ops.attention_fwd(qkv.view(b, S, W), attn.view(b, S, d), lse, H, self.scale, True, e.alibi, n_kv_heads=Hkv)
+            _, k, v = e._sdpa_heads(qkv, b, S)  # noqa: SLF001
+            self.cache[i, 0, :, :, :S].index_copy_(0, dst, k)   # the kv heads' k / v after clip, qk_ln and RoPE
+            self.cache[i, 1, :, :, :S].index_copy_(0, dst, v)
             ops.linear_fwd(attn, w.wo, w.bo, hmid, residual=h)
             ops.layernorm_fwd(hmid, w.g2, w.b2, ln, m, r, c.norm_eps)
             ops.linear_gelu_fwd(ln, w.wup, w.bup, z, u)
@@ -181,11 +184,11 @@ class KVDecoder:
             ops.layernorm_fwd(h, w.g1, w.b1, ln, m, r, c.norm_eps)
             self._linear(ln, w.wqkv, w.bqkv, qkv)
             self._qkv_post(w, qkv, x.get("qk_pre"), x.get("qk_tmp"), m, r)
-            ops.decode_append(qkv, pos, kc, vc, e.rope, c.n_heads, slot)
+            ops.decode_append(qkv, pos, kc, vc, e.rope, c.n_heads, slot, n_kv_heads=c.kv_n_heads)
             if tiles is None:
-                ops.decode_attention(qkv, kc, vc, pos, attn, c.n_heads, self.scale, e.alibi)
+                ops.decode_attention(qkv, kc, vc, pos, attn, c.n_heads, self.scale, e.alibi, n_kv_heads=c.kv_n_heads)
             else:
-                ops.cache_attention(qkv, kc, vc, tiles, attn, c.n_heads, self.scale, e.alibi)
+                ops.cache_attention(qkv, kc, vc, tiles, attn, c.n_heads, self.scale, e.alibi, n_kv_heads=c.kv_n_heads)
             self._linear(attn, w.wo, w.bo, hmid, residual=h)
             ops.layernorm_fwd(hmid, w.g2, w.b2, ln, m, r, c.norm_eps)
             self._linear(ln, w.wup, w.bup, u, gelu=True, pre=z)

@@ -250,7 +250,7 @@ class B200Engine:
             w.d_bqkv, w.d_bo, w.d_bup, w.d_bdown = (vg(p + "attn.Wqkv.bias"), vg(p + "attn.out_proj.bias"),
                                                     vg(p + "ffn.up_proj.bias"), vg(p + "ffn.down_proj.bias"))
             w.d_g1, w.d_b1, w.d_g2, w.d_b2 = vg(p + "norm_1.weight"), vg(p + "norm_1.bias"), vg(p + "norm_2.weight"), vg(p + "norm_2.bias")
-            # attn_config.qk_ln: LayerNorm over d_model on the query and key projections
+            # attn_config.qk_ln: LayerNorm on the query (d_model) and key (kv_n_heads * d_head) projections
             w.qk_g = [v32(p + "attn.q_ln.weight"), v32(p + "attn.k_ln.weight")]
             w.qk_b = [v32(p + "attn.q_ln.bias"), v32(p + "attn.k_ln.bias")]
             w.d_qk_g = [vg(p + "attn.q_ln.weight"), vg(p + "attn.k_ln.weight")]
@@ -381,7 +381,7 @@ class B200Engine:
         self._ws.clear()  # one live shape at a time (activations dominate memory)
         self._graphs.clear()  # captured graphs point into the old workspace
         c, dev = self.cfg, self.device
-        T, d, H, L = b * S, c.d_model, c.n_heads, c.n_layers
+        T, d, H, L, W = b * S, c.d_model, c.n_heads, c.n_layers, c.qkv_dim
         bf = lambda *s: torch.empty(*s, dtype=torch.bfloat16, device=dev)  # noqa: E731
         f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
         ws: dict[str, Any] = {"h": [bf(T, d) for _ in range(L + 1)], "layers": []}
@@ -391,21 +391,21 @@ class B200Engine:
                 continue
             if self.fp8:   # the GEMM inputs exist only as E4M3 (1 byte): 7·T·d instead of 12·T·d bytes of saved activations
                 u8 = lambda *s: torch.empty(*s, dtype=torch.uint8, device=dev)  # noqa: E731
-                ws["layers"].append({"ln1": u8(T, d), "m1": f32(T), "r1": f32(T), "qkv": bf(T, 3 * d), "attn": bf(T, d), "attn8": u8(T, d),
+                ws["layers"].append({"ln1": u8(T, d), "m1": f32(T), "r1": f32(T), "qkv": bf(T, W), "attn": bf(T, d), "attn8": u8(T, d),
                                      "lse": f32(b, H, S), "hmid": bf(T, d), "ln2": u8(T, d), "m2": f32(T), "r2": f32(T),
                                      "z": bf(T, c.expansion_ratio * d), "u": u8(T, c.expansion_ratio * d)})
             else:
-                ws["layers"].append({"ln1": bf(T, d), "m1": f32(T), "r1": f32(T), "qkv": bf(T, 3 * d), "attn": bf(T, d),
+                ws["layers"].append({"ln1": bf(T, d), "m1": f32(T), "r1": f32(T), "qkv": bf(T, W), "attn": bf(T, d),
                                      "lse": f32(b, H, S), "hmid": bf(T, d), "ln2": bf(T, d), "m2": f32(T), "r2": f32(T),
                                      "z": bf(T, c.expansion_ratio * d), "u": bf(T, c.expansion_ratio * d)})
             if c.clip_qkv:
-                ws["layers"][-1]["clipmask"] = torch.empty(T, 3 * d, dtype=torch.bool, device=dev)
+                ws["layers"][-1]["clipmask"] = torch.empty(T, W, dtype=torch.bool, device=dev)
             if c.qk_ln:   # pre-LayerNorm q / k (inputs of the two LN backward passes) and their row statistics
-                ws["layers"][-1].update(qk_pre=[bf(T, d), bf(T, d)], qk_m=[f32(T), f32(T)], qk_r=[f32(T), f32(T)])
-        if c.qk_ln:
+                ws["layers"][-1].update(qk_pre=[bf(T, d), bf(T, c.kv_dim)], qk_m=[f32(T), f32(T)], qk_r=[f32(T), f32(T)])
+        if c.qk_ln:   # scratch of the q / k LayerNorms, viewed at the width of the part in use (see _qk_parts)
             ws.update(qk_tmp=bf(T, d), qk_tmp2=bf(T, d))
         ws.update(lnf=bf(T, d), mf=f32(T), rf=f32(T), dlnf=bf(T, d), dh=bf(T, d), dhmid=bf(T, d), dln=bf(T, d),
-                  dqkv=bf(T, 3 * d), dattn=bf(T, d), dz=bf(T, c.expansion_ratio * d), delta=f32(b, H, S),
+                  dqkv=bf(T, W), dattn=bf(T, d), dz=bf(T, c.expansion_ratio * d), delta=f32(b, H, S),
                   logits=bf(min(self.lm_head_chunk, T), c.vocab_size))
         if self.fp8:   # E5M2 copy of the gradient currently flowing backward (one buffer, viewed at the width in use)
             ws["g8"] = torch.empty(T * max(c.expansion_ratio, 3) * d, dtype=torch.uint8, device=dev)
@@ -419,19 +419,36 @@ class B200Engine:
     def _kernel_attention(self, S: int) -> bool:
         return self.attn_mode == "b200" and S % 128 == 0
 
+    def _qk_parts(self) -> tuple[tuple[int, int], tuple[int, int]]:
+        """(first column, width) of q and of k in a fused qkv row: what ``q_ln`` / ``k_ln`` normalise."""
+        c = self.cfg
+        return (0, c.d_model), (c.d_model, c.kv_dim)
+
+    def _sdpa_heads(self, qkv: torch.Tensor, b: int, S: int) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """q [b, H, S, dh] and k, v [b, H_kv, S, dh]: views of the fused qkv."""
+        c = self.cfg
+        x = qkv.view(b, S, c.qkv_dim)
+        d, kvd = c.d_model, c.kv_dim
+        q = x[..., :d].view(b, S, c.n_heads, c.d_head).transpose(1, 2)
+        k, v = (x[..., lo:lo + kvd].view(b, S, c.kv_n_heads, c.d_head).transpose(1, 2) for lo in (d, d + kvd))
+        return q, k, v
+
     def _attention_fwd(self, lw: dict[str, Any], ws: dict[str, Any], b: int, S: int) -> None:
         c = self.cfg
         scale = 1.0 / math.sqrt(c.d_head)
         doc = ws["sequence_id"] is not None
         if self._kernel_attention(S):
-            ops.attention_fwd(lw["qkv"].view(b, S, 3 * c.d_model), lw["attn"].view(b, S, c.d_model), lw["lse"], c.n_heads, scale, True,
-                              self.alibi, ws["doc_start"] if doc else None)
+            ops.attention_fwd(lw["qkv"].view(b, S, c.qkv_dim), lw["attn"].view(b, S, c.d_model), lw["lse"], c.n_heads, scale, True,
+                              self.alibi, ws["doc_start"] if doc else None, n_kv_heads=c.kv_n_heads)
             return
         # library attention: kernels.attention=torch, an unsupported d_head, or a sequence length that is not a multiple
         # of the 128-row tiles (the shipped configs use 2048)
-        q, k, v = lw["qkv"].view(b, S, 3, c.n_heads, c.d_head).permute(2, 0, 3, 1, 4)
-        o = F.scaled_dot_product_attention(q, k, v, scale=scale, **self._sdpa_mask(S, q.dtype, ws["sequence_id"]))
+        q, k, v = self._sdpa_heads(lw["qkv"], b, S)
+        o = F.scaled_dot_product_attention(q, k, v, scale=scale, **self._sdpa_mask(S, q.dtype, ws["sequence_id"]), **self._gqa())
         lw["attn"].view(b, S, c.n_heads, c.d_head).copy_(o.transpose(1, 2))
+
+    def _gqa(self) -> dict[str, Any]:
+        return {"enable_gqa": True} if self.cfg.kv_n_heads != self.cfg.n_heads else {}
 
     def _sdpa_mask(self, S: int, dtype: torch.dtype, sequence_id: torch.Tensor | None = None) -> dict[str, Any]:
         if self.alibi is None and sequence_id is None:
@@ -450,20 +467,21 @@ class B200Engine:
         scale = 1.0 / math.sqrt(c.d_head)
         doc = ws["sequence_id"] is not None
         if self._kernel_attention(S):
-            ops.attention_bwd(lw["qkv"].view(b, S, 3 * c.d_model), lw["attn"].view(b, S, c.d_model),
-                              ws["dattn"].view(b, S, c.d_model), lw["lse"], ws["dqkv"].view(b, S, 3 * c.d_model), ws["delta"],
-                              c.n_heads, scale, True, self.alibi, ws["doc_start"] if doc else None, ws["doc_end"] if doc else None)
+            ops.attention_bwd(lw["qkv"].view(b, S, c.qkv_dim), lw["attn"].view(b, S, c.d_model),
+                              ws["dattn"].view(b, S, c.d_model), lw["lse"], ws["dqkv"].view(b, S, c.qkv_dim), ws["delta"],
+                              c.n_heads, scale, True, self.alibi, ws["doc_start"] if doc else None, ws["doc_end"] if doc else None,
+                              n_kv_heads=c.kv_n_heads)
             if self.rope is not None:   # gradients w.r.t. the un-rotated q, k
-                ops.rope_(ws["dqkv"].view(b, S, 3 * c.d_model), self.rope[0], self.rope[1], c.n_heads, inverse=True)
+                ops.rope_(ws["dqkv"].view(b, S, c.qkv_dim), self.rope[0], self.rope[1], c.n_heads, inverse=True, n_kv_heads=c.kv_n_heads)
             return
         with torch.enable_grad():
-            qkv = lw["qkv"].view(b, S, 3, c.n_heads, c.d_head).detach().requires_grad_(True)
-            q, k, v = qkv.permute(2, 0, 3, 1, 4)
-            o = F.scaled_dot_product_attention(q, k, v, scale=scale, **self._sdpa_mask(S, q.dtype, ws["sequence_id"]))
+            qkv = lw["qkv"].view(b, S, c.qkv_dim).detach().requires_grad_(True)
+            q, k, v = self._sdpa_heads(qkv, b, S)
+            o = F.scaled_dot_product_attention(q, k, v, scale=scale, **self._sdpa_mask(S, q.dtype, ws["sequence_id"]), **self._gqa())
             (g,) = torch.autograd.grad(o, qkv, ws["dattn"].view(b, S, c.n_heads, c.d_head).transpose(1, 2))
-        ws["dqkv"].view(b, S, 3, c.n_heads, c.d_head).copy_(g)
+        ws["dqkv"].view(b, S, c.qkv_dim).copy_(g)
         if self.rope is not None:
-            ops.rope_(ws["dqkv"].view(b, S, 3 * c.d_model), self.rope[0], self.rope[1], c.n_heads, inverse=True)
+            ops.rope_(ws["dqkv"].view(b, S, c.qkv_dim), self.rope[0], self.rope[1], c.n_heads, inverse=True, n_kv_heads=c.kv_n_heads)
 
     def _block_fwd(self, i: int, ws: dict[str, Any], b: int, S: int) -> None:
         """h[i] -> h[i+1]; the block internals land in ws["layers"][i] (also the recompute step under checkpointing)."""
@@ -478,14 +496,15 @@ class B200Engine:
         if c.clip_qkv:   # attn_config.clip_qkv: clamp the fused projection; remember where the gradient passes
             torch.logical_and(lw["qkv"] > -c.clip_qkv, lw["qkv"] < c.clip_qkv, out=lw["clipmask"])
             lw["qkv"].clamp_(-c.clip_qkv, c.clip_qkv)
-        if c.qk_ln:   # the q / k thirds are strided inside the fused buffer: normalise contiguous copies
-            qkv3 = lw["qkv"].view(-1, 3, c.d_model)
-            for j in range(2):
-                lw["qk_pre"][j].copy_(qkv3[:, j])
-                ops.layernorm_fwd(lw["qk_pre"][j], w.qk_g[j], w.qk_b[j], ws["qk_tmp"], lw["qk_m"][j], lw["qk_r"][j], c.norm_eps)
-                qkv3[:, j].copy_(ws["qk_tmp"])
+        if c.qk_ln:   # q / k are strided inside the fused buffer: normalise contiguous copies
+            T = lw["qkv"].shape[0]
+            for j, (lo, n) in enumerate(self._qk_parts()):
+                part, tmp = lw["qkv"][:, lo:lo + n], ws["qk_tmp"].view(-1)[: T * n].view(T, n)
+                lw["qk_pre"][j].copy_(part)
+                ops.layernorm_fwd(lw["qk_pre"][j], w.qk_g[j], w.qk_b[j], tmp, lw["qk_m"][j], lw["qk_r"][j], c.norm_eps)
+                part.copy_(tmp)
         if self.rope is not None:
-            ops.rope_(lw["qkv"].view(b, S, 3 * c.d_model), self.rope[0], self.rope[1], c.n_heads)
+            ops.rope_(lw["qkv"].view(b, S, c.qkv_dim), self.rope[0], self.rope[1], c.n_heads, n_kv_heads=c.kv_n_heads)
         self._attention_fwd(lw, ws, b, S)
         if self.fp8:
             ops.colsum_quant(lw["attn"], None, lw["attn8"], ops.E4M3, M, R("x_attn", i))
@@ -616,12 +635,13 @@ class B200Engine:
             return
         self._attention_bwd(lw, ws, b, S)
         if c.qk_ln:
-            dqkv3 = ws["dqkv"].view(-1, 3, c.d_model)
-            for j in range(2):
-                ws["qk_tmp"].copy_(dqkv3[:, j])
-                ops.layernorm_bwd(ws["qk_tmp"], lw["qk_pre"][j], w.qk_g[j], lw["qk_m"][j], lw["qk_r"][j], None, ws["qk_tmp2"],
-                                  w.d_qk_g[j], w.d_qk_b[j])
-                dqkv3[:, j].copy_(ws["qk_tmp2"])
+            T = ws["dqkv"].shape[0]
+            for j, (lo, n) in enumerate(self._qk_parts()):
+                part = ws["dqkv"][:, lo:lo + n]
+                tmp, tmp2 = (ws[k].view(-1)[: T * n].view(T, n) for k in ("qk_tmp", "qk_tmp2"))
+                tmp.copy_(part)
+                ops.layernorm_bwd(tmp, lw["qk_pre"][j], w.qk_g[j], lw["qk_m"][j], lw["qk_r"][j], None, tmp2, w.d_qk_g[j], w.d_qk_b[j])
+                part.copy_(tmp2)
         if c.clip_qkv:
             ws["dqkv"].mul_(lw["clipmask"])
         if not P.runs((i, "qkv")):

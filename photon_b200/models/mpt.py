@@ -42,12 +42,31 @@ class MPTConfig:
     norm_eps: float = 1e-5
     # attn_config.attn_uses_sequence_id: attention stays inside each document of a packed row (the collator's sequence_id)
     attn_uses_sequence_id: bool = False
+    # attn_config.attn_type grouped_query_attention / multiquery_attention: K / V have kv_n_heads heads (None: n_heads), query
+    # head h attending with kv head h // (n_heads // kv_n_heads)
+    kv_n_heads: int | None = None
     init_std: float | None = None  # None -> kaiming_normal_ (llm-foundry default)
     extra: dict[str, Any] = field(default_factory=dict)
+
+    def __post_init__(self) -> None:
+        if self.kv_n_heads is None:
+            self.kv_n_heads = self.n_heads
+        if self.kv_n_heads < 1 or self.n_heads % self.kv_n_heads:
+            raise ValueError(f"kv_n_heads = {self.kv_n_heads} must divide n_heads = {self.n_heads}")
 
     @property
     def d_head(self) -> int:
         return self.d_model // self.n_heads
+
+    @property
+    def kv_dim(self) -> int:
+        """Width of the k (and of the v) part of the fused QKV projection: ``kv_n_heads * d_head``."""
+        return self.kv_n_heads * self.d_head
+
+    @property
+    def qkv_dim(self) -> int:
+        """Output width of ``Wqkv``: q (``d_model``), then k, then v (``kv_dim`` each)."""
+        return self.d_model + 2 * self.kv_dim
 
     @classmethod
     def from_model_cfg(cls, m: dict[str, Any]) -> "MPTConfig":
@@ -55,6 +74,28 @@ class MPTConfig:
         m = dict(m)
         attn = dict(m.pop("attn_config", {}) or {})
         rope_cfg = attn.pop("rope_impl", None)
+        n_heads = m["n_heads"]
+        attn_type = attn.pop("attn_type", "multihead_attention")
+        kv = attn.pop("kv_n_heads", None)
+        if attn_type == "multihead_attention":
+            kv = None   # ignored, as llm-foundry does
+        elif attn_type == "multiquery_attention":
+            kv = 1
+        elif attn_type == "grouped_query_attention":
+            if kv is None:
+                raise ValueError("attn_config.attn_type: grouped_query_attention needs attn_config.kv_n_heads")
+            if int(kv) < 1 or n_heads % int(kv):
+                raise ValueError(f"attn_config.kv_n_heads = {kv} must divide n_heads = {n_heads}")
+            kv = int(kv)
+        else:
+            raise ValueError(f"unknown attn_config.attn_type {attn_type!r} (multihead_attention, grouped_query_attention or "
+                             "multiquery_attention)")
+        if attn_type != "multihead_attention":
+            # both change the names or shapes of the attention parameters, which are built here only for multi-head attention
+            if attn.get("qk_gn"):
+                raise ValueError(f"attn_config.qk_gn is not supported with {attn_type}")
+            if attn.get("fused_qkv", True) is False:
+                raise ValueError(f"attn_config.fused_qkv: false is not supported with {attn_type}")
         known = dict(
             d_model=m.pop("d_model"), n_heads=m.pop("n_heads"), n_layers=m.pop("n_layers"),
             expansion_ratio=m.pop("expansion_ratio", 4), max_seq_len=m.pop("max_seq_len", 2048),
@@ -62,7 +103,7 @@ class MPTConfig:
             alibi=bool(attn.pop("alibi", False)), alibi_bias_max=attn.pop("alibi_bias_max", 8),
             rope=bool(attn.pop("rope", False)), rope_theta=float(attn.pop("rope_theta", 10000.0)),
             qk_ln=bool(attn.pop("qk_ln", False)), clip_qkv=attn.pop("clip_qkv", None),
-            attn_uses_sequence_id=bool(attn.pop("attn_uses_sequence_id", False)),
+            attn_uses_sequence_id=bool(attn.pop("attn_uses_sequence_id", False)), kv_n_heads=kv,
             no_bias=bool(m.pop("no_bias", False)), learned_pos_emb=bool(m.pop("learned_pos_emb", True)),
         )
         for k in ("name", "init_device"):
@@ -78,7 +119,8 @@ class MPTConfig:
     def num_params(self) -> int:
         d, L, V, S, e = self.d_model, self.n_layers, self.vocab_size, self.max_seq_len, self.expansion_ratio
         b = 0 if self.no_bias else 1
-        per_block = (2 * d) * 2 + (3 * d * d + b * 3 * d) + (d * d + b * d) + (e * d * d + b * e * d) + (e * d * d + b * d)
+        w = self.qkv_dim
+        per_block = (2 * d) * 2 + (w * d + b * w) + (d * d + b * d) + (e * d * d + b * e * d) + (e * d * d + b * d)
         if self.no_bias:
             per_block -= 2 * d  # LN biases dropped too
         return V * d + (S * d if self.learned_pos_emb else 0) + L * per_block + (2 * d if not self.no_bias else d)
@@ -117,11 +159,11 @@ class MPTAttention(nn.Module):
         super().__init__()
         self.cfg = cfg
         d = cfg.d_model
-        self.Wqkv = nn.Linear(d, 3 * d, bias=not cfg.no_bias)
+        self.Wqkv = nn.Linear(d, cfg.qkv_dim, bias=not cfg.no_bias)
         self.out_proj = nn.Linear(d, d, bias=not cfg.no_bias)
         if cfg.qk_ln:
             self.q_ln = nn.LayerNorm(d, eps=cfg.norm_eps)
-            self.k_ln = nn.LayerNorm(d, eps=cfg.norm_eps)
+            self.k_ln = nn.LayerNorm(cfg.kv_dim, eps=cfg.norm_eps)
 
     def forward(self, x: torch.Tensor, rope: tuple[torch.Tensor, torch.Tensor] | None,
                 alibi: torch.Tensor | None, doc_keep: torch.Tensor | None = None) -> torch.Tensor:
@@ -131,15 +173,18 @@ class MPTAttention(nn.Module):
         qkv = self.Wqkv(x)
         if cfg.clip_qkv:
             qkv = qkv.clamp(-cfg.clip_qkv, cfg.clip_qkv)
-        q, k, v = qkv.chunk(3, dim=-1)
+        q, k, v = qkv.split([d, cfg.kv_dim, cfg.kv_dim], dim=-1)
         if cfg.qk_ln:
             q, k = self.q_ln(q).to(q.dtype), self.k_ln(k).to(k.dtype)
-        H, dh = cfg.n_heads, cfg.d_head
-        q, k, v = (t.view(B, S, H, dh).transpose(1, 2) for t in (q, k, v))
+        H, Hkv, dh = cfg.n_heads, cfg.kv_n_heads, cfg.d_head
+        q = q.view(B, S, H, dh).transpose(1, 2)
+        k, v = (t.view(B, S, Hkv, dh).transpose(1, 2) for t in (k, v))
         if rope is not None:
             q, k = apply_rope(q, rope[0][:S], rope[1][:S]), apply_rope(k, rope[0][:S], rope[1][:S])
         scale = 1.0 / math.sqrt(dh)
         if cfg.attn_impl == "torch" or (alibi is not None and cfg.attn_impl != "flash"):
+            if Hkv != H:   # query head h reads kv head h // (H // Hkv)
+                k, v = k.repeat_interleave(H // Hkv, dim=1), v.repeat_interleave(H // Hkv, dim=1)
             att = (q @ k.transpose(-1, -2)) * scale
             if alibi is not None:
                 att = att + alibi[:, :, :S, :S].to(att.dtype)
@@ -155,7 +200,8 @@ class MPTAttention(nn.Module):
                 if doc_keep is not None:
                     mask = mask & doc_keep
                 bias = mask if alibi is None else alibi[:, :, :S, :S].to(q.dtype).masked_fill(~mask, float("-inf"))
-            o = F.scaled_dot_product_attention(q, k, v, attn_mask=bias, is_causal=bias is None, scale=scale)
+            gqa = {"enable_gqa": True} if Hkv != H else {}
+            o = F.scaled_dot_product_attention(q, k, v, attn_mask=bias, is_causal=bias is None, scale=scale, **gqa)
         return self.out_proj(o.transpose(1, 2).reshape(B, S, d))
 
 
@@ -226,9 +272,9 @@ class MPTForCausalLM(nn.Module):
         for name, mod in self.named_modules():
             if isinstance(mod, nn.Linear):
                 if name.endswith("Wqkv"):  # fused: initialise q/k/v slices independently
-                    d = cfg.d_model
-                    for s in range(3):
-                        _fill(mod.weight[s * d:(s + 1) * d], mod.in_features)
+                    d, kvd = cfg.d_model, cfg.kv_dim
+                    for lo, hi in ((0, d), (d, d + kvd), (d + kvd, d + 2 * kvd)):
+                        _fill(mod.weight[lo:hi], mod.in_features)
                 else:
                     _fill(mod.weight, mod.in_features, residual=name.endswith(("out_proj", "down_proj")))
                 if mod.bias is not None:

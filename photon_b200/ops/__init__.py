@@ -259,20 +259,29 @@ def fused_optimizer_step(opt: Any, lr: float, grad_mult: torch.Tensor | float | 
 
 
 # ---------------------------------------------------------------------------- attention
+def _kv(n_heads: int, n_kv_heads: int | None) -> int:
+    return int(n_heads) if n_kv_heads is None else int(n_kv_heads)
+
+
 def attention_fwd(qkv: torch.Tensor, out: torch.Tensor, lse: torch.Tensor, n_heads: int, scale: float, causal: bool = True,
-                  alibi_slopes: torch.Tensor | None = None, doc_start: torch.Tensor | None = None) -> None:
-    """``alibi_slopes``: optional fp32 [n_heads]; adds ``slope_h * (key - query)`` to the scores (MPT ``attn_config.alibi``).
+                  alibi_slopes: torch.Tensor | None = None, doc_start: torch.Tensor | None = None,
+                  n_kv_heads: int | None = None) -> None:
+    """``qkv`` [B, S, (n_heads + 2 * n_kv_heads) * d_head]: the q heads, then the k heads, then the v heads; query head ``h``
+    attends with kv head ``h // (n_heads // n_kv_heads)`` (grouped-query attention; None: ``n_heads``, multi-head).
+    ``alibi_slopes``: optional fp32 [n_heads]; adds ``slope_h * (key - query)`` to the scores (MPT ``attn_config.alibi``).
     ``doc_start``: optional int32 [B*S] from :func:`doc_bounds` (causal only); query ``q`` then sees key ``k`` iff
     ``doc_start[q] <= k <= q``, and key tiles before a query tile's first document are skipped."""
-    ext().attention_fwd(qkv, out, lse, int(n_heads), float(scale), bool(causal), alibi_slopes, doc_start)
+    ext().attention_fwd(qkv, out, lse, int(n_heads), float(scale), bool(causal), alibi_slopes, doc_start, _kv(n_heads, n_kv_heads))
 
 
 def attention_bwd(qkv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor, dqkv: torch.Tensor,
                   delta: torch.Tensor, n_heads: int, scale: float, causal: bool = True,
                   alibi_slopes: torch.Tensor | None = None, doc_start: torch.Tensor | None = None,
-                  doc_end: torch.Tensor | None = None) -> None:
-    """``doc_start`` / ``doc_end`` (both or neither): the document mask of :func:`attention_fwd`."""
-    ext().attention_bwd(qkv, out, dout, lse, dqkv, delta, int(n_heads), float(scale), bool(causal), alibi_slopes, doc_start, doc_end)
+                  doc_end: torch.Tensor | None = None, n_kv_heads: int | None = None) -> None:
+    """``doc_start`` / ``doc_end`` (both or neither): the document mask of :func:`attention_fwd`. ``dqkv`` is shaped like
+    ``qkv``; with grouped-query attention the dK / dV of a kv head are summed over its query heads."""
+    ext().attention_bwd(qkv, out, dout, lse, dqkv, delta, int(n_heads), float(scale), bool(causal), alibi_slopes, doc_start, doc_end,
+                        _kv(n_heads, n_kv_heads))
 
 
 def doc_bounds(sequence_id: torch.Tensor, doc_start: torch.Tensor, doc_end: torch.Tensor) -> None:
@@ -281,10 +290,11 @@ def doc_bounds(sequence_id: torch.Tensor, doc_start: torch.Tensor, doc_end: torc
     ext().doc_bounds(sequence_id, doc_start, doc_end)
 
 
-def rope_(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_heads: int, inverse: bool = False) -> torch.Tensor:
-    """In-place rotary embedding (rotate-half) of the q and k thirds of ``qkv`` [B,S,3d]; ``inverse`` applies the
-    transposed rotation (what the gradients of q and k need)."""
-    ext().rope(qkv, cos, sin, int(n_heads), bool(inverse))
+def rope_(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_heads: int, inverse: bool = False,
+          n_kv_heads: int | None = None) -> torch.Tensor:
+    """In-place rotary embedding (rotate-half) of the ``n_heads`` q heads and ``n_kv_heads`` k heads of ``qkv``
+    [B, S, (n_heads + 2 * n_kv_heads) * d_head]; ``inverse`` applies the transposed rotation (what the gradients of q and k need)."""
+    ext().rope(qkv, cos, sin, int(n_heads), bool(inverse), _kv(n_heads, n_kv_heads))
     return qkv
 
 
@@ -303,27 +313,31 @@ def skinny_gemm(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor, bias: torch
 
 
 def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, pos: torch.Tensor, out: torch.Tensor, n_heads: int,
-                     scale: float, alibi_slopes: torch.Tensor | None = None) -> torch.Tensor:
+                     scale: float, alibi_slopes: torch.Tensor | None = None, n_kv_heads: int | None = None) -> torch.Tensor:
     """One query row per sequence (``q`` [B, >= H*dh]) against one layer of the cache (``k_cache`` / ``v_cache``
-    [B_max, H, S_max, dh]) over keys ``0..pos[b]`` (int32 on the device); ``out`` [B, H*dh]."""
-    ext().decode_attention(q, k_cache, v_cache, pos, out, int(n_heads), float(scale), alibi_slopes)
+    [B_max, n_kv_heads, S_max, dh]) over keys ``0..pos[b]`` (int32 on the device); ``out`` [B, H*dh]. One CTA serves all query
+    heads of a kv head, so each cached row is read once per group."""
+    ext().decode_attention(q, k_cache, v_cache, pos, out, int(n_heads), float(scale), alibi_slopes, _kv(n_heads, n_kv_heads))
     return out
 
 
 def decode_append(qkv: torch.Tensor, pos: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor,
-                  rope: tuple[torch.Tensor, torch.Tensor] | None, n_heads: int, slot: torch.Tensor | None = None) -> None:
-    """Rotate q / k of every row of the fused ``qkv`` [B, 3d] at position ``pos[b]`` (``rope`` = the ``rope_`` tables, or None)
-    and write k / v into the cache at ``pos[b]`` of slot ``slot[b]`` (int32 on the device; None: row ``b`` writes slot ``b``)."""
+                  rope: tuple[torch.Tensor, torch.Tensor] | None, n_heads: int, slot: torch.Tensor | None = None,
+                  n_kv_heads: int | None = None) -> None:
+    """Rotate q / k of every row of the fused ``qkv`` [B, (n_heads + 2 * n_kv_heads) * d_head] at position ``pos[b]`` (``rope`` =
+    the ``rope_`` tables, or None) and write the k / v heads into the cache at ``pos[b]`` of slot ``slot[b]`` (int32 on the
+    device; None: row ``b`` writes slot ``b``)."""
     cos, sin = rope if rope is not None else (None, None)
-    ext().decode_append(qkv, pos, k_cache, v_cache, cos, sin, int(n_heads), slot)
+    ext().decode_append(qkv, pos, k_cache, v_cache, cos, sin, int(n_heads), slot, _kv(n_heads, n_kv_heads))
 
 
 def cache_attention(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, tiles: torch.Tensor, out: torch.Tensor,
-                    n_heads: int, scale: float, alibi_slopes: torch.Tensor | None = None) -> torch.Tensor:
+                    n_heads: int, scale: float, alibi_slopes: torch.Tensor | None = None, n_kv_heads: int | None = None) -> torch.Tensor:
     """Several query rows per cache slot on the tensor cores. ``tiles`` int32 [T, 4] on the device, one row per tile
-    ``(slot, first_row, n_rows <= 64, first_pos)``: rows ``first_row + i`` of ``qkv`` [N, 3d] (q after RoPE) sit at positions
-    ``first_pos + i`` of that slot and attend to its keys ``0 .. first_pos + i``. Writes those rows of ``out`` [N, d] only."""
-    ext().cache_attention(qkv, k_cache, v_cache, tiles, out, int(n_heads), float(scale), alibi_slopes)
+    ``(slot, first_row, n_rows <= 64, first_pos)``: rows ``first_row + i`` of ``qkv`` [N, (n_heads + 2 * n_kv_heads) * d_head]
+    (q after RoPE) sit at positions ``first_pos + i`` of that slot and attend to its keys ``0 .. first_pos + i`` (query head
+    ``h`` to kv head ``h // (n_heads // n_kv_heads)``). Writes those rows of ``out`` [N, d] only."""
+    ext().cache_attention(qkv, k_cache, v_cache, tiles, out, int(n_heads), float(scale), alibi_slopes, _kv(n_heads, n_kv_heads))
     return out
 
 
