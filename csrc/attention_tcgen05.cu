@@ -30,6 +30,7 @@
 
 #include "attention_tcgen05.h"
 #include "gemm_tcgen05.h"
+#include "launch.h"
 #include "ptx.cuh"
 #include "wgmma.cuh"
 
@@ -560,62 +561,29 @@ __global__ void __launch_bounds__(DOC_THREADS) doc_bounds_kernel(const long long
   }
 }
 
-template <typename K>
-void set_smem(K kern, int bytes) {
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) throw std::runtime_error(std::string("attention smem attr: ") + cudaGetErrorString(e));
-}
-
 }  // namespace
 
 void attention_fwd_launch(const void* qkv, void* out, float* lse, int B, int S, int H, int Hkv, int dh, float scale, bool causal,
-                          int num_sms, cudaStream_t st, const float* alibi_slopes, const int* doc_start) {
-  (void)num_sms;
+                          cudaStream_t st, const float* alibi_slopes, const int* doc_start) {
   if (S % 128) throw std::runtime_error("photon_b200 attention: sequence length must be a multiple of 128");
   if (dh != 64 && dh != 128) throw std::runtime_error("photon_b200 attention: d_head must be 64 or 128");
-  if (doc_start && !causal) throw std::runtime_error("photon_b200 attention: the document mask needs the causal mask");
-  if (Hkv < 1 || H % Hkv) throw std::runtime_error("photon_b200 attention: the kv head count must divide the head count");
   const uint64_t w = uint64_t(H + 2 * Hkv) * dh;   // fused qkv row width
   CUtensorMap tm = make_tmap_2d(qkv, 2, false, w, uint64_t(B) * S, w * 2, 64, 128);
   const dim3 grid(S / 128, B * H);
-#define PB_FWD_G(DHV, AL, DOC, GQA)                                                                                  \
-  {                                                                                                                  \
-    static bool once = (set_smem(attn_fwd_kernel<DHV, AL, DOC, GQA>, FwdCfg<DHV>::SMEM), true);                      \
-    (void)once;                                                                                                      \
-    attn_fwd_kernel<DHV, AL, DOC, GQA><<<grid, 384, FwdCfg<DHV>::SMEM, st>>>(tm, (__nv_bfloat16*)out, lse, S, H, scale, \
-                                                                            causal ? 1 : 0, alibi_slopes, doc_start, \
-                                                                            Hkv);                                    \
-  }
-#define PB_FWD(DHV, AL, DOC)                                                                                         \
-  {                                                                                                                  \
-    if (Hkv == H) PB_FWD_G(DHV, AL, DOC, false)                                                                      \
-    else PB_FWD_G(DHV, AL, DOC, true)                                                                                \
-  }
-  if (!doc_start) {
-    if (dh == 64 && !alibi_slopes) PB_FWD(64, false, false)
-    else if (dh == 64) PB_FWD(64, true, false)
-    else if (!alibi_slopes) PB_FWD(128, false, false)
-    else PB_FWD(128, true, false)
-  } else {
-    if (dh == 64 && !alibi_slopes) PB_FWD(64, false, true)
-    else if (dh == 64) PB_FWD(64, true, true)
-    else if (!alibi_slopes) PB_FWD(128, false, true)
-    else PB_FWD(128, true, true)
-  }
-#undef PB_FWD
-#undef PB_FWD_G
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("attention fwd launch: ") + cudaGetErrorString(e));
+  with_bools([&](auto gqa, auto alibi, auto wide, auto doc) {
+    constexpr int DHV = wide ? 128 : 64;
+    auto kern = attn_fwd_kernel<DHV, alibi, doc, gqa>;
+    opt_in_smem(kern, FwdCfg<DHV>::SMEM);
+    kern<<<grid, 384, FwdCfg<DHV>::SMEM, st>>>(tm, (__nv_bfloat16*)out, lse, S, H, scale, causal ? 1 : 0, alibi_slopes, doc_start, Hkv);
+  }, Hkv != H, alibi_slopes != nullptr, dh == 128, doc_start != nullptr);
+  launched("attention fwd");
 }
 
-int attention_bwd_launch(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta, float* dq_acc,
-                         int B, int S, int H, int Hkv, int dh, float scale, bool causal, int num_sms, cudaStream_t st, const float* alibi_slopes,
-                         const int* doc_start, const int* doc_end) {
+void attention_bwd_launch(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta, float* dq_acc,
+                          int B, int S, int H, int Hkv, int dh, float scale, bool causal, int num_sms, cudaStream_t st, const float* alibi_slopes,
+                          const int* doc_start, const int* doc_end) {
   if (S % 128) throw std::runtime_error("photon_b200 attention: sequence length must be a multiple of 128");
   if (dh != 64 && dh != 128) throw std::runtime_error("photon_b200 attention backward: d_head must be 64 or 128");
-  if (bool(doc_start) != bool(doc_end)) throw std::runtime_error("photon_b200 attention backward: doc_start and doc_end go together");
-  if (doc_start && !causal) throw std::runtime_error("photon_b200 attention: the document mask needs the causal mask");
-  if (Hkv < 1 || H % Hkv) throw std::runtime_error("photon_b200 attention: the kv head count must divide the head count");
   const int sms = num_sms > 0 ? num_sms : 132;
   const int d = H * dh;
   const uint64_t w = uint64_t(H + 2 * Hkv) * dh;   // fused qkv row width
@@ -625,47 +593,27 @@ int attention_bwd_launch(const void* qkv, const void* out, const void* dout, con
     const long long n8 = rows * H * (dh / 8);
     const int blocks = int(std::min<long long>((n8 + 255) / 256, sms * 16));
     attn_bwd_delta_kernel<<<blocks, 256, 0, st>>>((const __nv_bfloat16*)out, (const __nv_bfloat16*)dout, delta, S, H, dh, rows);
+    launched("attention bwd delta");
   }
   CUtensorMap tmKV = make_tmap_2d(qkv, 2, false, w, uint64_t(rows), w * 2, 64, 128);
   CUtensorMap tmQ = make_tmap_2d(qkv, 2, false, w, uint64_t(rows), w * 2, 64, 64);
   CUtensorMap tmDO = make_tmap_2d(dout, 2, false, uint64_t(d), uint64_t(rows), uint64_t(d) * 2, 64, 64);
   const dim3 grid(S / 128, B * Hkv);
-#define PB_BWD_G(DHV, AL, DOC, GQA)                                                                                  \
-  {                                                                                                                  \
-    static bool once = (set_smem(attn_bwd_kernel<DHV, AL, DOC, GQA>, BwdCfg<DHV>::SMEM), true);                      \
-    (void)once;                                                                                                      \
-    attn_bwd_kernel<DHV, AL, DOC, GQA><<<grid, 384, BwdCfg<DHV>::SMEM, st>>>(tmKV, tmQ, tmDO, lse, delta, (__nv_bfloat16*)dqkv, \
-                                                                            S, H, scale, causal ? 1 : 0, dq_acc,        \
-                                                                            alibi_slopes, doc_start, doc_end, Hkv);     \
-  }
-#define PB_BWD(DHV, AL, DOC)                                                                                         \
-  {                                                                                                                  \
-    if (Hkv == H) PB_BWD_G(DHV, AL, DOC, false)                                                                      \
-    else PB_BWD_G(DHV, AL, DOC, true)                                                                                \
-  }
-  if (!doc_start) {
-    if (dh == 64 && !alibi_slopes) PB_BWD(64, false, false)
-    else if (dh == 64) PB_BWD(64, true, false)
-    else if (!alibi_slopes) PB_BWD(128, false, false)
-    else PB_BWD(128, true, false)
-  } else {
-    if (dh == 64 && !alibi_slopes) PB_BWD(64, false, true)
-    else if (dh == 64) PB_BWD(64, true, true)
-    else if (!alibi_slopes) PB_BWD(128, false, true)
-    else PB_BWD(128, true, true)
-  }
-#undef PB_BWD
-#undef PB_BWD_G
+  with_bools([&](auto gqa, auto alibi, auto wide, auto doc) {
+    constexpr int DHV = wide ? 128 : 64;
+    auto kern = attn_bwd_kernel<DHV, alibi, doc, gqa>;
+    opt_in_smem(kern, BwdCfg<DHV>::SMEM);
+    kern<<<grid, 384, BwdCfg<DHV>::SMEM, st>>>(tmKV, tmQ, tmDO, lse, delta, (__nv_bfloat16*)dqkv, S, H, scale, causal ? 1 : 0, dq_acc,
+                                               alibi_slopes, doc_start, doc_end, Hkv);
+  }, Hkv != H, alibi_slopes != nullptr, dh == 128, doc_start != nullptr);
+  launched("attention bwd");
   attn_bwd_dq_convert_kernel<<<sms * 8, 256, 0, st>>>(dq_acc, (__nv_bfloat16*)dqkv, rows, d, int(w), scale);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("attention bwd launch: ") + cudaGetErrorString(e));
-  return 3;
+  launched("attention bwd dq convert");
 }
 
 void doc_bounds_launch(const long long* sequence_id, int* doc_start, int* doc_end, int B, int S, cudaStream_t st) {
   doc_bounds_kernel<<<B, DOC_THREADS, 0, st>>>(sequence_id, doc_start, doc_end, S);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("doc_bounds launch: ") + cudaGetErrorString(e));
+  launched("doc_bounds");
 }
 
 // ---------------------------------------------------------------------------------------------- RoPE
@@ -708,12 +656,10 @@ __global__ void __launch_bounds__(256) rope_kernel(__nv_bfloat16* __restrict__ q
 void rope_launch(void* qkv, const float* cosT, const float* sinT, long long T, int S, int H, int Hkv, int dh, bool inverse,
                  cudaStream_t st) {
   if (dh % 16) throw std::runtime_error("photon_b200 rope: d_head must be a multiple of 16");
-  if (Hkv < 1 || H % Hkv) throw std::runtime_error("photon_b200 rope: the kv head count must divide the head count");
   const long long n = T * (H + Hkv) * (dh / 16);
   const int blocks = int(std::min<long long>((n + 255) / 256, 132 * 16));
   rope_kernel<<<blocks, 256, 0, st>>>((__nv_bfloat16*)qkv, cosT, sinT, T, S, H, Hkv, dh, inverse ? 1 : 0);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("rope launch: ") + cudaGetErrorString(e));
+  launched("rope");
 }
 
 }  // namespace pb

@@ -11,6 +11,7 @@
 #include <cstdlib>
 #include <limits>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "comm.h"
@@ -19,13 +20,16 @@
 #include "gemm_tcgen05.h"
 #include "attention_tcgen05.h"
 #include "decode.h"
+#include "launch.h"
 
 namespace py = pybind11;
 using torch::Tensor;
 
-namespace {
-
+namespace pb {
 std::atomic<long long> g_launches{0};
+}
+
+namespace {
 
 inline cudaStream_t stream_of(const Tensor& t) { return at::cuda::getCurrentCUDAStream(t.device().index()).stream(); }
 
@@ -40,7 +44,13 @@ inline void check_f32(const Tensor& t, const char* name) {
   check_cuda(t, name);
   TORCH_CHECK(t.scalar_type() == at::kFloat, name, " must be float32");
 }
-inline const void* opt_ptr(const c10::optional<Tensor>& t) { return t.has_value() ? t->data_ptr() : nullptr; }
+template <class T = void>
+T* opt_ptr(const c10::optional<Tensor>& t) {
+  if (!t.has_value()) return nullptr;
+  if constexpr (std::is_void_v<T>) return t->data_ptr();
+  else return t->data_ptr<T>();
+}
+inline int num_sms() { return at::cuda::getCurrentDeviceProperties()->multiProcessorCount; }
 // The fused memory-bound kernels read and write rows as `bytes`-wide vectors (16: uint4 / float4, 8: four fp8 bytes as uint2):
 // the base pointer and, for a 2-D operand, the row stride must be multiples of that width. Checked before any launch, since a
 // misaligned vector access faults the device instead of raising.
@@ -60,15 +70,17 @@ inline void check_numel(const Tensor& t, int64_t n, const char* op, const char* 
   } while (0)
 
 // ---------------------------------------------------------------------------------- GEMM
-// a: [M,K] (a_mn=0) or [K,M] (a_mn=1);  b: [N,K] (b_mn=0) or [K,N] (b_mn=1);  d: [M,N]
-void gemm(const Tensor& a, const Tensor& b, Tensor& d, int a_mn, int b_mn, int epi, const c10::optional<Tensor>& bias,
-          const c10::optional<Tensor>& aux, c10::optional<Tensor> d2, bool accumulate, double alpha, int cluster) {
-  check_bf16(a, "a");
-  check_bf16(b, "b");
+// fp8 operands (1-byte tensors: torch.uint8 or float8 storage)
+inline bool is_byte(const Tensor& t) {
+  return t.scalar_type() == at::kByte || t.scalar_type() == at::kFloat8_e4m3fn || t.scalar_type() == at::kFloat8_e5m2;
+}
+// a: [M,K] (a_mn=0) or [K,M] (a_mn=1);  b: [N,K] (b_mn=0) or [K,N] (b_mn=1);  d: [M,N]. The checks and arguments gemm and
+// gemm_fp8 share; the caller checks the operand dtypes and holds the device guard.
+pb::GemmArgs gemm_args(const Tensor& a, const Tensor& b, Tensor& d, int a_mn, int b_mn, int epi, const c10::optional<Tensor>& bias,
+                       const c10::optional<Tensor>& aux, const c10::optional<Tensor>& d2, bool accumulate, double alpha, int cluster) {
   check_cuda(d, "d");
   TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && d.dim() == 2, "gemm operands must be 2-D");
   TORCH_CHECK(a.stride(1) == 1 && b.stride(1) == 1 && d.stride(1) == 1, "gemm operands must have unit inner stride");
-  c10::cuda::CUDAGuard guard(a.device());
   pb::GemmArgs g;
   g.M = int(a_mn ? a.size(1) : a.size(0));
   g.K = int(a_mn ? a.size(0) : a.size(1));
@@ -98,62 +110,33 @@ void gemm(const Tensor& a, const Tensor& b, Tensor& d, int a_mn, int b_mn, int e
     TORCH_CHECK(d2->size(0) == g.M && d2->size(1) == g.N && d2->stride(1) == 1, "d2 must be [M,N]");
     g.D2 = d2->data_ptr(), g.ldd2 = d2->stride(0);
   }
-  g.num_sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+  g.num_sms = num_sms();
   g.cluster = cluster;
-  pb::gemm_bf16_launch(g, stream_of(a));
-  g_launches += 1;
+  return g;
 }
-
-// fp8 operands (1-byte tensors: torch.uint8 or float8 storage). `meta` = float32 [3, n_roles] = (scale, scale_inv, amax) rows.
-inline bool is_byte(const Tensor& t) {
-  return t.scalar_type() == at::kByte || t.scalar_type() == at::kFloat8_e4m3fn || t.scalar_type() == at::kFloat8_e5m2;
+void gemm(const Tensor& a, const Tensor& b, Tensor& d, int a_mn, int b_mn, int epi, const c10::optional<Tensor>& bias,
+          const c10::optional<Tensor>& aux, c10::optional<Tensor> d2, bool accumulate, double alpha, int cluster) {
+  check_bf16(a, "a");
+  check_bf16(b, "b");
+  c10::cuda::CUDAGuard guard(a.device());
+  pb::gemm_launch(gemm_args(a, b, d, a_mn, b_mn, epi, bias, aux, d2, accumulate, alpha, cluster), stream_of(a));
 }
+// `meta` = float32 [3, n_roles] = (scale, scale_inv, amax) rows
 void gemm_fp8(const Tensor& a, const Tensor& b, Tensor& d, int a_mn, int b_mn, int epi, int a_fmt, int b_fmt, const Tensor& meta, int role_a,
               int role_b, const c10::optional<Tensor>& bias, const c10::optional<Tensor>& aux, c10::optional<Tensor> d2, bool accumulate,
               double alpha, int cluster, c10::optional<Tensor> d8, int role_out) {
   check_cuda(a, "a");
   check_cuda(b, "b");
-  check_cuda(d, "d");
   TORCH_CHECK(is_byte(a) && is_byte(b), "gemm_fp8 operands must be 1-byte tensors");
-  TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && d.dim() == 2, "gemm operands must be 2-D");
-  TORCH_CHECK(a.stride(1) == 1 && b.stride(1) == 1 && d.stride(1) == 1, "gemm operands must have unit inner stride");
   check_f32(meta, "meta");
   TORCH_CHECK(meta.dim() == 2 && meta.size(0) == 3 && meta.is_contiguous(), "meta must be contiguous float32 [3, n_roles]");
   const int64_t nr = meta.size(1);
   TORCH_CHECK(role_a >= 0 && role_a < nr && role_b >= 0 && role_b < nr, "role index out of range");
   c10::cuda::CUDAGuard guard(a.device());
-  pb::GemmArgs g;
+  pb::GemmArgs g = gemm_args(a, b, d, a_mn, b_mn, epi, bias, aux, d2, accumulate, alpha, cluster);
   g.fp8 = 1, g.a_fmt = a_fmt, g.b_fmt = b_fmt;
-  g.M = int(a_mn ? a.size(1) : a.size(0));
-  g.K = int(a_mn ? a.size(0) : a.size(1));
-  g.N = int(b_mn ? b.size(1) : b.size(0));
-  TORCH_CHECK((b_mn ? b.size(0) : b.size(1)) == g.K, "gemm: K mismatch between a and b");
-  TORCH_CHECK(d.size(0) == g.M && d.size(1) == g.N, "gemm: output shape mismatch");
-  g.A = a.data_ptr(), g.B = b.data_ptr(), g.D = d.data_ptr();
-  g.lda = a.stride(0), g.ldb = b.stride(0), g.ldd = d.stride(0);
-  g.a_mn = a_mn, g.b_mn = b_mn, g.epi = epi, g.accumulate = accumulate ? 1 : 0, g.alpha = float(alpha);
   const float* m = meta.data_ptr<float>();
   g.sinv_a = m + nr + role_a, g.sinv_b = m + nr + role_b;
-  if (epi == pb::EPI_F32) {
-    TORCH_CHECK(d.scalar_type() == at::kFloat, "EPI_F32 needs a float32 output");
-  } else {
-    TORCH_CHECK(d.scalar_type() == at::kBFloat16, "bf16 epilogues need a bfloat16 output");
-  }
-  if (bias.has_value()) {
-    check_f32(*bias, "bias");
-    TORCH_CHECK(bias->numel() == g.N, "bias length must equal N");
-    g.bias = bias->data_ptr<float>();
-  }
-  if (aux.has_value()) {
-    check_bf16(*aux, "aux");
-    TORCH_CHECK(aux->size(0) == g.M && aux->size(1) == g.N && aux->stride(1) == 1, "aux must be [M,N]");
-    g.aux = aux->data_ptr(), g.ld_aux = aux->stride(0);
-  }
-  if (d2.has_value()) {
-    check_bf16(*d2, "d2");
-    TORCH_CHECK(d2->size(0) == g.M && d2->size(1) == g.N && d2->stride(1) == 1, "d2 must be [M,N]");
-    g.D2 = d2->data_ptr(), g.ldd2 = d2->stride(0);
-  }
   if (d8.has_value()) {
     TORCH_CHECK(is_byte(*d8) && d8->size(0) == g.M && d8->size(1) == g.N && d8->stride(1) == 1, "d8 must be a 1-byte [M,N] tensor");
     TORCH_CHECK(role_out >= 0 && role_out < nr, "role_out out of range");
@@ -161,24 +144,19 @@ void gemm_fp8(const Tensor& a, const Tensor& b, Tensor& d, int a_mn, int b_mn, i
     g.out_scale = m + role_out;
     g.out_amax = const_cast<float*>(m) + 2 * nr + role_out;
   }
-  g.num_sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
-  g.cluster = cluster;
   // wgmma reads 8-bit operands K-major only: an MN-major operand is transposed into scratch first
   Tensor at_, bt_;
   if (a_mn) {
     at_ = torch::empty({g.M, g.K}, a.options().dtype(at::kByte));
     pb::transpose_u8(a.data_ptr(), a.stride(0), at_.data_ptr(), g.K, g.M, stream_of(a));
     g.A = at_.data_ptr(), g.lda = g.K, g.a_mn = 0;
-    g_launches += 1;
   }
   if (b_mn) {
     bt_ = torch::empty({g.N, g.K}, b.options().dtype(at::kByte));
     pb::transpose_u8(b.data_ptr(), b.stride(0), bt_.data_ptr(), g.K, g.N, stream_of(a));
     g.B = bt_.data_ptr(), g.ldb = g.K, g.b_mn = 0;
-    g_launches += 1;
   }
   pb::gemm_launch(g, stream_of(a));
-  g_launches += 1;
 }
 // block-scaled MXFP8: quantise a bf16 matrix (rows padded to `rblk` 128-row blocks in the scale array) / multiply
 std::vector<Tensor> mx_quantize(const Tensor& x, int64_t rblk) {
@@ -191,7 +169,6 @@ std::vector<Tensor> mx_quantize(const Tensor& x, int64_t rblk) {
   auto q = torch::empty({R, K}, x.options().dtype(at::kByte));
   auto sf = torch::zeros({K / 128, rblk, 512}, x.options().dtype(at::kByte));
   pb::mx_quantize(x.data_ptr(), x.stride(0), q.data_ptr(), sf.data_ptr(), R, int(K), int(rblk), stream_of(x));
-  g_launches += 1;
   return {q, sf};
 }
 void gemm_mxfp8(const Tensor& a8, const Tensor& b8, Tensor& d, const Tensor& sfa, const Tensor& sfb, const c10::optional<Tensor>& bias) {
@@ -203,10 +180,8 @@ void gemm_mxfp8(const Tensor& a8, const Tensor& b8, Tensor& d, const Tensor& sfa
   TORCH_CHECK(sfb.is_contiguous() && sfb.numel() == int64_t(K / 128) * (2 * ((N + 255) / 256)) * 512, "sfb must be [K/128][2*ceil(N/256)][512]");
   if (bias.has_value()) check_f32(*bias, "bias");
   c10::cuda::CUDAGuard guard(a8.device());
-  pb::gemm_mxfp8_launch(a8.data_ptr(), b8.data_ptr(), d.data_ptr(), sfa.data_ptr(), sfb.data_ptr(),
-                        bias.has_value() ? bias->data_ptr<float>() : nullptr, M, N, K, d.stride(0),
-                        at::cuda::getCurrentDeviceProperties()->multiProcessorCount, stream_of(a8));
-  g_launches += 1;
+  pb::gemm_mxfp8_launch(a8.data_ptr(), b8.data_ptr(), d.data_ptr(), sfa.data_ptr(), sfb.data_ptr(), opt_ptr<float>(bias), M, N, K,
+                        d.stride(0), num_sms(), stream_of(a8));
 }
 void layernorm_fwd_q8(const Tensor& x, const Tensor& gamma, const c10::optional<Tensor>& beta, Tensor& y8, Tensor& mean, Tensor& rstd,
                       double eps, Tensor& meta, int role) {
@@ -233,9 +208,8 @@ void layernorm_fwd_q8(const Tensor& x, const Tensor& gamma, const c10::optional<
   }
   c10::cuda::CUDAGuard guard(x.device());
   float* m = meta.data_ptr<float>();
-  pb::layernorm_fwd_q8(x.data_ptr(), gamma.data_ptr<float>(), beta.has_value() ? beta->data_ptr<float>() : nullptr, y8.data_ptr(),
+  pb::layernorm_fwd_q8(x.data_ptr(), gamma.data_ptr<float>(), opt_ptr<float>(beta), y8.data_ptr(),
                        mean.data_ptr<float>(), rstd.data_ptr<float>(), x.numel() / d, d, float(eps), m + role, m + 2 * nr + role, stream_of(x));
-  g_launches += 1;
 }
 // out_sum[j] += sum_t dy[t,j] and / or y8 = fp8(dy * scale[role]) with amax[role] updated — one read of dy
 void colsum_quant(const Tensor& dy, c10::optional<Tensor> out_sum, c10::optional<Tensor> y8, int fmt, c10::optional<Tensor> meta, int role) {
@@ -263,9 +237,8 @@ void colsum_quant(const Tensor& dy, c10::optional<Tensor> out_sum, c10::optional
     amax = meta->data_ptr<float>() + 2 * nr + role;
     y = y8->data_ptr(), ld8 = y8->stride(0);
   }
-  pb::colsum_quant(dy.data_ptr(), dy.stride(0), out_sum.has_value() ? out_sum->data_ptr<float>() : nullptr, y, ld8, fmt, scale, amax,
+  pb::colsum_quant(dy.data_ptr(), dy.stride(0), opt_ptr<float>(out_sum), y, ld8, fmt, scale, amax,
                    dy.size(0), int(dy.size(1)), stream_of(dy));
-  g_launches += 1;
 }
 void fp8_quantize_segments(const Tensor& src, Tensor& dst8, const Tensor& seg, Tensor& meta, int role0) {
   check_bf16(src, "src");
@@ -280,7 +253,6 @@ void fp8_quantize_segments(const Tensor& src, Tensor& dst8, const Tensor& seg, T
   float* m = meta.data_ptr<float>();
   pb::quantize_segments(src.data_ptr(), dst8.data_ptr(), reinterpret_cast<const long long*>(seg.data_ptr<int64_t>()), n, m + role0,
                         m + nr + role0, m + 2 * nr + role0, stream_of(src));
-  g_launches += 2;
 }
 void fp8_update_scales(Tensor& meta, Tensor& hist, const Tensor& fmax, Tensor& pos, int n, double margin_mult) {
   check_f32(meta, "meta");
@@ -293,10 +265,11 @@ void fp8_update_scales(Tensor& meta, Tensor& hist, const Tensor& fmax, Tensor& p
   float* m = meta.data_ptr<float>();
   pb::update_scales(m, m + nr, m + 2 * nr, hist.data_ptr<float>(), fmax.data_ptr<float>(), pos.data_ptr<int>(), n, int(hist.size(1)),
                     float(margin_mult), stream_of(meta));
-  g_launches += 1;
 }
 
 // ---------------------------------------------------------------------------------- attention
+// n_kv_heads = -1 means multi-head attention: as many kv heads as query heads
+inline int kv_heads(int n_heads, int n_kv_heads) { return n_kv_heads == -1 ? n_heads : n_kv_heads; }
 // head counts of a fused qkv row of `width` elements: H q heads, then Hkv k heads and Hkv v heads of d_head each; returns d_head
 int64_t check_qkv_heads(int64_t width, int n_heads, int n_kv_heads, const char* what) {
   TORCH_CHECK(n_heads > 0 && n_kv_heads > 0 && n_heads % n_kv_heads == 0, what, ": n_kv_heads = ", n_kv_heads,
@@ -338,16 +311,13 @@ void attention_fwd(const Tensor& qkv, Tensor& out, Tensor& lse, int n_heads, dou
   check_bf16(qkv, "qkv");
   check_bf16(out, "out");
   check_f32(lse, "lse");
-  n_kv_heads = n_kv_heads == -1 ? n_heads : n_kv_heads;   // -1: multi-head attention
+  n_kv_heads = kv_heads(n_heads, n_kv_heads);
   check_attention_args(qkv, out, lse, n_heads, n_kv_heads, causal, alibi_slopes);
   check_doc_args(qkv, causal, doc_start, c10::nullopt);
   c10::cuda::CUDAGuard guard(qkv.device());
   const int B = int(qkv.size(0)), S = int(qkv.size(1)), dh = int(qkv.size(2) / (n_heads + 2 * n_kv_heads));
   pb::attention_fwd_launch(qkv.data_ptr(), out.data_ptr(), lse.data_ptr<float>(), B, S, n_heads, n_kv_heads, dh, float(scale), causal,
-                           at::cuda::getCurrentDeviceProperties()->multiProcessorCount, stream_of(qkv),
-                           alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr,
-                           doc_start.has_value() ? doc_start->data_ptr<int>() : nullptr);
-  g_launches += 1;
+                           stream_of(qkv), opt_ptr<float>(alibi_slopes), opt_ptr<int>(doc_start));
 }
 void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, const Tensor& lse, Tensor& dqkv, Tensor& delta,
                    int n_heads, double scale, bool causal, const c10::optional<Tensor>& alibi_slopes,
@@ -358,7 +328,7 @@ void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, con
   check_bf16(dqkv, "dqkv");
   check_f32(lse, "lse");
   check_f32(delta, "delta");
-  n_kv_heads = n_kv_heads == -1 ? n_heads : n_kv_heads;   // -1: multi-head attention
+  n_kv_heads = kv_heads(n_heads, n_kv_heads);
   check_attention_args(qkv, out, lse, n_heads, n_kv_heads, causal, alibi_slopes);
   check_doc_args(qkv, causal, doc_start, doc_end);
   TORCH_CHECK(doc_start.has_value() == doc_end.has_value(), "attention_bwd: doc_start needs doc_end");
@@ -370,13 +340,9 @@ void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, con
   // the fp32 dQ accumulator comes from the caching allocator on this stream: eagerly it is recycled in stream order, under
   // CUDA-graph capture it comes from the graph's private pool and lives as long as the graph
   Tensor dq_acc = at::empty({(int64_t)B * S, d}, qkv.options().dtype(at::kFloat));
-  const int launched = pb::attention_bwd_launch(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr<float>(), dqkv.data_ptr(),
-                                                delta.data_ptr<float>(), dq_acc.data_ptr<float>(), B, S, n_heads, n_kv_heads, dh, float(scale), causal,
-                                                at::cuda::getCurrentDeviceProperties()->multiProcessorCount, stream_of(qkv),
-                                                alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr,
-                                                doc_start.has_value() ? doc_start->data_ptr<int>() : nullptr,
-                                                doc_end.has_value() ? doc_end->data_ptr<int>() : nullptr);
-  g_launches += launched;
+  pb::attention_bwd_launch(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr<float>(), dqkv.data_ptr(), delta.data_ptr<float>(),
+                           dq_acc.data_ptr<float>(), B, S, n_heads, n_kv_heads, dh, float(scale), causal, num_sms(), stream_of(qkv),
+                           opt_ptr<float>(alibi_slopes), opt_ptr<int>(doc_start), opt_ptr<int>(doc_end));
 }
 // sequence_id int64 [B,S] -> doc_start / doc_end int32 [B*S] (first / last row of each row's document)
 void doc_bounds(const Tensor& sequence_id, Tensor& doc_start, Tensor& doc_end) {
@@ -393,21 +359,19 @@ void doc_bounds(const Tensor& sequence_id, Tensor& doc_start, Tensor& doc_end) {
   if (B == 0 || S == 0) return;
   pb::doc_bounds_launch(reinterpret_cast<const long long*>(sequence_id.data_ptr<int64_t>()), doc_start.data_ptr<int>(),
                         doc_end.data_ptr<int>(), int(B), int(S), stream_of(sequence_id));
-  g_launches += 1;
 }
 void rope(Tensor& qkv, const Tensor& cos_t, const Tensor& sin_t, int n_heads, bool inverse, int n_kv_heads) {
   check_bf16(qkv, "qkv");
   check_f32(cos_t, "cos");
   check_f32(sin_t, "sin");
   TORCH_CHECK(qkv.dim() == 3 && qkv.is_contiguous(), "qkv must be contiguous [B,S,(n_heads+2*n_kv_heads)*d_head]");
-  n_kv_heads = n_kv_heads == -1 ? n_heads : n_kv_heads;   // -1: multi-head attention
+  n_kv_heads = kv_heads(n_heads, n_kv_heads);
   const int dh = int(check_qkv_heads(qkv.size(2), n_heads, n_kv_heads, "rope"));
   c10::cuda::CUDAGuard guard(qkv.device());
   const int S = int(qkv.size(1));
   TORCH_CHECK(cos_t.is_contiguous() && sin_t.is_contiguous() && cos_t.size(0) >= S && cos_t.size(1) == dh / 2, "cos/sin must be [>=S, dh/2]");
   pb::rope_launch(qkv.data_ptr(), cos_t.data_ptr<float>(), sin_t.data_ptr<float>(), (long long)qkv.size(0) * S, S, n_heads, n_kv_heads, dh, inverse,
                   stream_of(qkv));
-  g_launches += 1;
 }
 
 // ---------------------------------------------------------------------------------- decoding
@@ -415,9 +379,13 @@ inline void check_i32(const Tensor& t, const char* name) {
   check_cuda(t, name);
   TORCH_CHECK(t.scalar_type() == at::kInt && t.is_contiguous(), name, " must be contiguous int32");
 }
-inline void check_aligned16(const Tensor& t, const char* name) {
-  TORCH_CHECK((reinterpret_cast<uintptr_t>(t.data_ptr()) & 15) == 0 && (t.dim() < 2 || t.stride(0) % 8 == 0), name,
-              " must be 16-byte aligned with a row stride that is a multiple of 8 elements");
+// one layer of the k / v cache, [B_max, Hkv, S_max, dh], with Hkv the resolved n_kv_heads, which divides n_heads
+void check_kv_cache(const Tensor& kc, const Tensor& vc, int n_heads, int n_kv_heads, const char* op) {
+  check_bf16(kc, "k_cache");
+  check_bf16(vc, "v_cache");
+  TORCH_CHECK(kc.dim() == 4 && kc.is_contiguous() && vc.sizes() == kc.sizes() && vc.is_contiguous(), "k/v cache must be contiguous [B_max, Hkv, S_max, dh]");
+  TORCH_CHECK(n_heads > 0 && n_kv_heads > 0 && kc.size(1) == n_kv_heads && n_heads % n_kv_heads == 0, op,
+              ": cache heads must equal n_kv_heads and n_kv_heads divide n_heads");
 }
 // y[M,N] = epilogue(x[M,K] w[N,K]^T), 1 <= M <= 64
 void skinny_gemm(const Tensor& x, const Tensor& w, Tensor& y, const c10::optional<Tensor>& bias, const c10::optional<Tensor>& residual,
@@ -430,9 +398,9 @@ void skinny_gemm(const Tensor& x, const Tensor& w, Tensor& y, const c10::optiona
   TORCH_CHECK(x.size(1) == w.size(1), "skinny_gemm: K mismatch between x and w");
   TORCH_CHECK(y.size(0) == x.size(0) && y.size(1) == w.size(0), "skinny_gemm: output must be [M, N]");
   TORCH_CHECK(x.size(0) >= 1 && x.size(0) <= 64, "skinny_gemm: 1 <= M <= 64 rows");
-  TORCH_CHECK(x.size(1) % 8 == 0, "skinny_gemm: K must be a multiple of 8");
-  check_aligned16(x, "x");
-  check_aligned16(w, "w");
+  TORCH_CHECK(x.size(1) > 0 && x.size(1) % 8 == 0 && w.size(0) > 0, "skinny_gemm: K must be a positive multiple of 8 and N positive");
+  check_vec(x, "skinny_gemm", "x");
+  check_vec(w, "skinny_gemm", "w");
   TORCH_CHECK(epi >= pb::SKINNY_PLAIN && epi <= pb::SKINNY_GELU, "skinny_gemm: unknown epilogue");
   c10::cuda::CUDAGuard guard(x.device());
   pb::SkinnyArgs a;
@@ -452,26 +420,22 @@ void skinny_gemm(const Tensor& x, const Tensor& w, Tensor& y, const c10::optiona
                 "residual must be [M, N]");
     a.R = residual->data_ptr(), a.ldr = residual->stride(0);
   }
-  a.num_sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+  a.num_sms = num_sms();
   const int splits = pb::skinny_gemm_splits(a.M, a.N, a.K, a.num_sms);
   Tensor part;
   if (splits > 1) part = torch::empty({(long long)splits * a.M * a.N}, x.options().dtype(at::kFloat));
   pb::skinny_gemm_launch(a, splits > 1 ? part.data_ptr<float>() : nullptr, stream_of(x));
-  g_launches += splits > 1 ? 2 : 1;
 }
 // kc / vc: one layer of the cache, [B_max, Hkv, S_max, dh]; q: rows of [B, >= H*dh] (the q heads of the fused qkv)
 void decode_attention(const Tensor& q, const Tensor& kc, const Tensor& vc, const Tensor& pos, Tensor& out, int n_heads, double scale,
                       const c10::optional<Tensor>& alibi_slopes, int n_kv_heads) {
   check_bf16(q, "q");
-  check_bf16(kc, "k_cache");
-  check_bf16(vc, "v_cache");
   check_bf16(out, "out");
   check_i32(pos, "pos");
-  TORCH_CHECK(kc.dim() == 4 && kc.is_contiguous() && vc.sizes() == kc.sizes() && vc.is_contiguous(), "k/v cache must be contiguous [B_max, Hkv, S_max, dh]");
-  n_kv_heads = n_kv_heads == -1 ? n_heads : n_kv_heads;   // -1: multi-head attention
+  n_kv_heads = kv_heads(n_heads, n_kv_heads);
+  check_kv_cache(kc, vc, n_heads, n_kv_heads, "decode_attention");
   const int B = int(q.size(0)), Hkv = int(kc.size(1)), H = n_heads, S = int(kc.size(2)), dh = int(kc.size(3));
-  TORCH_CHECK(n_heads > 0 && n_kv_heads > 0 && Hkv == n_kv_heads && n_heads % n_kv_heads == 0 && (dh == 64 || dh == 128),
-              "decode_attention: cache heads must equal n_kv_heads, n_kv_heads divide n_heads and d_head be 64 or 128");
+  TORCH_CHECK(dh == 64 || dh == 128, "decode_attention: d_head must be 64 or 128");
   TORCH_CHECK(B <= kc.size(0) && pos.numel() >= B, "decode_attention: batch larger than the cache or the position vector");
   TORCH_CHECK(q.dim() == 2 && q.stride(1) == 1 && q.size(1) >= H * dh, "q must be [B, >= H*dh] with unit inner stride");
   TORCH_CHECK(out.dim() == 2 && out.size(0) == B && out.size(1) == H * dh && out.stride(1) == 1, "out must be [B, H*dh]");
@@ -484,22 +448,18 @@ void decode_attention(const Tensor& q, const Tensor& kc, const Tensor& vc, const
   Tensor po = torch::empty({(long long)B * H * splits * dh}, q.options().dtype(at::kFloat));
   Tensor pml = torch::empty({(long long)B * H * splits * 2}, q.options().dtype(at::kFloat));
   pb::decode_attention_launch(q.data_ptr(), q.stride(0), kc.data_ptr(), vc.data_ptr(), pos.data_ptr<int>(), out.data_ptr(), out.stride(0),
-                              po.data_ptr<float>(), pml.data_ptr<float>(), B, H, Hkv, dh, S, float(scale),
-                              alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr, stream_of(q));
-  g_launches += 2;
+                              po.data_ptr<float>(), pml.data_ptr<float>(), B, H, Hkv, dh, S, float(scale), opt_ptr<float>(alibi_slopes),
+                              stream_of(q));
 }
 void decode_append(Tensor& qkv, const Tensor& pos, Tensor& kc, Tensor& vc, const c10::optional<Tensor>& cos_t,
                    const c10::optional<Tensor>& sin_t, int n_heads, const c10::optional<Tensor>& slot, int n_kv_heads) {
   check_bf16(qkv, "qkv");
-  check_bf16(kc, "k_cache");
-  check_bf16(vc, "v_cache");
   check_i32(pos, "pos");
-  TORCH_CHECK(kc.dim() == 4 && kc.is_contiguous() && vc.sizes() == kc.sizes() && vc.is_contiguous(), "k/v cache must be contiguous [B_max, Hkv, S_max, dh]");
-  n_kv_heads = n_kv_heads == -1 ? n_heads : n_kv_heads;   // -1: multi-head attention
+  n_kv_heads = kv_heads(n_heads, n_kv_heads);
+  check_kv_cache(kc, vc, n_heads, n_kv_heads, "decode_append");
   const int B = int(qkv.size(0)), Hkv = int(kc.size(1)), H = n_heads, S = int(kc.size(2)), dh = int(kc.size(3));
-  TORCH_CHECK(n_heads > 0 && n_kv_heads > 0 && Hkv == n_kv_heads && n_heads % n_kv_heads == 0, "decode_append: cache heads must equal n_kv_heads and divide n_heads");
   TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == (H + 2 * Hkv) * dh && qkv.stride(1) == 1, "qkv must be [B, (n_heads+2*n_kv_heads)*d_head]");
-  check_aligned16(qkv, "qkv");
+  check_vec(qkv, "decode_append", "qkv");
   TORCH_CHECK(pos.numel() >= B, "decode_append: position vector shorter than the batch");
   if (slot.has_value()) {
     check_i32(*slot, "slot");
@@ -515,29 +475,24 @@ void decode_append(Tensor& qkv, const Tensor& pos, Tensor& kc, Tensor& vc, const
                 "cos/sin must be [>= S_max, dh/2]");
   }
   c10::cuda::CUDAGuard guard(qkv.device());
-  pb::decode_append_launch(qkv.data_ptr(), qkv.stride(0), pos.data_ptr<int>(), kc.data_ptr(), vc.data_ptr(),
-                           cos_t.has_value() ? cos_t->data_ptr<float>() : nullptr, sin_t.has_value() ? sin_t->data_ptr<float>() : nullptr,
-                           B, H, Hkv, dh, S, slot.has_value() ? slot->data_ptr<int>() : nullptr, stream_of(qkv));
-  g_launches += 1;
+  pb::decode_append_launch(qkv.data_ptr(), qkv.stride(0), pos.data_ptr<int>(), kc.data_ptr(), vc.data_ptr(), opt_ptr<float>(cos_t),
+                           opt_ptr<float>(sin_t), B, H, Hkv, dh, S, opt_ptr<int>(slot), stream_of(qkv));
 }
 // query rows of qkv [N, (H+2*Hkv)*dh] in tiles (int32 [T, 4]: slot, first_row, n_rows <= 64, first_pos) against one cache layer
 void cache_attention(const Tensor& qkv, const Tensor& kc, const Tensor& vc, const Tensor& tiles, Tensor& out, int n_heads, double scale,
                      const c10::optional<Tensor>& alibi_slopes, int n_kv_heads) {
   check_bf16(qkv, "qkv");
-  check_bf16(kc, "k_cache");
-  check_bf16(vc, "v_cache");
   check_bf16(out, "out");
   check_i32(tiles, "tiles");
-  TORCH_CHECK(kc.dim() == 4 && kc.is_contiguous() && vc.sizes() == kc.sizes() && vc.is_contiguous(), "k/v cache must be contiguous [B_max, Hkv, S_max, dh]");
-  n_kv_heads = n_kv_heads == -1 ? n_heads : n_kv_heads;   // -1: multi-head attention
+  n_kv_heads = kv_heads(n_heads, n_kv_heads);
+  check_kv_cache(kc, vc, n_heads, n_kv_heads, "cache_attention");
   const int Bm = int(kc.size(0)), Hkv = int(kc.size(1)), H = n_heads, S = int(kc.size(2)), dh = int(kc.size(3));
-  TORCH_CHECK(n_heads > 0 && n_kv_heads > 0 && Hkv == n_kv_heads && n_heads % n_kv_heads == 0 && (dh == 64 || dh == 128),
-              "cache_attention: cache heads must equal n_kv_heads, n_kv_heads divide n_heads and d_head be 64 or 128");
+  TORCH_CHECK(dh == 64 || dh == 128, "cache_attention: d_head must be 64 or 128");
   TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == (H + 2 * Hkv) * dh && qkv.stride(1) == 1,
               "qkv must be [N, (n_heads+2*n_kv_heads)*d_head] with unit inner stride");
-  check_aligned16(qkv, "qkv");
+  check_vec(qkv, "cache_attention", "qkv");
   TORCH_CHECK(out.dim() == 2 && out.size(0) == qkv.size(0) && out.size(1) == H * dh && out.stride(1) == 1, "out must be [N, H*dh]");
-  check_aligned16(out, "out");
+  check_vec(out, "cache_attention", "out");
   TORCH_CHECK(tiles.dim() == 2 && tiles.size(1) == 4, "tiles must be int32 [T, 4] (slot, first_row, n_rows, first_pos)");
   if (alibi_slopes.has_value()) {
     check_f32(*alibi_slopes, "alibi_slopes");
@@ -545,9 +500,8 @@ void cache_attention(const Tensor& qkv, const Tensor& kc, const Tensor& vc, cons
   }
   c10::cuda::CUDAGuard guard(qkv.device());
   pb::cache_attention_launch(qkv.data_ptr(), qkv.stride(0), qkv.size(0), kc.data_ptr(), vc.data_ptr(), tiles.data_ptr<int>(),
-                             int(tiles.size(0)), out.data_ptr(), out.stride(0), Bm, H, Hkv, dh, S, float(scale),
-                             alibi_slopes.has_value() ? alibi_slopes->data_ptr<float>() : nullptr, stream_of(qkv));
-  g_launches += 1;
+                             int(tiles.size(0)), out.data_ptr(), out.stride(0), Bm, H, Hkv, dh, S, float(scale), opt_ptr<float>(alibi_slopes),
+                             stream_of(qkv));
 }
 void embed_pos(const Tensor& ids, const Tensor& pos, const Tensor& wte, const c10::optional<Tensor>& wpe, Tensor& out) {
   check_i32(ids, "ids");
@@ -564,7 +518,6 @@ void embed_pos(const Tensor& ids, const Tensor& pos, const Tensor& wte, const c1
   c10::cuda::CUDAGuard guard(ids.device());
   pb::embed_pos_launch(ids.data_ptr<int>(), pos.data_ptr<int>(), wte.data_ptr(), opt_ptr(wpe), out.data_ptr(), B, d, int(wte.size(0)),
                        stream_of(ids));
-  g_launches += 1;
 }
 void argmax_advance(const Tensor& logits, Tensor& ids, c10::optional<Tensor> pos) {
   check_bf16(logits, "logits");
@@ -577,9 +530,8 @@ void argmax_advance(const Tensor& logits, Tensor& ids, c10::optional<Tensor> pos
     TORCH_CHECK(pos->numel() >= B, "pos shorter than the batch");
   }
   c10::cuda::CUDAGuard guard(logits.device());
-  pb::argmax_advance_launch(logits.data_ptr(), logits.stride(0), B, int(logits.size(1)), ids.data_ptr<int>(),
-                            pos.has_value() ? pos->data_ptr<int>() : nullptr, stream_of(logits));
-  g_launches += 1;
+  pb::argmax_advance_launch(logits.data_ptr(), logits.stride(0), B, int(logits.size(1)), ids.data_ptr<int>(), opt_ptr<int>(pos),
+                            stream_of(logits));
 }
 
 // ---------------------------------------------------------------------------------- fused ops
@@ -601,7 +553,6 @@ void embed_fwd(const Tensor& ids, const Tensor& wte, const c10::optional<Tensor>
   }
   c10::cuda::CUDAGuard guard(ids.device());
   pb::embed_fwd(ids.data_ptr<int64_t>(), wte.data_ptr(), opt_ptr(wpe), out.data_ptr(), ids.numel(), S, d, int(wte.size(0)), stream_of(ids));
-  g_launches += 1;
 }
 // dwte / dwpe: either may be None (a frozen embedding); the kernel of a missing one is not launched
 void embed_bwd(const Tensor& ids, const Tensor& dh, c10::optional<Tensor> dwte, c10::optional<Tensor> dwpe, int S) {
@@ -623,10 +574,8 @@ void embed_bwd(const Tensor& ids, const Tensor& dh, c10::optional<Tensor> dwte, 
     check_vec(*dwpe, "embed_bwd", "dwpe");
   }
   c10::cuda::CUDAGuard guard(ids.device());
-  pb::embed_bwd(ids.data_ptr<int64_t>(), dh.data_ptr(), dwte.has_value() ? dwte->data_ptr<float>() : nullptr,
-                dwpe.has_value() ? dwpe->data_ptr<float>() : nullptr, ids.numel(), S, d, dwte.has_value() ? int(dwte->size(0)) : 0,
-                stream_of(ids));
-  g_launches += int(dwte.has_value()) + int(dwpe.has_value());
+  pb::embed_bwd(ids.data_ptr<int64_t>(), dh.data_ptr(), opt_ptr<float>(dwte), opt_ptr<float>(dwpe), ids.numel(), S, d,
+                dwte.has_value() ? int(dwte->size(0)) : 0, stream_of(ids));
 }
 // dst[C,R] = src[R,C]^T for a 1-byte matrix (row stride ld): the K-major copy of an fp8 operand that is stored MN-major
 void transpose_u8(const Tensor& src, Tensor& dst) {
@@ -635,7 +584,6 @@ void transpose_u8(const Tensor& src, Tensor& dst) {
   TORCH_CHECK(dst.size(0) == src.size(1) && dst.size(1) == src.size(0), "dst must be [C,R] for src [R,C]");
   c10::cuda::CUDAGuard guard(src.device());
   pb::transpose_u8(src.data_ptr(), src.stride(0), dst.data_ptr(), int(src.size(0)), int(src.size(1)), stream_of(src));
-  g_launches += 1;
 }
 // gamma / beta: fp32 [d]; mean / rstd: fp32 [T] with T = x.numel() / d; y / dx / dres shaped like x
 void check_layernorm(const char* op, const Tensor& x, const Tensor& gamma, const c10::optional<Tensor>& beta, const Tensor& mean,
@@ -672,9 +620,8 @@ void layernorm_fwd(const Tensor& x, const Tensor& gamma, const c10::optional<Ten
   check_like_x("layernorm_fwd", y, x, "y");
   c10::cuda::CUDAGuard guard(x.device());
   const int d = int(x.size(-1));
-  pb::layernorm_fwd(x.data_ptr(), gamma.data_ptr<float>(), beta.has_value() ? beta->data_ptr<float>() : nullptr, y.data_ptr(),
+  pb::layernorm_fwd(x.data_ptr(), gamma.data_ptr<float>(), opt_ptr<float>(beta), y.data_ptr(),
                     mean.data_ptr<float>(), rstd.data_ptr<float>(), x.numel() / d, d, float(eps), stream_of(x));
-  g_launches += 1;
 }
 void layernorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& gamma, const Tensor& mean, const Tensor& rstd,
                    const c10::optional<Tensor>& dres, Tensor& dx, c10::optional<Tensor> dgamma, c10::optional<Tensor> dbeta) {
@@ -691,9 +638,7 @@ void layernorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& gamma, const
   }
   c10::cuda::CUDAGuard guard(x.device());
   pb::layernorm_bwd(dy.data_ptr(), x.data_ptr(), gamma.data_ptr<float>(), mean.data_ptr<float>(), rstd.data_ptr<float>(), opt_ptr(dres),
-                    dx.data_ptr(), dgamma.has_value() ? dgamma->data_ptr<float>() : nullptr,
-                    dbeta.has_value() ? dbeta->data_ptr<float>() : nullptr, x.numel() / d, d, stream_of(x));
-  g_launches += (dgamma.has_value() || dbeta.has_value()) ? 2 : 1;
+                    dx.data_ptr(), opt_ptr<float>(dgamma), opt_ptr<float>(dbeta), x.numel() / d, d, stream_of(x));
 }
 void col_sum(const Tensor& dy, Tensor& out) {
   check_bf16(dy, "dy");
@@ -706,7 +651,6 @@ void col_sum(const Tensor& dy, Tensor& out) {
   c10::cuda::CUDAGuard guard(dy.device());
   pb::col_reduce(dy.data_ptr(), dy.stride(0), nullptr, nullptr, nullptr, out.data_ptr<float>(), nullptr, dy.size(0), int(dy.size(1)),
                  stream_of(dy));
-  g_launches += 1;
 }
 void cross_entropy(Tensor& logits, const Tensor& targets, double grad_scale, bool write_grad, Tensor& stats,
                    c10::optional<Tensor> row_lse, const c10::optional<Tensor>& unigram_logp) {
@@ -728,9 +672,7 @@ void cross_entropy(Tensor& logits, const Tensor& targets, double grad_scale, boo
   }
   c10::cuda::CUDAGuard guard(logits.device());
   pb::cross_entropy(logits.data_ptr(), logits.stride(0), targets.data_ptr<int64_t>(), logits.size(0), int(logits.size(1)), float(grad_scale),
-                    write_grad, stats.data_ptr<double>(), row_lse.has_value() ? row_lse->data_ptr<float>() : nullptr,
-                    unigram_logp.has_value() ? unigram_logp->data_ptr<float>() : nullptr, stream_of(logits));
-  g_launches += 1;
+                    write_grad, stats.data_ptr<double>(), opt_ptr<float>(row_lse), opt_ptr<float>(unigram_logp), stream_of(logits));
 }
 // any length: the kernel reads float4s and then the last numel % 4 elements
 void flat_l2_norm(const Tensor& x, Tensor& scratch_f64, Tensor& out_f32) {
@@ -742,7 +684,6 @@ void flat_l2_norm(const Tensor& x, Tensor& scratch_f64, Tensor& out_f32) {
   CUDA_OK(cudaMemsetAsync(scratch_f64.data_ptr(), 0, sizeof(double), st));
   pb::flat_sqnorm(x.data_ptr<float>(), x.numel(), scratch_f64.data_ptr<double>(), st);
   pb::sqrt_finalize(scratch_f64.data_ptr<double>(), out_f32.data_ptr<float>(), st);
-  g_launches += 2;
 }
 void axpby(Tensor& acc, const Tensor& x, double a, double b) {
   check_f32(acc, "acc");
@@ -750,7 +691,6 @@ void axpby(Tensor& acc, const Tensor& x, double a, double b) {
   TORCH_CHECK(acc.numel() == x.numel() && acc.numel() % 4 == 0, "axpby: sizes must match and be multiples of 4");
   c10::cuda::CUDAGuard guard(acc.device());
   pb::axpby(acc.data_ptr<float>(), x.data_ptr<float>(), float(a), float(b), acc.numel(), stream_of(acc));
-  g_launches += 1;
 }
 void cast_bf16(const Tensor& src, Tensor& dst) {
   check_f32(src, "src");
@@ -758,7 +698,6 @@ void cast_bf16(const Tensor& src, Tensor& dst) {
   TORCH_CHECK(src.numel() == dst.numel() && src.numel() % 4 == 0, "cast: sizes must match and be multiples of 4");
   c10::cuda::CUDAGuard guard(src.device());
   pb::cast_fp32_to_bf16(src.data_ptr<float>(), dst.data_ptr(), src.numel(), stream_of(src));
-  g_launches += 1;
 }
 void fused_optimizer(Tensor& p, const Tensor& g, Tensor& m, Tensor& v, c10::optional<Tensor> shadow, int kind, bool first_step, double lr,
                      double beta1, double beta2, double eps, double decay, double clip, double step_size, double inv_sqrt_bc2,
@@ -789,9 +728,7 @@ void fused_optimizer(Tensor& p, const Tensor& g, Tensor& m, Tensor& v, c10::opti
   h.clip = std::isfinite(clip) ? float(clip) : std::numeric_limits<float>::infinity();
   h.step_size = float(step_size), h.inv_sqrt_bc2 = float(inv_sqrt_bc2);
   pb::fused_optimizer(p.data_ptr<float>(), g.data_ptr<float>(), kind != 2 ? m.data_ptr<float>() : nullptr, kind != 2 ? v.data_ptr<float>() : nullptr,
-                      shadow.has_value() ? shadow->data_ptr() : nullptr, p.numel(), h,
-                      grad_mult.has_value() ? grad_mult->data_ptr<float>() : nullptr, stream_of(p));
-  g_launches += 1;
+                      opt_ptr(shadow), p.numel(), h, opt_ptr<float>(grad_mult), stream_of(p));
 }
 
 // ---------------------------------------------------------------------------------- symmetric arena (CUDA IPC)
@@ -890,9 +827,7 @@ void fed_round(const std::vector<int64_t>& ctl_ptrs, int rank, int device, int64
     a.seg_bounds = reinterpret_cast<const long long*>(seg_bounds->data_ptr<int64_t>());
     a.seg_sums = seg_sums->data_ptr<double>();
   }
-  pb::fed_round_launch(a, c, uint32_t(epoch), at::cuda::getCurrentDeviceProperties()->multiProcessorCount,
-                       at::cuda::getCurrentCUDAStream(device).stream());
-  g_launches += 1;
+  pb::fed_round_launch(a, c, uint32_t(epoch), num_sms(), at::cuda::getCurrentCUDAStream(device).stream());
 }
 // ZeRO-3: accumulate the mean over ranks of slice `rank` of the unit's staging planes into `dst` (see comm.cu)
 void zero3_reduce(const std::vector<int64_t>& ctl_ptrs, int rank, int device, int64_t epoch, const std::vector<int64_t>& stage_ptrs,
@@ -910,9 +845,7 @@ void zero3_reduce(const std::vector<int64_t>& ctl_ptrs, int rank, int device, in
   a.stage_mc = reinterpret_cast<const float*>(stage_mc);
   a.per = per;
   a.scale = 1.0f / float(c.n);
-  pb::zero3_reduce_launch(a, c, uint32_t(epoch), at::cuda::getCurrentDeviceProperties()->multiProcessorCount,
-                          at::cuda::getCurrentCUDAStream(device).stream());
-  g_launches += 1;
+  pb::zero3_reduce_launch(a, c, uint32_t(epoch), num_sms(), at::cuda::getCurrentCUDAStream(device).stream());
 }
 // ZeRO-3 under amp_fp8: global amax exchange + E4M3 quantisation of this rank's pieces of every block weight matrix (see comm.cu)
 void zero3_fp8_requant(const std::vector<int64_t>& ctl_ptrs, int rank, int device, int64_t epoch, const Tensor& w16, Tensor& w8,
@@ -938,9 +871,7 @@ void zero3_fp8_requant(const std::vector<int64_t>& ctl_ptrs, int rank, int devic
   for (int i = 0; i < c.n; ++i) a.amax[i] = reinterpret_cast<float*>(amax_ptrs[i]);
   a.meta = meta.data_ptr<float>(), a.n_roles = meta.size(1), a.roles = roles.data_ptr<int>();
   a.fmax = 448.0f;
-  pb::zero3_fp8_requant_launch(a, c, uint32_t(epoch), at::cuda::getCurrentDeviceProperties()->multiProcessorCount,
-                               at::cuda::getCurrentCUDAStream(device).stream());
-  g_launches += 1;
+  pb::zero3_fp8_requant_launch(a, c, uint32_t(epoch), num_sms(), at::cuda::getCurrentCUDAStream(device).stream());
 }
 
 // device-to-device copy between (possibly peer-mapped) raw addresses on the current stream: the copy engines pull a parameter
@@ -960,9 +891,7 @@ void ddp_allreduce(const std::vector<int64_t>& ctl_ptrs, int rank, int device, i
   for (int i = 0; i < c.n; ++i) a.buf[i] = reinterpret_cast<float*>(buf_ptrs[i]);
   a.lo = lo, a.hi = hi;
   a.buf_mc = reinterpret_cast<float*>(buf_mc);
-  pb::ddp_allreduce_launch(a, c, uint32_t(epoch), out_norm.has_value() ? out_norm->data_ptr<float>() : nullptr,
-                           at::cuda::getCurrentDeviceProperties()->multiProcessorCount, at::cuda::getCurrentCUDAStream(device).stream());
-  g_launches += out_norm.has_value() ? 2 : 1;
+  pb::ddp_allreduce_launch(a, c, uint32_t(epoch), opt_ptr<float>(out_norm), num_sms(), at::cuda::getCurrentCUDAStream(device).stream());
 }
 void ddp_zero_step(const std::vector<int64_t>& ctl_ptrs, int rank, int device, int64_t epoch, const std::vector<int64_t>& grad_ptrs,
                    const std::vector<int64_t>& param_ptrs, const std::vector<int64_t>& shadow_ptrs, Tensor m, Tensor v, int64_t lo, int64_t hi,
@@ -987,19 +916,16 @@ void ddp_zero_step(const std::vector<int64_t>& ctl_ptrs, int rank, int device, i
   a.grads_mc = reinterpret_cast<const float*>(grads_mc);
   a.params_mc = reinterpret_cast<float*>(params_mc);
   a.shadow_mc = shadow_ptrs.empty() ? nullptr : reinterpret_cast<void*>(shadow_mc);
-  pb::ddp_zero_step_launch(a, c, uint32_t(epoch), out_norm.has_value() ? out_norm->data_ptr<float>() : nullptr,
-                           at::cuda::getCurrentDeviceProperties()->multiProcessorCount, at::cuda::getCurrentCUDAStream(device).stream());
-  g_launches += 1;
+  pb::ddp_zero_step_launch(a, c, uint32_t(epoch), opt_ptr<float>(out_norm), num_sms(), at::cuda::getCurrentCUDAStream(device).stream());
 }
 void set_wsum(int64_t ctl_ptr, int device, double w, bool zero_sums) {
   c10::cuda::CUDAGuard guard(static_cast<c10::DeviceIndex>(device));
   pb::set_wsum(reinterpret_cast<uint32_t*>(ctl_ptr), float(w), zero_sums, at::cuda::getCurrentCUDAStream(device).stream());
-  g_launches += 1;
 }
 
-long long launch_count() { return g_launches.load(); }
-void reset_launch_count() { g_launches = 0; }
-void add_launch_count(long long n) { g_launches += n; }  // launches replayed from a CUDA graph
+long long launch_count() { return pb::g_launches.load(); }
+void reset_launch_count() { pb::g_launches = 0; }
+void add_launch_count(long long n) { pb::g_launches += n; }  // launches replayed from a CUDA graph
 
 }  // namespace
 

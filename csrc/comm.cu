@@ -22,6 +22,7 @@
 
 #include "comm.h"
 #include "fp8_round.cuh"
+#include "launch.h"
 #include "optim_dev.cuh"
 #include "ptx.cuh"
 
@@ -638,36 +639,37 @@ int ctl_status_word_offset() { return CP_STATUS; }
 void fed_round_launch(const FedRoundArgs& a, const CommCtl& c, uint32_t epoch, int num_sms, cudaStream_t st) {
   if ((a.lo % 256) || (a.hi % 4)) throw std::runtime_error("fed_round: the shard must start on a 256-element boundary and end on a multiple of 4");
   fed_round_kernel<<<sm_count(num_sms), 512, 0, st>>>(a, c, epoch);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("fed_round launch: ") + cudaGetErrorString(e));
+  launched("fed_round");
 }
 void ddp_allreduce_launch(const AllReduceArgs& a, const CommCtl& c, uint32_t epoch, float* out_norm, int num_sms, cudaStream_t st) {
   if ((a.lo % 4) || (a.hi % 4)) throw std::runtime_error("ddp_allreduce: shard bounds must be multiples of 4");
   ddp_allreduce_kernel<<<sm_count(num_sms), 512, 0, st>>>(a, c, epoch);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("ddp_allreduce launch: ") + cudaGetErrorString(e));
-  if (out_norm) allreduce_norm_finalize_kernel<<<1, 1, 0, st>>>(c.ctl[c.rank], c.n, out_norm);
+  launched("ddp_allreduce");
+  if (out_norm) {
+    allreduce_norm_finalize_kernel<<<1, 1, 0, st>>>(c.ctl[c.rank], c.n, out_norm);
+    launched("allreduce_norm_finalize");
+  }
 }
 void ddp_zero_step_launch(const ZeroStepArgs& a, const CommCtl& c, uint32_t epoch, float* out_norm, int num_sms, cudaStream_t st) {
   if ((a.lo % 4) || (a.hi % 4)) throw std::runtime_error("ddp_zero_step: shard bounds must be multiples of 4");
   ddp_zero_step_kernel<<<sm_count(num_sms), 512, 0, st>>>(a, c, epoch, out_norm);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("ddp_zero_step launch: ") + cudaGetErrorString(e));
+  launched("ddp_zero_step");
 }
 void zero3_reduce_launch(const ShardReduceArgs& a, const CommCtl& c, uint32_t epoch, int num_sms, cudaStream_t st) {
   // a pure barrier (per == 0) needs one block; the reduction is bandwidth bound well below a full grid
   const int grid = a.per == 0 ? 1 : sm_count(num_sms);
   zero3_reduce_kernel<<<grid, 512, 0, st>>>(a, c, epoch);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("zero3_reduce launch: ") + cudaGetErrorString(e));
+  launched("zero3_reduce");
 }
 void zero3_fp8_requant_launch(const Zero3RequantArgs& a, const CommCtl& c, uint32_t epoch, int num_sms, cudaStream_t st) {
   if (a.n_w <= 0 || a.n_w > 12288) throw std::runtime_error("zero3_fp8_requant: 1..12288 weight matrices (one fp32 scale each in shared memory)");
   zero3_fp8_requant_kernel<<<sm_count(num_sms), 512, sizeof(float) * a.n_w, st>>>(a, c, epoch);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("zero3_fp8_requant launch: ") + cudaGetErrorString(e));
+  launched("zero3_fp8_requant");
 }
 
-void set_wsum(uint32_t* ctl, float w, bool zero_sums, cudaStream_t st) { set_wsum_kernel<<<1, 1, 0, st>>>(ctl, w, zero_sums ? 1 : 0); }
+void set_wsum(uint32_t* ctl, float w, bool zero_sums, cudaStream_t st) {
+  set_wsum_kernel<<<1, 1, 0, st>>>(ctl, w, zero_sums ? 1 : 0);
+  launched("set_wsum");
+}
 
 }  // namespace pb

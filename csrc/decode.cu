@@ -23,18 +23,13 @@
 
 #include "decode.h"
 #include "gemm_tcgen05.h"
+#include "launch.h"
 #include "ptx.cuh"
 #include "wgmma.cuh"
 
 namespace pb {
 
 namespace {
-
-#define PB_DECODE_CHECK(name)                                                                            \
-  do {                                                                                                   \
-    cudaError_t e__ = cudaGetLastError();                                                                \
-    if (e__ != cudaSuccess) throw std::runtime_error(std::string(name " launch: ") + cudaGetErrorString(e__)); \
-  } while (0)
 
 constexpr float LOG2E = 1.4426950408889634f;
 
@@ -173,19 +168,14 @@ __global__ void __launch_bounds__(256) skinny_reduce_kernel(const SkParams p) {
 template <int NB, int EPI>
 void skinny_launch_inst(const CUtensorMap& tw, const CUtensorMap& tx, const SkParams& p, int tiles, cudaStream_t st) {
   auto kern = skinny_gemm_kernel<NB, EPI>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, sk_smem_bytes<NB>());
-    if (e != cudaSuccess) throw std::runtime_error(std::string("skinny gemm smem attr: ") + cudaGetErrorString(e));
-    configured = true;
-  }
+  opt_in_smem(kern, sk_smem_bytes<NB>());
   kern<<<dim3(tiles, p.splits), SK_THREADS, sk_smem_bytes<NB>(), st>>>(tw, tx, p);
-  PB_DECODE_CHECK("skinny gemm");
+  launched("skinny gemm");
   if (p.splits > 1) {
     const long long total = (long long)p.M * p.N;
     const int blocks = int(std::min<long long>((total + 255) / 256, 132 * 8));
     skinny_reduce_kernel<EPI><<<blocks, 256, 0, st>>>(p);
-    PB_DECODE_CHECK("skinny gemm split reduce");
+    launched("skinny gemm split reduce");
   }
 }
 
@@ -666,8 +656,6 @@ int skinny_gemm_splits(int M, int N, int K, int num_sms) {
 }
 
 void skinny_gemm_launch(const SkinnyArgs& a, float* partials, cudaStream_t st) {
-  if (a.M < 1 || a.M > 64) throw std::runtime_error("photon_b200 skinny gemm: 1 <= M <= 64");
-  if (a.N < 1 || a.K < 1 || a.K % 8) throw std::runtime_error("photon_b200 skinny gemm: K must be a positive multiple of 8");
   const int splits = skinny_gemm_splits(a.M, a.N, a.K, a.num_sms);
   if (splits > 1 && !partials) throw std::runtime_error("photon_b200 skinny gemm: split-K needs the fp32 partial buffer");
   SkParams p{};
@@ -692,7 +680,6 @@ void decode_attention_launch(const void* q, long long ldq, const void* kc, const
                              float* partial_o, float* partial_ml, int B, int H, int Hkv, int dh, int s_max, float scale,
                              const float* alibi_slopes, cudaStream_t st) {
   if (B < 1) return;
-  if (Hkv < 1 || H % Hkv) throw std::runtime_error("photon_b200 decode attention: the kv head count must divide the head count");
   const int n_split = decode_attention_splits(s_max);
   const dim3 grid(n_split, Hkv, B);
   const int G = H / Hkv;
@@ -700,44 +687,36 @@ void decode_attention_launch(const void* q, long long ldq, const void* kc, const
   const auto* kk = (const __nv_bfloat16*)kc;
   const auto* vv = (const __nv_bfloat16*)vc;
   const float sc = scale * LOG2E;
-#define PB_DA(D, A)                                                                                                         \
-  {                                                                                                                         \
-    if (G == 1) PB_DA_NG(D, A, 1)                                                                                           \
-    else if (G == 2) PB_DA_NG(D, A, 2)                                                                                      \
-    else if (G <= 4) PB_DA_NG(D, A, 4)                                                                                      \
-    else PB_DA_NG(D, A, 8)                                                                                                  \
-    PB_DECODE_CHECK("decode attention");                                                                                    \
-    decode_combine_kernel<D><<<dim3(H, B), D, 0, st>>>(partial_o, partial_ml, pos, (__nv_bfloat16*)out, ldo, H, n_split);   \
-    PB_DECODE_CHECK("decode attention combine");                                                                            \
-    return;                                                                                                                 \
-  }
-#define PB_DA_NG(D, A, NG)                                                                                                   \
-  decode_attn_kernel<D, A, NG><<<grid, DA_THREADS, 0, st>>>(qq, ldq, kk, vv, pos, partial_o, partial_ml, H, Hkv, s_max, n_split, sc, \
-                                                           alibi_slopes);
-  if (dh == 64 && !alibi_slopes) PB_DA(64, false)
-  if (dh == 64) PB_DA(64, true)
-  if (dh == 128 && !alibi_slopes) PB_DA(128, false)
-  if (dh == 128) PB_DA(128, true)
-#undef PB_DA_NG
-#undef PB_DA
-  throw std::runtime_error("photon_b200 decode attention: d_head must be 64 or 128");
+  with_bools([&](auto alibi, auto wide) {
+    constexpr int D = wide ? 128 : 64;
+    // the G query heads of a kv head are scored NG at a time
+    const auto attn = [&](auto NG) {
+      decode_attn_kernel<D, alibi, NG><<<grid, DA_THREADS, 0, st>>>(qq, ldq, kk, vv, pos, partial_o, partial_ml, H, Hkv, s_max, n_split, sc,
+                                                                   alibi_slopes);
+    };
+    if (G == 1) attn(std::integral_constant<int, 1>{});
+    else if (G == 2) attn(std::integral_constant<int, 2>{});
+    else if (G <= 4) attn(std::integral_constant<int, 4>{});
+    else attn(std::integral_constant<int, 8>{});
+    launched("decode attention");
+    decode_combine_kernel<D><<<dim3(H, B), D, 0, st>>>(partial_o, partial_ml, pos, (__nv_bfloat16*)out, ldo, H, n_split);
+    launched("decode attention combine");
+  }, alibi_slopes != nullptr, dh == 128);
 }
 
 void decode_append_launch(void* qkv, long long ldqkv, const int* pos, void* kc, void* vc, const float* cosT, const float* sinT, int B,
                           int H, int Hkv, int dh, int s_max, const int* slot, cudaStream_t st) {
   if (B < 1) return;
   if (dh % 16) throw std::runtime_error("photon_b200 decode append: d_head must be a multiple of 16");
-  if (Hkv < 1 || H % Hkv) throw std::runtime_error("photon_b200 decode append: the kv head count must divide the head count");
   decode_append_kernel<<<B, 128, 0, st>>>((__nv_bfloat16*)qkv, ldqkv, pos, slot, (__nv_bfloat16*)kc, (__nv_bfloat16*)vc, cosT, sinT, H,
                                           Hkv, dh, s_max);
-  PB_DECODE_CHECK("decode append");
+  launched("decode append");
 }
 
 void cache_attention_launch(const void* qkv, long long ldq, long long n_q, const void* kc, const void* vc, const int* tiles, int n_tiles,
                             void* out, long long ldo, int B_max, int H, int Hkv, int dh, int s_max, float scale,
                             const float* alibi_slopes, cudaStream_t st) {
   if (n_tiles < 1 || n_q < 1) return;
-  if (Hkv < 1 || H % Hkv) throw std::runtime_error("photon_b200 cache attention: the kv head count must divide the head count");
   const long long kv_rows = (long long)B_max * Hkv * s_max;
   if (kv_rows >= (1LL << 31)) throw std::runtime_error("photon_b200 cache attention: the cache has more than 2^31 rows per layer");
   const CUtensorMap tq = make_tmap_2d(qkv, 2, false, uint64_t(H + 2 * Hkv) * dh, uint64_t(n_q), uint64_t(ldq) * 2, 64, CA_BQ);
@@ -746,38 +725,25 @@ void cache_attention_launch(const void* qkv, long long ldq, long long n_q, const
   const dim3 grid(n_tiles, H);
   const auto* tt = reinterpret_cast<const int4*>(tiles);
   const float sc = scale * LOG2E;
-#define PB_CA(D, A)                                                                                                              \
-  {                                                                                                                              \
-    auto kern = cache_attn_kernel<D, A>;                                                                                         \
-    static bool configured = false;                                                                                              \
-    if (!configured) {                                                                                                           \
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, CaCfg<D>::SMEM);                   \
-      if (e != cudaSuccess) throw std::runtime_error(std::string("cache attention smem attr: ") + cudaGetErrorString(e));       \
-      configured = true;                                                                                                         \
-    }                                                                                                                            \
-    kern<<<grid, CA_THREADS, CaCfg<D>::SMEM, st>>>(tq, tk, tv, tt, (__nv_bfloat16*)out, ldo, n_q, H, Hkv, s_max, sc,        \
-                                                   alibi_slopes);                                                               \
-    PB_DECODE_CHECK("cache attention");                                                                                          \
-    return;                                                                                                                      \
-  }
-  if (dh == 64 && !alibi_slopes) PB_CA(64, false)
-  if (dh == 64) PB_CA(64, true)
-  if (dh == 128 && !alibi_slopes) PB_CA(128, false)
-  if (dh == 128) PB_CA(128, true)
-#undef PB_CA
-  throw std::runtime_error("photon_b200 cache attention: d_head must be 64 or 128");
+  with_bools([&](auto alibi, auto wide) {
+    constexpr int D = wide ? 128 : 64;
+    auto kern = cache_attn_kernel<D, alibi>;
+    opt_in_smem(kern, CaCfg<D>::SMEM);
+    kern<<<grid, CA_THREADS, CaCfg<D>::SMEM, st>>>(tq, tk, tv, tt, (__nv_bfloat16*)out, ldo, n_q, H, Hkv, s_max, sc, alibi_slopes);
+  }, alibi_slopes != nullptr, dh == 128);
+  launched("cache attention");
 }
 
 void embed_pos_launch(const int* ids, const int* pos, const void* wte, const void* wpe, void* out, int B, int d, int V, cudaStream_t st) {
   if (B < 1) return;
   embed_pos_kernel<<<B, 128, 0, st>>>(ids, pos, (const __nv_bfloat16*)wte, (const __nv_bfloat16*)wpe, (__nv_bfloat16*)out, d, V);
-  PB_DECODE_CHECK("embed_pos");
+  launched("embed_pos");
 }
 
 void argmax_advance_launch(const void* logits, long long ldl, int B, int V, int* ids, int* pos, cudaStream_t st) {
   if (B < 1) return;
   argmax_advance_kernel<<<B, 1024, 0, st>>>((const __nv_bfloat16*)logits, ldl, V, ids, pos);
-  PB_DECODE_CHECK("argmax");
+  launched("argmax");
 }
 
 }  // namespace pb

@@ -22,6 +22,7 @@
 
 #include "fp8_ops.h"
 #include "fp8_round.cuh"
+#include "launch.h"
 #include "ptx.cuh"
 
 namespace pb {
@@ -237,27 +238,16 @@ __global__ void update_scales_kernel(float* __restrict__ scale, float* __restric
   if (threadIdx.x == 0) *pos = *pos + 1;
 }
 
-#define PB_CHECK_LAUNCH(name)                                                                          \
-  do {                                                                                                 \
-    cudaError_t e__ = cudaGetLastError();                                                              \
-    if (e__ != cudaSuccess) throw std::runtime_error(std::string(name " launch: ") + cudaGetErrorString(e__)); \
-  } while (0)
-
 }  // namespace
 
 void layernorm_fwd_q8(const void* x, const float* gamma, const float* beta, void* y8, float* mean, float* rstd, long long T, int d,
                       float eps, const float* scale, float* amax, cudaStream_t st) {
   if (d % 8 || d > 16 * 256) throw std::runtime_error("layernorm_fwd_q8: d must be a multiple of 8 and <= 4096");
-  const int nch = (d + 255) / 256;
-#define PB_LN_Q8(N)                                                                                                                     \
-  if (nch <= N) {                                                                                                                       \
-    ln_fwd_q8_kernel<N><<<int((T + 7) / 8), 256, 0, st>>>((const __nv_bfloat16*)x, gamma, beta, (uint8_t*)y8, mean, rstd, T, d, eps, scale, \
-                                                          amax);                                                                        \
-    PB_CHECK_LAUNCH("layernorm_fwd_q8");                                                                                                \
-    return;                                                                                                                             \
-  }
-  PB_LN_Q8(1) PB_LN_Q8(2) PB_LN_Q8(3) PB_LN_Q8(4) PB_LN_Q8(6) PB_LN_Q8(8) PB_LN_Q8(10) PB_LN_Q8(12) PB_LN_Q8(16)
-#undef PB_LN_Q8
+  with_ln_chunks((d + 255) / 256, [&](auto N) {
+    ln_fwd_q8_kernel<N><<<int((T + 7) / 8), 256, 0, st>>>((const __nv_bfloat16*)x, gamma, beta, (uint8_t*)y8, mean, rstd, T, d, eps, scale,
+                                                          amax);
+  });
+  launched("layernorm_fwd_q8");
 }
 
 void colsum_quant(const void* dy, long long ld, float* out_sum, void* y8, long long ld8, int fmt, const float* scale, float* amax,
@@ -272,7 +262,7 @@ void colsum_quant(const void* dy, long long ld, float* out_sum, void* y8, long l
     colsum_quant_kernel<0><<<grid, 256, 0, st>>>((const __nv_bfloat16*)dy, ld, out_sum, (uint8_t*)y8, ld8, scale, amax, T, d, rows_per);
   else
     colsum_quant_kernel<1><<<grid, 256, 0, st>>>((const __nv_bfloat16*)dy, ld, out_sum, (uint8_t*)y8, ld8, scale, amax, T, d, rows_per);
-  PB_CHECK_LAUNCH("colsum_quant");
+  launched("colsum_quant");
 }
 
 void quantize_segments(const void* src_bf16, void* dst8, const long long* seg_dev, int n_seg, float* scale, float* scale_inv, float* amax,
@@ -284,16 +274,16 @@ void quantize_segments(const void* src_bf16, void* dst8, const long long* seg_de
   if (bx < 1) bx = 1;
   if (bx > 64) bx = 64;
   seg_amax_kernel<<<dim3(bx, n_seg), 256, 0, st>>>((const __nv_bfloat16*)src_bf16, seg_dev, amax);
-  PB_CHECK_LAUNCH("seg_amax");
+  launched("seg_amax");
   seg_quant_kernel<<<dim3(bx, n_seg), 256, 0, st>>>((const __nv_bfloat16*)src_bf16, (uint8_t*)dst8, seg_dev, amax, scale, scale_inv, 448.0f);
-  PB_CHECK_LAUNCH("seg_quant");
+  launched("seg_quant");
 }
 
 void update_scales(float* scale, float* scale_inv, float* amax, float* hist, const float* fmax, int* pos, int n, int H, float margin_mult,
                    cudaStream_t st) {
   if (n <= 0) return;
   update_scales_kernel<<<1, 256, 0, st>>>(scale, scale_inv, amax, hist, fmax, pos, n, H, margin_mult);
-  PB_CHECK_LAUNCH("update_scales");
+  launched("update_scales");
 }
 
 }  // namespace pb

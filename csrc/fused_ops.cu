@@ -9,12 +9,12 @@
 #include <stdint.h>
 
 #include <algorithm>
-#include <atomic>
 #include <cstdlib>
 #include <stdexcept>
 #include <string>
 
 #include "fused_ops.h"
+#include "launch.h"
 #include "optim_dev.cuh"
 #include "ptx.cuh"
 
@@ -665,39 +665,28 @@ inline int grid_for(long long work_items, int block, int max_blocks = 132 * 8) {
 
 }  // namespace
 
-#define PB_CHECK_LAUNCH(name)                                                                          \
-  do {                                                                                                 \
-    cudaError_t e__ = cudaGetLastError();                                                              \
-    if (e__ != cudaSuccess) throw std::runtime_error(std::string(name " launch: ") + cudaGetErrorString(e__)); \
-  } while (0)
-
 void embed_fwd(const int64_t* ids, const void* wte, const void* wpe, void* out, long long T, int S, int d, int V, cudaStream_t st) {
   embed_fwd_kernel<<<grid_for(T, 1, 132 * 16), 128, 0, st>>>(ids, (const __nv_bfloat16*)wte, (const __nv_bfloat16*)wpe,
                                                             (__nv_bfloat16*)out, T, S, d, V);
-  PB_CHECK_LAUNCH("embed_fwd");
+  launched("embed_fwd");
 }
 void embed_bwd(const int64_t* ids, const void* dh, float* dwte, float* dwpe, long long T, int S, int d, int V, cudaStream_t st) {
   if (dwte) {   // null when the token embedding is frozen
     embed_bwd_wte_kernel<<<grid_for(T, 1, 132 * 16), 128, 0, st>>>(ids, (const __nv_bfloat16*)dh, dwte, T, d, V);
-    PB_CHECK_LAUNCH("embed_bwd_wte");
+    launched("embed_bwd_wte");
   }
   if (dwpe) {
     embed_bwd_wpe_kernel<<<S, 128, 0, st>>>((const __nv_bfloat16*)dh, dwpe, int(T / S), S, d);
-    PB_CHECK_LAUNCH("embed_bwd_wpe");
+    launched("embed_bwd_wpe");
   }
 }
 void layernorm_fwd(const void* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, long long T, int d,
                    float eps, cudaStream_t st) {
   if (d % 8 || d > LN_MAXCH * 256) throw std::runtime_error("layernorm: d must be a multiple of 8 and <= 4096");
-  const int nch = (d + 255) / 256;
-#define PB_LN_FWD(N)                                                                                                            \
-  if (nch <= N) {                                                                                                               \
-    ln_fwd_kernel<N><<<int((T + 7) / 8), 256, 0, st>>>((const __nv_bfloat16*)x, gamma, beta, (__nv_bfloat16*)y, mean, rstd, T, d, eps); \
-    PB_CHECK_LAUNCH("layernorm_fwd");                                                                                           \
-    return;                                                                                                                     \
-  }
-  PB_LN_FWD(1) PB_LN_FWD(2) PB_LN_FWD(3) PB_LN_FWD(4) PB_LN_FWD(6) PB_LN_FWD(8) PB_LN_FWD(10) PB_LN_FWD(12) PB_LN_FWD(16)
-#undef PB_LN_FWD
+  with_ln_chunks((d + 255) / 256, [&](auto N) {
+    ln_fwd_kernel<N><<<int((T + 7) / 8), 256, 0, st>>>((const __nv_bfloat16*)x, gamma, beta, (__nv_bfloat16*)y, mean, rstd, T, d, eps);
+  });
+  launched("layernorm_fwd");
 }
 void col_reduce(const void* dy, long long ld, const void* x, const float* mean, const float* rstd, float* out_sum, float* out_dot,
                 long long T, int d, cudaStream_t st) {
@@ -708,7 +697,7 @@ void col_reduce(const void* dy, long long ld, const void* x, const float* mean, 
   dim3 grid(col_blocks, int((T + rows_per - 1) / rows_per));
   col_reduce_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)dy, ld, (const __nv_bfloat16*)x, mean, rstd, out_sum, out_dot, T, d,
                                           rows_per);
-  PB_CHECK_LAUNCH("col_reduce");
+  launched("col_reduce");
 }
 void layernorm_bwd(const void* dy, const void* x, const float* gamma, const float* mean, const float* rstd, const void* dres, void* dx,
                    float* dgamma, float* dbeta, long long T, int d, cudaStream_t st) {
@@ -717,26 +706,18 @@ void layernorm_bwd(const void* dy, const void* x, const float* gamma, const floa
   if ((dgamma || dbeta) && nch <= 4) {
     // d <= 1024: dx and the dgamma / dbeta column sums in ONE pass over dy and x
     const int grid = int(std::min<long long>((T + 7) / 8, 132 * 2));   // 2 resident blocks per SM
-#define PB_LN_FUSED(N)                                                                                                      \
-  if (nch <= N) {                                                                                                           \
-    ln_bwd_fused_kernel<N><<<grid, 256, 0, st>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, gamma, mean, rstd,           \
-                                                 (const __nv_bfloat16*)dres, (__nv_bfloat16*)dx, dgamma, dbeta, T, d);      \
-    PB_CHECK_LAUNCH("layernorm_bwd_fused");                                                                                 \
-    return;                                                                                                                 \
+    with_ln_chunks<4>(nch, [&](auto N) {
+      ln_bwd_fused_kernel<N><<<grid, 256, 0, st>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, gamma, mean, rstd,
+                                                   (const __nv_bfloat16*)dres, (__nv_bfloat16*)dx, dgamma, dbeta, T, d);
+    });
+    launched("layernorm_bwd_fused");
+    return;
   }
-    PB_LN_FUSED(1) PB_LN_FUSED(2) PB_LN_FUSED(3) PB_LN_FUSED(4)
-#undef PB_LN_FUSED
-  }
-  bool done = false;
-#define PB_LN_BWD(N)                                                                                                  \
-  if (!done && nch <= N) {                                                                                            \
-    ln_bwd_dx_kernel<N><<<int((T + 7) / 8), 256, 0, st>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, gamma, mean, rstd, \
-                                                          (const __nv_bfloat16*)dres, (__nv_bfloat16*)dx, T, d);      \
-    done = true;                                                                                                      \
-  }
-  PB_LN_BWD(1) PB_LN_BWD(2) PB_LN_BWD(3) PB_LN_BWD(4) PB_LN_BWD(6) PB_LN_BWD(8) PB_LN_BWD(10) PB_LN_BWD(12) PB_LN_BWD(16)
-#undef PB_LN_BWD
-  PB_CHECK_LAUNCH("layernorm_bwd_dx");
+  with_ln_chunks(nch, [&](auto N) {
+    ln_bwd_dx_kernel<N><<<int((T + 7) / 8), 256, 0, st>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, gamma, mean, rstd,
+                                                          (const __nv_bfloat16*)dres, (__nv_bfloat16*)dx, T, d);
+  });
+  launched("layernorm_bwd_dx");
   if (dgamma || dbeta) col_reduce(dy, d, x, mean, rstd, dbeta, dgamma, T, d, st);
 }
 void cross_entropy(void* logits, long long ld, const int64_t* targets, long long rows, int V, float grad_scale, bool write_grad,
@@ -748,46 +729,36 @@ void cross_entropy(void* logits, long long ld, const int64_t* targets, long long
   // that is a multiple of 8. ce_kernel (two reads of the row from HBM) therefore runs only for rows over 200 KiB (V > 102400)
   // or under PB_CE_SMEM=0.
   if (smem_path && row_bytes <= 200 * 1024) {
-    // the row lives in shared memory between the two passes: one HBM read of the logits instead of two. The opt-in to more
-    // than 48 KiB of dynamic shared memory is a per-device attribute of the kernel, so it is set once on each device.
-    static std::atomic<bool> configured[64];
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess || dev < 0 || dev >= 64) throw std::runtime_error("cross_entropy: no usable current device");
-    if (!configured[dev].load()) {
-      e = cudaFuncSetAttribute(ce_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-      if (e != cudaSuccess) throw std::runtime_error(std::string("cross_entropy smem attr: ") + cudaGetErrorString(e));
-      configured[dev].store(true);
-    }
+    // the row lives in shared memory between the two passes: one HBM read of the logits instead of two
+    opt_in_smem(ce_smem_kernel, 200 * 1024);
     ce_smem_kernel<<<int(rows), 512, row_bytes, st>>>((__nv_bfloat16*)logits, ld, targets, V, grad_scale, write_grad ? 1 : 0, stats, row_lse,
                                                       unigram_logp);
-    PB_CHECK_LAUNCH("cross_entropy");
-    return;
+  } else {
+    ce_kernel<<<int(rows), 256, 0, st>>>((__nv_bfloat16*)logits, ld, targets, V, grad_scale, write_grad ? 1 : 0, stats, row_lse,
+                                         unigram_logp);
   }
-  ce_kernel<<<int(rows), 256, 0, st>>>((__nv_bfloat16*)logits, ld, targets, V, grad_scale, write_grad ? 1 : 0, stats, row_lse,
-                                       unigram_logp);
-  PB_CHECK_LAUNCH("cross_entropy");
+  launched("cross_entropy");
 }
 void flat_sqnorm(const float* x, long long n, double* out_accum, cudaStream_t st) {
   sqnorm_kernel<<<grid_for(n / 4, 256, 132 * 4), 256, 0, st>>>(x, n, out_accum);
-  PB_CHECK_LAUNCH("flat_sqnorm");
+  launched("flat_sqnorm");
 }
 void sqrt_finalize(const double* in, float* out, cudaStream_t st) {
   sqrt_finalize_kernel<<<1, 1, 0, st>>>(in, out);
-  PB_CHECK_LAUNCH("sqrt_finalize");
+  launched("sqrt_finalize");
 }
 void axpby(float* acc, const float* x, float a, float b, long long n, cudaStream_t st) {
   axpby_kernel<<<grid_for(n / 4, 256, 132 * 8), 256, 0, st>>>(acc, x, a, b, n / 4);
-  PB_CHECK_LAUNCH("axpby");
+  launched("axpby");
 }
 void cast_fp32_to_bf16(const float* src, void* dst, long long n, cudaStream_t st) {
   cast_bf16_kernel<<<grid_for(n / 4, 256, 132 * 8), 256, 0, st>>>(src, (__nv_bfloat16*)dst, n / 4);
-  PB_CHECK_LAUNCH("cast_bf16");
+  launched("cast_bf16");
 }
 void fused_optimizer(float* p, const float* g, float* m, float* v, void* shadow, long long n, const OptimHyper& h,
                      const float* grad_mult, cudaStream_t st) {
   optim_kernel<<<grid_for(n / 4, 256, 132 * 8), 256, 0, st>>>(p, g, m, v, (__nv_bfloat16*)shadow, n / 4, h, grad_mult);
-  PB_CHECK_LAUNCH("fused_optimizer");
+  launched("fused_optimizer");
 }
 
 }  // namespace pb

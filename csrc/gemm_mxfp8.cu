@@ -20,6 +20,7 @@
 #include <string>
 
 #include "gemm_tcgen05.h"
+#include "launch.h"
 #include "ptx.cuh"
 #include "wgmma.cuh"
 
@@ -212,8 +213,7 @@ void mx_quantize(const void* x_bf16, long long ld, void* q8, void* sf, long long
   long long blocks = (groups + 255) / 256;
   if (blocks > 132 * 16) blocks = 132 * 16;
   mx_quantize_kernel<<<int(blocks), 256, 0, st>>>((const __nv_bfloat16*)x_bf16, ld, (uint8_t*)q8, (uint8_t*)sf, R, K, rblk);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("mx_quantize launch: ") + cudaGetErrorString(e));
+  launched("mx_quantize");
 }
 
 void gemm_mxfp8_launch(const void* A, const void* B, void* D, const void* sfa, const void* sfb, const float* bias, int M, int N, int K,
@@ -227,17 +227,11 @@ void gemm_mxfp8_launch(const void* A, const void* B, void* D, const void* sfa, c
   p.mblk128 = p.tiles_m, p.nblk128 = 2 * ((N + 255) / 256);
   p.sfa = reinterpret_cast<const uint8_t*>(sfa), p.sfb = reinterpret_cast<const uint8_t*>(sfb), p.bias = bias;
   p.d = reinterpret_cast<__nv_bfloat16*>(D), p.ldd = ldd;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_mx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e != cudaSuccess) throw std::runtime_error(std::string("gemm_mxfp8 smem attr: ") + cudaGetErrorString(e));
-    configured = true;
-  }
+  opt_in_smem(gemm_mx_kernel, SMEM_BYTES);
   int sms = num_sms > 0 ? num_sms : 132;
   const int tiles = p.tiles_m * p.tiles_n;
   gemm_mx_kernel<<<tiles < sms ? tiles : sms, NUM_THREADS, SMEM_BYTES, stream>>>(ta, tb, p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("gemm_mxfp8 launch: ") + cudaGetErrorString(e));
+  launched("gemm_mxfp8");
 }
 
 }  // namespace pb

@@ -21,6 +21,7 @@
 #include <string>
 
 #include "gemm_tcgen05.h"
+#include "launch.h"
 #include "ptx.cuh"
 #include "wgmma.cuh"
 
@@ -462,12 +463,7 @@ template <int A_MN, int B_MN, int EPI, int CL, int F8>
 static void launch_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& td, const CUtensorMap& td2, const Params& p, int grid,
                       cudaStream_t stream) {
   auto kern = gemm_kernel<A_MN, B_MN, EPI, CL, F8>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e != cudaSuccess) throw std::runtime_error(std::string("gemm smem attr: ") + cudaGetErrorString(e));
-    configured = true;
-  }
+  opt_in_smem(kern, SMEM_BYTES);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(NUM_THREADS);
@@ -480,8 +476,8 @@ static void launch_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CUtens
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, td, td2, p);
-  if (e != cudaSuccess) throw std::runtime_error(std::string("gemm launch: ") + cudaGetErrorString(e));
+  cudaLaunchKernelEx(&cfg, kern, ta, tb, td, td2, p);
+  launched("gemm");
 }
 
 template <int A_MN, int B_MN, int EPI, int F8>
@@ -497,8 +493,7 @@ void transpose_u8(const void* src, long long ld, void* dst, int R, int C, cudaSt
     transpose_u8_v16_kernel<<<grid, 256, 0, stream>>>((const uint8_t*)src, ld, (uint8_t*)dst, R);
   else
     transpose_u8_kernel<<<grid, 256, 0, stream>>>((const uint8_t*)src, ld, (uint8_t*)dst, R, C);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("transpose_u8 launch: ") + cudaGetErrorString(e));
+  launched("transpose_u8");
 }
 
 // Operands are bf16 or, with g.fp8, 8-bit floats (E4M3 / E5M2 chosen per operand, fp32 accumulate, per-tensor de-scales
@@ -604,7 +599,5 @@ void gemm_launch(const GemmArgs& g, cudaStream_t stream) {
 #undef PB_CASE
   throw std::runtime_error("photon_b200 gemm: unsupported (a_major, b_major, epilogue, operand type) combination");
 }
-
-void gemm_bf16_launch(const GemmArgs& g, cudaStream_t stream) { gemm_launch(g, stream); }
 
 }  // namespace pb

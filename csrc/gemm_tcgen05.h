@@ -45,7 +45,6 @@ struct GemmArgs {
 };
 
 void gemm_launch(const GemmArgs& g, cudaStream_t stream);
-void gemm_bf16_launch(const GemmArgs& g, cudaStream_t stream);   // same entry (kept for callers that predate fp8)
 // [R, C] bytes (row stride ld) -> [C, R] contiguous: an MN-major fp8 operand made K-major
 void transpose_u8(const void* src, long long ld, void* dst, int R, int C, cudaStream_t stream);
 
