@@ -11,11 +11,12 @@
 //                 (the S accumulator layout converts to the A fragment layout in place) and V consumed MN-major as stored.
 //
 // Backward (attn_bwd_kernel<DH>): one CTA = one (batch, kv head, 128-key tile) holding K_j, V_j in shared memory; warpgroups 1, 2
-// own 64 key rows each and walk the 64-row query tiles i (causal: those that see the key tile) of each of the G query heads
-// of the group in turn, so dK / dV of the whole group accumulate in registers (no atomics): S^T = K Q^T and dP^T = V dO^T
-// (shared-memory operands), P^T and dS^T in registers, dV += P^T dO and dK += dS^T Q with the register A operand; dS^T is also
-// staged in shared memory, where it reads as an MN-major dS for dQ = dS K (each warpgroup one half of the head dimension);
-// dQ partial tiles leave through fp32 red.global.add into an accumulator that a last kernel converts to bf16.
+// own 64 key rows each and walk the query steps (128 rows at d_head 64, 64 at d_head 128; causal: those that see the key
+// tile) of each of the G query heads of the group in turn, so dK / dV of the whole group accumulate in registers (no
+// atomics). The producer brings each step's Q, dO and their lse / delta rows. S^T = K Q^T and dP^T = V dO^T (shared-memory
+// operands), P^T and dS^T in registers, dV += P^T dO and dK += dS^T Q with the register A operand; dS^T is also written to a
+// double-buffered shared-memory tile, where it reads as an MN-major dS for dQ = dS K (each warpgroup one 64 x 64 block); each
+// warp's dQ rows leave through shared memory and a TMA reduce-add into an fp32 accumulator that a last kernel converts to bf16.
 //
 // Replaces flash-attn 2.x (mma.sync/cp.async) the reference calls through llm-foundry (SURVEY §2.5 K4).
 #include <cuda.h>
@@ -289,13 +290,19 @@ __global__ void attn_bwd_dq_convert_kernel(const float* __restrict__ dq_acc, __n
   }
 }
 
+// d_head 64 walks 128-query steps: S^T and dP^T are m64n128 (64 + 64 fp32 per thread) next to dV and dK (32 + 32), inside the
+// 240-register consumer budget (setmaxnreg 240 / 24). d_head 128 doubles dV and dK, so it keeps 64-query steps.
 template <int DH>
 struct BwdCfg {
   static constexpr int CH = DH / 64;                        // 64-column swizzle chunks per tile
+  static constexpr int BQS = DH == 64 ? 128 : 64;           // query rows per step
   static constexpr int KT = 128 * 128 * CH;                 // [128 x DH] bf16 (K, V)
-  static constexpr int QT = 64 * 128 * CH;                  // [64 x DH] bf16 (Q, dO)
-  static constexpr int DS = 128 * 128;                      // dS^T: [128 keys][64 queries] bf16
-  static constexpr int SMEM = 2 * KT + 4 * QT + DS + 256 + 1024;
+  static constexpr int QC = BQS * 128;                      // one 64-column chunk of a [BQS x DH] bf16 tile (Q, dO)
+  static constexpr int QT = QC * CH;
+  static constexpr int DS = 128 * BQS * 2;                  // dS^T: [128 keys][BQS queries] bf16, 64 queries per swizzle chunk
+  static constexpr int DQW = 16 * 64 * 4;                   // one consumer warp's dQ staging: [16 rows][64 columns] fp32
+  static constexpr int RS = 3 * BQS * 4;                    // the step's lse, delta (fp32) and doc_start (int) rows
+  static constexpr int SMEM = 2 * KT + 4 * QT + 2 * DS + 8 * DQW + 2 * RS + 256 + 1024;
   static_assert(SMEM <= 232448, "smem budget");
 };
 
@@ -305,25 +312,35 @@ __device__ __forceinline__ void wgmma_acc_rs(float (&d)[DH / 2], const uint32_t 
   else wgmma_bf16_rs_n128<1>(d, a, db, 1u);
 }
 
+// S^T / dP^T of one step: [64 keys x N queries], both operands K-major
+template <int N>
+__device__ __forceinline__ void wgmma_ss_kmajor(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
+  if constexpr (N == 128) wgmma_bf16_ss_n128<0, 0>(d, da, db, scale_d);
+  else wgmma_bf16_ss_n64<0, 0>(d, da, db, scale_d);
+}
+
 // DOC: as in the forward; doc_end [B*S] holds the last row of each row's document, so the query walk of a key tile stops at
-// the 64-row tile holding the end of its last key's document. GQA: as in the forward.
+// the step holding the end of its last key's document. GQA: as in the forward.
 template <int DH, bool ALIBI, bool DOC, bool GQA>
 __global__ void __launch_bounds__(384, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
-                const float* __restrict__ lse, const float* __restrict__ delta, __nv_bfloat16* __restrict__ dqkv, int S, int H, float scale,
-                int causal, float* __restrict__ dq_acc, const float* __restrict__ alibi_slopes, const int* __restrict__ doc_start,
-                const int* __restrict__ doc_end, int HKV) {
+                const __grid_constant__ CUtensorMap tmDQ, const float* __restrict__ lse, const float* __restrict__ delta,
+                __nv_bfloat16* __restrict__ dqkv, int S, int H, float scale, int causal, const float* __restrict__ alibi_slopes,
+                const int* __restrict__ doc_start, const int* __restrict__ doc_end, int HKV) {
   using C = BwdCfg<DH>;
+  constexpr int BQS = C::BQS;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sK = smem;
   uint8_t* sV = sK + C::KT;
   uint8_t* sQ = sV + C::KT;              // [2]
   uint8_t* sDO = sQ + 2 * C::QT;         // [2]
-  uint8_t* sDS = sDO + 2 * C::QT;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sDS + C::DS);
+  uint8_t* sDS = sDO + 2 * C::QT;        // [2]
+  uint8_t* sDQ = sDS + 2 * C::DS;        // [8 consumer warps]
+  uint8_t* sRS = sDQ + 8 * C::DQW;       // [2] lse, delta, doc_start of the Q / dO stage's rows
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sRS + 2 * C::RS);
   uint64_t* kv_full = bars;
-  uint64_t* q_full = bars + 1;           // [2] Q_i + dO_i
+  uint64_t* q_full = bars + 1;           // [2] Q_i + dO_i + their row statistics
   uint64_t* q_empty = bars + 3;          // [2]
 
   const int jt = int(gridDim.x) - 1 - int(blockIdx.x);   // causal: small key tiles see the most query tiles - start them first
@@ -332,8 +349,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
   const int G = GQA ? H / hkv : 1, h0 = hk * G;           // query heads h0 .. h0 + G - 1 read this kv head
   const int d_model = H * DH;
   const int k_col = d_model + hk * DH, v_col = GQA ? k_col + HKV * DH : 2 * d_model + hk * DH;
-  const int i0 = causal ? jt * 2 : 0;                      // 64-row query tiles
-  const int n_q = DOC ? doc_end[b * S + jt * 128 + 127] / 64 + 1 : S / 64;
+  const int i0 = causal ? jt * (128 / BQS) : 0;            // query steps of BQS rows
+  const int n_q = DOC ? doc_end[b * S + jt * 128 + 127] / BQS + 1 : S / BQS;
   const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
 
@@ -341,6 +358,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
     prefetch_tmap(&tmKV);
     prefetch_tmap(&tmQ);
     prefetch_tmap(&tmDO);
+    prefetch_tmap(&tmDQ);
     mbar_init(kv_full, 1);
     for (int s2 = 0; s2 < 2; ++s2) {
       mbar_init(&q_full[s2], 1);
@@ -351,7 +369,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
   __syncthreads();
 
   if (wg == 0) {
-    regs_dealloc<40>();
+    regs_dealloc<24>();
     if (threadIdx.x == 0) {
       mbar_expect_tx(kv_full, 2 * C::KT);
 #pragma unroll
@@ -361,73 +379,76 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
       }
       for (int h = h0; h < h0 + G; ++h) {
         for (int i = i0; i < n_q; ++i) {
-          const int n = (h - h0) * (n_q - i0) + i - i0, st = n & 1;   // (query head, query tile) items in walk order
+          const int n = (h - h0) * (n_q - i0) + i - i0, st = n & 1;   // (query head, query step) items in walk order
           mbar_wait(&q_empty[st], ((n >> 1) & 1) ^ 1);
-          mbar_expect_tx(&q_full[st], 2 * C::QT);
+          mbar_expect_tx(&q_full[st], 2 * C::QT + (DOC ? 3 : 2) * BQS * 4);
 #pragma unroll
           for (int c = 0; c < C::CH; ++c) {
-            tma_load_2d(sQ + st * C::QT + c * 8192, &tmQ, &q_full[st], h * DH + c * 64, b * S + i * 64);
-            tma_load_2d(sDO + st * C::QT + c * 8192, &tmDO, &q_full[st], h * DH + c * 64, b * S + i * 64);
+            tma_load_2d(sQ + st * C::QT + c * C::QC, &tmQ, &q_full[st], h * DH + c * 64, b * S + i * BQS);
+            tma_load_2d(sDO + st * C::QT + c * C::QC, &tmDO, &q_full[st], h * DH + c * 64, b * S + i * BQS);
           }
+          const long long row = ((long long)b * H + h) * S + i * BQS;
+          uint8_t* rs_st = sRS + st * C::RS;
+          bulk_load(rs_st, lse + row, BQS * 4, &q_full[st]);
+          bulk_load(rs_st + BQS * 4, delta + row, BQS * 4, &q_full[st]);
+          if (DOC) bulk_load(rs_st + 2 * BQS * 4, doc_start + (long long)b * S + i * BQS, BQS * 4, &q_full[st]);
         }
       }
     }
     return;
   }
-  regs_alloc<232>();
+  regs_alloc<240>();
   const int cw = wg - 1;
   const int wq = (threadIdx.x >> 5) & 3;
   const int g = lane >> 2, t4 = lane & 3;
   const int kl0 = cw * 64 + wq * 16 + g;          // this thread's key rows inside the tile: kl0, kl0 + 8
   const int key0 = jt * 128 + kl0;
   const float sc = scale * LOG2E;
-  // the multi-head instances read their head's row statistics here, where the multi-head kernel always has
+  // the multi-head instances read their head's slope here, where the multi-head kernel always has
   const float slope2_mh = ALIBI && !GQA ? alibi_slopes[h0] * LOG2E : 0.f;
-  const float* lse_mh = lse + (long long)bk * S;
-  const float* delta_mh = delta + (long long)bk * S;
-  const int* dstart_b = DOC ? doc_start + (long long)b * S : nullptr;
   float dv[DH / 2], dk[DH / 2];
 #pragma unroll
   for (int i = 0; i < DH / 2; ++i) dv[i] = 0.f, dk[i] = 0.f;
   mbar_wait(kv_full, 0);
-  // the query tiles of query head h; n0: the walk position of its first tile (the group's heads come one after the other)
-  auto walk = [&](const int h, const int n0) {
+  // the query steps of each query head of the group in turn (one head for the multi-head instances)
+  for (int h = h0; h < h0 + G; ++h) {
     const float slope2 = !GQA ? slope2_mh : ALIBI ? alibi_slopes[h] * LOG2E : 0.f;
-    const float* lse_bh = GQA ? lse + ((long long)b * H + h) * S : lse_mh;
-    const float* delta_bh = GQA ? delta + ((long long)b * H + h) * S : delta_mh;
     for (int i = i0; i < n_q; ++i) {
-      const int n = n0 + i - i0, st = n & 1;
-      const int q0 = i * 64;
+      const int n = (h - h0) * (n_q - i0) + i - i0, st = n & 1;   // walk position, as in the producer
+      const int q0 = i * BQS;
       uint8_t* q_st = sQ + st * C::QT;
       uint8_t* do_st = sDO + st * C::QT;
-      float s[32], dp[32];
+      uint8_t* ds_st = sDS + st * C::DS;
+      float s[BQS / 2], dp[BQS / 2];
       mbar_wait(&q_full[st], (n >> 1) & 1);
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < DH / 16; ++kk) {   // S^T = K Q^T
         const int c = kk >> 2, off = (kk & 3) * 32;
-        wgmma_bf16_ss_n64<0, 0>(s, desc_add(desc_sw128(sK + c * 16384 + cw * 8192, 16), off), desc_add(desc_sw128(q_st + c * 8192, 16), off),
-                                kk > 0 ? 1u : 0u);
+        wgmma_ss_kmajor<BQS>(s, desc_add(desc_sw128(sK + c * 16384 + cw * 8192, 16), off), desc_add(desc_sw128(q_st + c * C::QC, 16), off),
+                             kk > 0 ? 1u : 0u);
       }
 #pragma unroll
       for (int kk = 0; kk < DH / 16; ++kk) {   // dP^T = V dO^T
         const int c = kk >> 2, off = (kk & 3) * 32;
-        wgmma_bf16_ss_n64<0, 0>(dp, desc_add(desc_sw128(sV + c * 16384 + cw * 8192, 16), off), desc_add(desc_sw128(do_st + c * 8192, 16), off),
-                                kk > 0 ? 1u : 0u);
+        wgmma_ss_kmajor<BQS>(dp, desc_add(desc_sw128(sV + c * 16384 + cw * 8192, 16), off), desc_add(desc_sw128(do_st + c * C::QC, 16), off),
+                             kk > 0 ? 1u : 0u);
       }
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_fence_regs(s);
       wgmma_fence_regs(dp);
-      // P^T = exp(S^T * scale + alibi - lse[q]) (masked where query < key), dS^T = P^T * (dP^T - delta[q])
-      uint32_t pa[4][4], da[4][4];
+      // P^T = exp(S^T * scale + alibi - lse[q]) (masked where query < key, which only the step overlapping the key tile has),
+      // dS^T = P^T * (dP^T - delta[q])
+      const bool diag = causal && i < i0 + 128 / BQS;   // the steps that overlap the key tile
+      const uint32_t rs = smem_u32(sRS + st * C::RS) + 8 * t4;   // this thread's query columns in the staged rows
+      uint32_t pa[BQS / 16][4], da[BQS / 16][4];
 #pragma unroll
-      for (int j8 = 0; j8 < 8; ++j8) {
+      for (int j8 = 0; j8 < BQS / 8; ++j8) {
         const int qa = q0 + 8 * j8 + 2 * t4;
-        const float2 L = *reinterpret_cast<const float2*>(lse_bh + qa);
-        const float2 D = *reinterpret_cast<const float2*>(delta_bh + qa);
-        int2 DS = make_int2(0, 0);
-        if (DOC) DS = *reinterpret_cast<const int2*>(dstart_b + qa);   // through L1, like lse / delta
+        const float2 L = ld_shared_f32x2(rs + 32 * j8);
+        const float2 D = ld_shared_f32x2(rs + BQS * 4 + 32 * j8);
+        const int2 DS = DOC ? ld_shared_s32x2(rs + 2 * BQS * 4 + 32 * j8) : make_int2(0, 0);
         float pv[4], dsv[4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
@@ -435,7 +456,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
           float x = fmaf(s[4 * j8 + e], sc, -((e & 1) ? L.y : L.x) * LOG2E);
           if (ALIBI) x = fmaf(slope2, float(key - q), x);
           float pr = exp2f(x);
-          if (causal && q < key) pr = 0.f;
+          if (diag && q < key) pr = 0.f;
           if (DOC && ((e & 1) ? DS.y : DS.x) > key) pr = 0.f;
           pv[e] = pr;
           dsv[e] = pr * (dp[4 * j8 + e] - ((e & 1) ? D.y : D.x));
@@ -451,55 +472,66 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
       }
       wgmma_fence();
 #pragma unroll
-      for (int kc = 0; kc < 4; ++kc) {   // dV += P^T dO, dK += dS^T Q (B operands MN-major: 16 query rows per k-step)
-        wgmma_acc_rs<DH>(dv, pa[kc], desc_add(desc_sw128(do_st, 8192), kc * 2048));
-        wgmma_acc_rs<DH>(dk, da[kc], desc_add(desc_sw128(q_st, 8192), kc * 2048));
+      for (int kc = 0; kc < BQS / 16; ++kc) {   // dV += P^T dO, dK += dS^T Q (B operands MN-major: 16 query rows per k-step)
+        wgmma_acc_rs<DH>(dv, pa[kc], desc_add(desc_sw128(do_st, C::QC), kc * 2048));
+        wgmma_acc_rs<DH>(dk, da[kc], desc_add(desc_sw128(q_st, C::QC), kc * 2048));
       }
       wgmma_commit();
-      // dS^T -> shared memory (row = key, 64 queries = 128 bytes, 128-byte swizzle); both warpgroups' previous dQ MMAs are done
-      named_bar_sync(1, 256);
+      // dS^T -> this step's buffer (row = key, 64 queries = 128 bytes per chunk, 128-byte swizzle)
 #pragma unroll
-      for (int j8 = 0; j8 < 8; ++j8) {
+      for (int j8 = 0; j8 < BQS / 8; ++j8) {
         const int kc = j8 >> 1, hi = (j8 & 1) * 2;
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
           const int kl = kl0 + 8 * hh;
-          *reinterpret_cast<uint32_t*>(sDS + kl * 128 + ((j8 ^ (kl & 7)) << 4) + 4 * t4) = da[kc][hi + hh];
+          *reinterpret_cast<uint32_t*>(ds_st + (j8 >> 3) * 16384 + kl * 128 + (((j8 & 7) ^ (kl & 7)) << 4) + 4 * t4) = da[kc][hi + hh];
         }
       }
       fence_proxy_async_smem();
+      // the dQ MMAs read both warpgroups' key rows of dS^T. The buffer was last read by the dQ MMAs two steps back, which each
+      // warpgroup waited for before it reached the previous step's barrier, so this is the step's only cross-warpgroup barrier.
       named_bar_sync(1, 256);
-      // dQ[64 queries, this warpgroup's half of the head] = dS K: A = dS (MN-major: queries contiguous), B = K (MN-major)
-      float dq[DH / 4];
+      // dQ = dS K for this warpgroup's 64 x 64 block: A = dS (MN-major: queries contiguous), B = K (MN-major)
+      float dq[32];
       wgmma_fence();
 #pragma unroll
       for (int kc = 0; kc < 8; ++kc) {
-        const uint64_t ad = desc_add(desc_sw128(sDS, 16384), kc * 2048);
-        if constexpr (DH == 128) {
-          wgmma_bf16_ss_n64<1, 1>(dq, ad, desc_add(desc_sw128(sK + cw * 16384, 16384), kc * 2048), kc > 0 ? 1u : 0u);
-        } else {
-          wgmma_bf16_ss_n32<1, 1>(dq, ad, desc_add(desc_sw128(sK + cw * 64, 16384), kc * 2048), kc > 0 ? 1u : 0u);
-        }
+        wgmma_bf16_ss_n64<1, 1>(dq, desc_add(desc_sw128(ds_st + (DH == 64 ? cw * 16384 : 0), 16384), kc * 2048),
+                                desc_add(desc_sw128(sK + (DH == 128 ? cw * 16384 : 0), 16384), kc * 2048), kc > 0 ? 1u : 0u);
       }
       wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(dq);
+      wgmma_wait<1>();   // dV and dK are done with the Q / dO stage
       wgmma_fence_regs(dv);
       wgmma_fence_regs(dk);
       __syncwarp();
       if (lane == 0) mbar_arrive(&q_empty[st]);
+      wgmma_wait<0>();
+      wgmma_fence_regs(dq);
+      // dQ -> this warp's staging -> one bulk reduce-add per 32-column box into dq_acc; only the staging's previous read by
+      // the bulk copy is waited for, not its global write. The warp's tile is 16 rows of the warpgroup's 64 x 64 block (d_head
+      // 64: its 64 queries of the step; d_head 128: its half of the head dimension), staged as two [16 rows][32 fp32] boxes in
+      // the 128-byte swizzle of the reduce-add tensor map.
+      uint8_t* sDQw = sDQ + (cw * 4 + wq) * C::DQW;
+      if (lane == 0) tma_wait_read<0>();
+      __syncwarp();
 #pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        float* dst = dq_acc + (long long)(b * S + q0 + wq * 16 + g + 8 * hh) * d_model + h * DH + cw * (DH / 2) + 2 * t4;
+      for (int j = 0; j < 8; ++j) {
 #pragma unroll
-        for (int j = 0; j < DH / 16; ++j) red_add_f32x2(dst + 8 * j, dq[4 * j + 2 * hh], dq[4 * j + 2 * hh + 1]);
+        for (int hh = 0; hh < 2; ++hh) {
+          const int r = g + 8 * hh, unit = (2 * (j & 3) + (t4 >> 1)) ^ g;   // r & 7 == g
+          *reinterpret_cast<float2*>(sDQw + (j >> 2) * 2048 + r * 128 + (unit << 4) + 8 * (t4 & 1)) =
+              make_float2(dq[4 * j + 2 * hh], dq[4 * j + 2 * hh + 1]);
+        }
+      }
+      fence_proxy_async_smem();
+      __syncwarp();
+      if (lane == 0) {
+        const int row = b * S + q0 + (DH == 64 ? cw * 64 : 0) + wq * 16, col = h * DH + (DH == 128 ? cw * 64 : 0);
+        tma_reduce_add_2d(&tmDQ, sDQw, col, row);
+        tma_reduce_add_2d(&tmDQ, sDQw + 2048, col + 32, row);
+        tma_commit();
       }
     }
-  };
-  if constexpr (GQA) {
-    for (int h = h0; h < h0 + G; ++h) walk(h, (h - h0) * (n_q - i0));
-  } else {
-    walk(h0, 0);
   }
   // dK (x scale), dV of the kv head (summed over its query heads) -> bf16 -> dqkv
 #pragma unroll
@@ -512,6 +544,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
       *reinterpret_cast<uint32_t*>(vrow + 8 * j + 2 * t4) = pack_bf16(dv[4 * j + 2 * hh], dv[4 * j + 2 * hh + 1]);
     }
   }
+  if (lane == 0) tma_wait_read<0>();   // the staging stays in place until the last reduce-add has read it
 }
 
 // ======================================================================================= document bounds
@@ -588,6 +621,9 @@ void attention_bwd_launch(const void* qkv, const void* out, const void* dout, co
   const int d = H * dh;
   const uint64_t w = uint64_t(H + 2 * Hkv) * dh;   // fused qkv row width
   const long long rows = (long long)B * S;
+  // the kernel bulk-copies lse / delta / doc_start rows of 64 or 128 entries: 16-byte aligned base addresses keep them aligned
+  for (const void* p : {(const void*)lse, (const void*)delta, (const void*)doc_start})
+    if (reinterpret_cast<uintptr_t>(p) & 15) throw std::runtime_error("photon_b200 attention backward: lse, delta and doc_start must be 16-byte aligned");
   cudaMemsetAsync(dq_acc, 0, size_t(rows) * d * sizeof(float), st);
   {
     const long long n8 = rows * H * (dh / 8);
@@ -596,15 +632,17 @@ void attention_bwd_launch(const void* qkv, const void* out, const void* dout, co
     launched("attention bwd delta");
   }
   CUtensorMap tmKV = make_tmap_2d(qkv, 2, false, w, uint64_t(rows), w * 2, 64, 128);
-  CUtensorMap tmQ = make_tmap_2d(qkv, 2, false, w, uint64_t(rows), w * 2, 64, 64);
-  CUtensorMap tmDO = make_tmap_2d(dout, 2, false, uint64_t(d), uint64_t(rows), uint64_t(d) * 2, 64, 64);
+  CUtensorMap tmDQ = make_tmap_2d(dq_acc, 4, true, uint64_t(d), uint64_t(rows), uint64_t(d) * 4, 32, 16);   // one warp's 16 x 32 box
   const dim3 grid(S / 128, B * Hkv);
   with_bools([&](auto gqa, auto alibi, auto wide, auto doc) {
     constexpr int DHV = wide ? 128 : 64;
+    using C = BwdCfg<DHV>;
+    CUtensorMap tmQ = make_tmap_2d(qkv, 2, false, w, uint64_t(rows), w * 2, 64, C::BQS);
+    CUtensorMap tmDO = make_tmap_2d(dout, 2, false, uint64_t(d), uint64_t(rows), uint64_t(d) * 2, 64, C::BQS);
     auto kern = attn_bwd_kernel<DHV, alibi, doc, gqa>;
-    opt_in_smem(kern, BwdCfg<DHV>::SMEM);
-    kern<<<grid, 384, BwdCfg<DHV>::SMEM, st>>>(tmKV, tmQ, tmDO, lse, delta, (__nv_bfloat16*)dqkv, S, H, scale, causal ? 1 : 0, dq_acc,
-                                               alibi_slopes, doc_start, doc_end, Hkv);
+    opt_in_smem(kern, C::SMEM);
+    kern<<<grid, 384, C::SMEM, st>>>(tmKV, tmQ, tmDO, tmDQ, lse, delta, (__nv_bfloat16*)dqkv, S, H, scale, causal ? 1 : 0, alibi_slopes,
+                                     doc_start, doc_end, Hkv);
   }, Hkv != H, alibi_slopes != nullptr, dh == 128, doc_start != nullptr);
   launched("attention bwd");
   attn_bwd_dq_convert_kernel<<<sms * 8, 256, 0, st>>>(dq_acc, (__nv_bfloat16*)dqkv, rows, d, int(w), scale);

@@ -11,7 +11,8 @@ namespace pb {
 void attention_fwd_launch(const void* qkv, void* out, float* lse, int B, int S, int H, int Hkv, int dh, float scale, bool causal,
                           cudaStream_t st, const float* alibi_slopes = nullptr, const int* doc_start = nullptr);
 // dqkv: bf16 shaped like qkv (dK / dV of a kv head summed over its query heads); delta: fp32 scratch [B,H,S]; dq_acc: fp32 scratch [B*S, H*dh],
-// owned by the caller (zeroed here on st, then read by the last kernel on st). doc_start / doc_end: both or neither
+// owned by the caller (zeroed here on st, then read by the last kernel on st). doc_start / doc_end: both or neither. lse, delta
+// and doc_start must be 16-byte aligned
 void attention_bwd_launch(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta, float* dq_acc,
                           int B, int S, int H, int Hkv, int dh, float scale, bool causal, int num_sms, cudaStream_t st,
                           const float* alibi_slopes = nullptr, const int* doc_start = nullptr, const int* doc_end = nullptr);
