@@ -77,7 +77,8 @@ inline bool is_byte(const Tensor& t) {
 // a: [M,K] (a_mn=0) or [K,M] (a_mn=1);  b: [N,K] (b_mn=0) or [K,N] (b_mn=1);  d: [M,N]. The checks and arguments gemm and
 // gemm_fp8 share; the caller checks the operand dtypes and holds the device guard.
 pb::GemmArgs gemm_args(const Tensor& a, const Tensor& b, Tensor& d, int a_mn, int b_mn, int epi, const c10::optional<Tensor>& bias,
-                       const c10::optional<Tensor>& aux, const c10::optional<Tensor>& d2, bool accumulate, double alpha, int cluster) {
+                       const c10::optional<Tensor>& aux, const c10::optional<Tensor>& d2, bool accumulate, double alpha, int cluster,
+                       const c10::optional<Tensor>& aux2 = c10::nullopt) {
   check_cuda(d, "d");
   TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && d.dim() == 2, "gemm operands must be 2-D");
   TORCH_CHECK(a.stride(1) == 1 && b.stride(1) == 1 && d.stride(1) == 1, "gemm operands must have unit inner stride");
@@ -105,6 +106,11 @@ pb::GemmArgs gemm_args(const Tensor& a, const Tensor& b, Tensor& d, int a_mn, in
     TORCH_CHECK(aux->size(0) == g.M && aux->size(1) == g.N && aux->stride(1) == 1, "aux must be [M,N]");
     g.aux = aux->data_ptr(), g.ld_aux = aux->stride(0);
   }
+  if (aux2.has_value()) {
+    check_bf16(*aux2, "aux2");
+    TORCH_CHECK(aux2->size(0) == g.M && aux2->size(1) == g.N && aux2->stride(1) == 1, "aux2 must be [M,N]");
+    g.aux2 = aux2->data_ptr(), g.ld_aux2 = aux2->stride(0);
+  }
   if (d2.has_value()) {
     check_bf16(*d2, "d2");
     TORCH_CHECK(d2->size(0) == g.M && d2->size(1) == g.N && d2->stride(1) == 1, "d2 must be [M,N]");
@@ -115,11 +121,12 @@ pb::GemmArgs gemm_args(const Tensor& a, const Tensor& b, Tensor& d, int a_mn, in
   return g;
 }
 void gemm(const Tensor& a, const Tensor& b, Tensor& d, int a_mn, int b_mn, int epi, const c10::optional<Tensor>& bias,
-          const c10::optional<Tensor>& aux, c10::optional<Tensor> d2, bool accumulate, double alpha, int cluster) {
+          const c10::optional<Tensor>& aux, c10::optional<Tensor> d2, bool accumulate, double alpha, int cluster,
+          const c10::optional<Tensor>& aux2) {
   check_bf16(a, "a");
   check_bf16(b, "b");
   c10::cuda::CUDAGuard guard(a.device());
-  pb::gemm_launch(gemm_args(a, b, d, a_mn, b_mn, epi, bias, aux, d2, accumulate, alpha, cluster), stream_of(a));
+  pb::gemm_launch(gemm_args(a, b, d, a_mn, b_mn, epi, bias, aux, d2, accumulate, alpha, cluster, aux2), stream_of(a));
 }
 // `meta` = float32 [3, n_roles] = (scale, scale_inv, amax) rows
 void gemm_fp8(const Tensor& a, const Tensor& b, Tensor& d, int a_mn, int b_mn, int epi, int a_fmt, int b_fmt, const Tensor& meta, int role_a,
@@ -401,7 +408,7 @@ void skinny_gemm(const Tensor& x, const Tensor& w, Tensor& y, const c10::optiona
   TORCH_CHECK(x.size(1) > 0 && x.size(1) % 8 == 0 && w.size(0) > 0, "skinny_gemm: K must be a positive multiple of 8 and N positive");
   check_vec(x, "skinny_gemm", "x");
   check_vec(w, "skinny_gemm", "w");
-  TORCH_CHECK(epi >= pb::SKINNY_PLAIN && epi <= pb::SKINNY_GELU, "skinny_gemm: unknown epilogue");
+  TORCH_CHECK(epi >= pb::SKINNY_PLAIN && epi <= pb::SKINNY_MUL, "skinny_gemm: unknown epilogue");
   c10::cuda::CUDAGuard guard(x.device());
   pb::SkinnyArgs a;
   a.X = x.data_ptr(), a.W = w.data_ptr(), a.Y = y.data_ptr();
@@ -413,8 +420,8 @@ void skinny_gemm(const Tensor& x, const Tensor& w, Tensor& y, const c10::optiona
     TORCH_CHECK(bias->numel() == a.N && bias->is_contiguous(), "bias must be contiguous with N elements");
     a.bias = bias->data_ptr<float>();
   }
-  if (epi == pb::SKINNY_RESIDUAL) {
-    TORCH_CHECK(residual.has_value(), "the residual epilogue needs the residual");
+  if (epi == pb::SKINNY_RESIDUAL || epi == pb::SKINNY_MUL) {
+    TORCH_CHECK(residual.has_value(), "the residual and multiply epilogues need the residual / multiplier");
     check_bf16(*residual, "residual");
     TORCH_CHECK(residual->dim() == 2 && residual->size(0) == a.M && residual->size(1) == a.N && residual->stride(1) == 1,
                 "residual must be [M, N]");
@@ -933,7 +940,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "photon_b200 sm_90a kernels (wgmma/TMA GEMM + attention, fused norm/loss/optimizer, NVLink collectives)";
   m.def("gemm", &gemm, py::arg("a"), py::arg("b"), py::arg("d"), py::arg("a_mn") = 0, py::arg("b_mn") = 0, py::arg("epi") = 0,
         py::arg("bias") = py::none(), py::arg("aux") = py::none(), py::arg("d2") = py::none(), py::arg("accumulate") = false,
-        py::arg("alpha") = 1.0, py::arg("cluster") = 0);
+        py::arg("alpha") = 1.0, py::arg("cluster") = 0, py::arg("aux2") = py::none());
   m.def("gemm_fp8", &gemm_fp8, py::arg("a"), py::arg("b"), py::arg("d"), py::arg("a_mn"), py::arg("b_mn"), py::arg("epi"), py::arg("a_fmt"),
         py::arg("b_fmt"), py::arg("meta"), py::arg("role_a"), py::arg("role_b"), py::arg("bias") = py::none(), py::arg("aux") = py::none(),
         py::arg("d2") = py::none(), py::arg("accumulate") = false, py::arg("alpha") = 1.0, py::arg("cluster") = 0,
@@ -1014,7 +1021,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.attr("EPI_GELU_GRAD") = int(pb::EPI_GELU_GRAD);
   m.attr("EPI_MUL") = int(pb::EPI_MUL);
   m.attr("EPI_GELU_GRAD_Q8") = int(pb::EPI_GELU_GRAD_Q8);
+  m.attr("EPI_SILU_GRAD") = int(pb::EPI_SILU_GRAD);
+  m.attr("EPI_MUL2") = int(pb::EPI_MUL2);
   m.attr("SKINNY_PLAIN") = int(pb::SKINNY_PLAIN);
   m.attr("SKINNY_RESIDUAL") = int(pb::SKINNY_RESIDUAL);
   m.attr("SKINNY_GELU") = int(pb::SKINNY_GELU);
+  m.attr("SKINNY_SILU") = int(pb::SKINNY_SILU);
+  m.attr("SKINNY_MUL") = int(pb::SKINNY_MUL);
 }

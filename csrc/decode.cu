@@ -58,6 +58,8 @@ __device__ __forceinline__ float sk_finish(float v, const SkParams& p, int m, in
   if (p.bias) v += __ldg(p.bias + n);
   if (EPI == SKINNY_RESIDUAL) v += __bfloat162float(p.R[(long long)m * p.ldr + n]);
   if (EPI == SKINNY_GELU) v = gelu_exact(v);
+  if (EPI == SKINNY_SILU) v *= silu_sigmoid(v);
+  if (EPI == SKINNY_MUL) v *= __bfloat162float(p.R[(long long)m * p.ldr + n]);
   return v;
 }
 
@@ -671,6 +673,8 @@ void skinny_gemm_launch(const SkinnyArgs& a, float* partials, cudaStream_t st) {
   if (a.epi == SKINNY_PLAIN) skinny_launch_nb<SKINNY_PLAIN>(tw, a, p, tiles, st);
   else if (a.epi == SKINNY_RESIDUAL) skinny_launch_nb<SKINNY_RESIDUAL>(tw, a, p, tiles, st);
   else if (a.epi == SKINNY_GELU) skinny_launch_nb<SKINNY_GELU>(tw, a, p, tiles, st);
+  else if (a.epi == SKINNY_SILU) skinny_launch_nb<SKINNY_SILU>(tw, a, p, tiles, st);
+  else if (a.epi == SKINNY_MUL) skinny_launch_nb<SKINNY_MUL>(tw, a, p, tiles, st);
   else throw std::runtime_error("photon_b200 skinny gemm: unknown epilogue");
 }
 

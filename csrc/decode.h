@@ -20,6 +20,8 @@ enum SkinnyEpi : int {
   SKINNY_PLAIN = 0,      // Y = X W^T (+ bias)
   SKINNY_RESIDUAL = 1,   // Y = X W^T (+ bias) + R
   SKINNY_GELU = 2,       // Y = gelu_exact(X W^T (+ bias))  (the formula of the training epilogue)
+  SKINNY_SILU = 3,       // Y = silu(X W^T (+ bias))  (the formula of the training epilogue)
+  SKINNY_MUL = 4,        // Y = (X W^T (+ bias)) * R  (R: the multiplier, passed where the residual goes)
 };
 
 struct SkinnyArgs {
@@ -27,7 +29,7 @@ struct SkinnyArgs {
   const void* W = nullptr;   // [N, K] bf16, row stride ldw
   void* Y = nullptr;         // [M, N] bf16, row stride ldy
   const float* bias = nullptr;
-  const void* R = nullptr;   // residual [M, N] bf16, row stride ldr
+  const void* R = nullptr;   // residual (SKINNY_RESIDUAL) or multiplier (SKINNY_MUL) [M, N] bf16, row stride ldr
   long long ldx = 0, ldw = 0, ldy = 0, ldr = 0;
   int M = 0, N = 0, K = 0;
   int epi = SKINNY_PLAIN;

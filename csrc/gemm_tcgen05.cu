@@ -4,9 +4,9 @@
 //     producer thread (its warpgroup hands its registers to the MMA warpgroups with setmaxnreg)
 //   * two MMA warpgroups, 64 rows of the 128 x 256 tile each: wgmma.mma_async (bf16: m64n256k16, fp8: m64n256k32) with the
 //     fp32 accumulators in registers; a stage is released as soon as the next stage's MMAs are issued (wait_group 1)
-//   * epilogue: bias / residual / GELU / dGELU / fp8 re-quantisation in registers, then stmatrix into a per-warpgroup 128B-swizzled
-//     staging buffer and TMA stores (cp.async.bulk.tensor) that drain while the next tile's mainloop runs; fp32 outputs (weight
-//     gradients, split-K partials) go straight from registers, accumulated by red.global.add
+//   * epilogue: bias / residual / GELU / SiLU / dGELU / gating multipliers / fp8 re-quantisation in registers, then stmatrix
+//     into a per-warpgroup 128B-swizzled staging buffer and TMA stores (cp.async.bulk.tensor) that drain while the next tile's
+//     mainloop runs; fp32 outputs (weight gradients, split-K partials) go straight from registers, accumulated by red.global.add
 //   * bf16 operands may be K-major ([rows,K] row-major) or MN-major ([K,rows] row-major) so forward, dgrad (B = W as stored)
 //     and wgrad (A = dY^T, B = X^T as stored) need no transposes; wgmma reads 8-bit operands K-major only, so an MN-major fp8
 //     operand is transposed into scratch first (transpose_u8)
@@ -48,10 +48,13 @@ struct Params {
   int M, N, K;
   int tiles_m, tiles_n, m_fastest;
   const float* bias;            // [N] fp32 or nullptr
-  const __nv_bfloat16* aux;     // residual (EPI_RESIDUAL) or pre-activation z (EPI_DGELU) or multiplier (EPI_MUL)
+  const __nv_bfloat16* aux;     // residual (EPI_RESIDUAL) or pre-activation z (EPI_DGELU) or multiplier (EPI_MUL, EPI_MUL2)
   long long ld_aux;             // row stride of aux, elements
-  float* d;                     // EPI_F32 output (the other outputs are written through their tensor maps)
-  long long ldd;
+  union {                       // (a union: the parameter block of the other epilogues keeps its size and offsets)
+    float* d;                   // EPI_F32 output (the other outputs are written through their tensor maps)
+    const __nv_bfloat16* aux2;  // EPI_MUL2: the second multiplier
+  };
+  long long ldd;                // row stride of d or aux2, elements
   int accumulate;               // EPI_F32: reduce-add into D instead of overwrite
   float alpha;                  // scale applied to the accumulator before the epilogue
   int splits, kb_per_split;     // split-K (EPI_F32 + accumulate): work item = (tile, k-range)
@@ -85,8 +88,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   constexpr int BK = F8 ? 128 : 64;            // K elements per stage (128 bytes per row)
   constexpr int MNC = F8 ? 128 : 64;           // MN elements in one 128-byte row of an MN-major tile
   constexpr int CHUNK = BK * ROW_BYTES;        // bytes of one MN-major chunk: BK k-rows of 128 bytes
-  constexpr bool TWO_OUT = EPI == EPI_GELU_DUAL || EPI == EPI_GELU_GRAD || EPI == EPI_GELU_GRAD_Q8;
-  constexpr bool AUX = EPI == EPI_RESIDUAL || EPI == EPI_DGELU || EPI == EPI_MUL;
+  constexpr bool TWO_OUT = EPI == EPI_GELU_DUAL || EPI == EPI_GELU_GRAD || EPI == EPI_GELU_GRAD_Q8 || EPI == EPI_SILU_GRAD ||
+                          EPI == EPI_MUL2;
+  constexpr bool AUX = EPI == EPI_RESIDUAL || EPI == EPI_DGELU || EPI == EPI_MUL || EPI == EPI_MUL2;
   static_assert(!F8 || (!A_MN && !B_MN), "8-bit wgmma operands are K-major");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -194,6 +198,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         for (int i = lane; i < 64; i += 32) {
           const int r = row0 + wq * 16 + (i >> 2), c = n_blk * BN + (i & 3) * 64;
           if (r < p.M && c < p.N) prefetch_l2(p.aux + (long long)r * p.ld_aux + c);
+          if (EPI == EPI_MUL2 && r < p.M && c < p.N) prefetch_l2(p.aux2 + (long long)r * p.ldd + c);
         }
       }
       int prev = -1;
@@ -268,6 +273,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       //   * two outputs, 64 columns: D2's box in slot 0, D's in slot 1;
       //   * one output read with aux, 64 columns: one box, in the slot the previous pass did not use (the aux loads of a wider
       //     pass would not fit the register budget);
+      //   * EPI_MUL2 (two outputs read with two multipliers): as two outputs, with the pass's aux loaded at its start (holding
+      //     the next pass's two multipliers through the stores does not fit the register budget);
       //   * one output, 128 columns: two boxes, one per slot.
       // Only the issuing thread waits for its earlier stores to have been read out of the slots, so the writes to global memory
       // drain under the next pass and the next tile's mainloop.
@@ -277,7 +284,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       uint8_t* stg = sE + cw * EPI_WG_BYTES;
       const uint32_t stg_u32 = smem_u32(stg);
       // aux of one pass (bf16 pairs; 0 outside [M, N]): the next pass's are loaded before this pass's barriers and stores
-      uint32_t ax[JP][2];
+      uint32_t ax[JP][2], ax2[JP][2];
       const auto load_aux = [&](int q) {
 #pragma unroll
         for (int jj = 0; jj < JP; ++jj)
@@ -286,13 +293,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             const long long row = (long long)row0 + wq * 16 + g + 8 * h;
             const int col = n_blk * BN + q * CPP + 8 * jj + 2 * t4;
             ax[jj][h] = (col < p.N && row < p.M) ? __ldg(reinterpret_cast<const uint32_t*>(p.aux + row * p.ld_aux + col)) : 0u;
+            if (EPI == EPI_MUL2)
+              ax2[jj][h] = (col < p.N && row < p.M) ? __ldg(reinterpret_cast<const uint32_t*>(p.aux2 + row * p.ldd + col)) : 0u;
           }
       };
-      if (AUX) load_aux(0);
+      if (AUX && EPI != EPI_MUL2) load_aux(0);
 #pragma unroll
       for (int q = 0; q < BN / CPP; ++q) {
         const int cq = n_blk * BN + q * CPP;      // first output column of the pass
         if (cq >= p.N) break;
+        if (EPI == EPI_MUL2) load_aux(q);
         const uint32_t slot = ONE_SLOT ? (pass_ctr++ & 1) * EPI_SLOT : 0;
         const auto slots_free = [&] {             // the previous boxes in the slots this pass writes have been read out
           if ((threadIdx.x & 127) == 0) {
@@ -335,9 +345,17 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             }
             if (AUX) {
               const float2 f = unpack_bf16(ax[jj][h]);
-              if (EPI == EPI_RESIDUAL) v0 += f.x, v1 += f.y;
-              else if (EPI == EPI_MUL) v0 *= f.x, v1 *= f.y;
-              else v0 *= gelu_grad(f.x), v1 *= gelu_grad(f.y);
+              if (EPI == EPI_RESIDUAL) {
+                v0 += f.x, v1 += f.y;
+              } else if (EPI == EPI_MUL) {
+                v0 *= f.x, v1 *= f.y;
+              } else if (EPI == EPI_MUL2) {
+                const float2 f2 = unpack_bf16(ax2[jj][h]);
+                o2[jj][h] = pack_bf16(v0 * f2.x, v1 * f2.y);
+                v0 *= f.x, v1 *= f.y;
+              } else {
+                v0 *= gelu_grad(f.x), v1 *= gelu_grad(f.y);
+              }
             }
             if (EPI == EPI_GELU_DUAL) {
               o2[jj][h] = pack_bf16(v0, v1);   // z (pre-activation)
@@ -355,12 +373,17 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 st_shared_u16(stg_u32 + EPI_SLOT + (wq * 16 + g + 8 * h) * 64 + 8 * jj + 2 * t4, pack_e4m3x2(v0 * q8_scale, v1 * q8_scale));
                 continue;
               }
+            } else if (EPI == EPI_SILU_GRAD) {
+              // silu and its derivative share the sigmoid (one exp); the derivative is saved as EPI_GELU_GRAD saves gelu'
+              const float s0 = silu_sigmoid(v0), s1 = silu_sigmoid(v1);
+              o2[jj][h] = pack_bf16(silu_grad_from(v0, s0), silu_grad_from(v1, s1));
+              v0 *= s0, v1 *= s1;
             }
             o1[jj][h] = pack_bf16(v0, v1);
           }
           if (EPI == EPI_GELU_GRAD_Q8 && (jj & 1)) stage_pair(jj - 1);
         }
-        if (AUX && q + 1 < BN / CPP) load_aux(q + 1);
+        if (AUX && EPI != EPI_MUL2 && q + 1 < BN / CPP) load_aux(q + 1);
         if (EPI != EPI_GELU_GRAD_Q8) {
           slots_free();
 #pragma unroll
@@ -513,14 +536,18 @@ void gemm_launch(const GemmArgs& g, cudaStream_t stream) {
                           : make_tmap_2d(g.A, eb, false, g.K, g.M, g.lda * eb, BKE, BM);
   CUtensorMap tb = g.b_mn ? make_tmap_2d(g.B, eb, false, g.N, g.K, g.ldb * eb, MNC, BKE)
                           : make_tmap_2d(g.B, eb, false, g.K, g.N, g.ldb * eb, BKE, BN / cluster);
-  const bool two_out = g.epi == EPI_GELU_DUAL || g.epi == EPI_GELU_GRAD || g.epi == EPI_GELU_GRAD_Q8;
-  if (two_out && !g.D2) throw std::runtime_error("photon_b200 gemm: the two-output GELU epilogues need the second output");
+  const bool two_out = g.epi == EPI_GELU_DUAL || g.epi == EPI_GELU_GRAD || g.epi == EPI_GELU_GRAD_Q8 || g.epi == EPI_SILU_GRAD ||
+                       g.epi == EPI_MUL2;
+  if (two_out && !g.D2) throw std::runtime_error("photon_b200 gemm: the two-output epilogues need the second output");
   const auto aligned16 = [](const void* ptr, long long ld_bytes) { return !(reinterpret_cast<uintptr_t>(ptr) & 15) && !(ld_bytes % 16); };
   // the TMA store writes whole 16-byte pieces of a row, so the E4M3 output also needs N % 16 == 0 (bf16 rows: N % 8 == 0)
   if (g.epi == EPI_GELU_GRAD_Q8 && (!g.fp8 || !g.D8 || !aligned16(g.D8, g.ldd8) || g.N % 16))
     throw std::runtime_error("photon_b200 gemm: the fp8-output epilogue needs fp8 operands, a 16-byte aligned fp8 output and row stride, and N % 16 == 0");
-  if ((g.epi == EPI_RESIDUAL || g.epi == EPI_DGELU || g.epi == EPI_MUL) && (!g.aux || (g.ld_aux % 8) || (reinterpret_cast<uintptr_t>(g.aux) & 15)))
+  if ((g.epi == EPI_RESIDUAL || g.epi == EPI_DGELU || g.epi == EPI_MUL || g.epi == EPI_MUL2) &&
+      (!g.aux || (g.ld_aux % 8) || (reinterpret_cast<uintptr_t>(g.aux) & 15)))
     throw std::runtime_error("photon_b200 gemm: aux operand missing or not 16-byte aligned");
+  if (g.epi == EPI_MUL2 && (!g.aux2 || (g.ld_aux2 % 8) || (reinterpret_cast<uintptr_t>(g.aux2) & 15)))
+    throw std::runtime_error("photon_b200 gemm: aux2 operand missing or not 16-byte aligned");
   if (g.bias && (reinterpret_cast<uintptr_t>(g.bias) & 15)) throw std::runtime_error("photon_b200 gemm: bias must be 16-byte aligned");
   if (g.epi != EPI_GELU_GRAD_Q8 && ((reinterpret_cast<uintptr_t>(g.D) & 15) || (g.ldd % 8)))
     throw std::runtime_error("photon_b200 gemm: output must be 16-byte aligned");
@@ -541,6 +568,7 @@ void gemm_launch(const GemmArgs& g, cudaStream_t stream) {
   p.aux = reinterpret_cast<const __nv_bfloat16*>(g.aux);
   p.ld_aux = g.ld_aux;
   p.d = reinterpret_cast<float*>(g.D), p.ldd = g.ldd;
+  if (g.epi == EPI_MUL2) p.aux2 = reinterpret_cast<const __nv_bfloat16*>(g.aux2), p.ldd = g.ld_aux2;
   p.accumulate = g.accumulate;
   p.alpha = g.alpha;
   p.a_fmt = g.a_fmt, p.b_fmt = g.b_fmt, p.sinv_a = g.sinv_a, p.sinv_b = g.sinv_b;
@@ -589,6 +617,11 @@ void gemm_launch(const GemmArgs& g, cudaStream_t stream) {
   PB_CASE(1, 1, EPI_BF16, 0)
   PB_CASE(1, 0, EPI_F32, 0)
   PB_CASE(1, 0, EPI_BF16, 0)
+  // gated / SiLU feed-forward blocks: activation + derivative, the two-multiplier forward and dgrad, the accumulating dgrad
+  PB_CASE(0, 0, EPI_SILU_GRAD, 0)
+  PB_CASE(0, 0, EPI_MUL2, 0)
+  PB_CASE(0, 1, EPI_MUL2, 0)
+  PB_CASE(0, 1, EPI_RESIDUAL, 0)
   // fp8 operands (K-major; the bindings transpose MN-major ones): forward, dgrad and wgrad epilogues
   PB_CASE(0, 0, EPI_BF16, 1)
   PB_CASE(0, 0, EPI_RESIDUAL, 1)

@@ -16,6 +16,11 @@ enum Epilogue : int {
   EPI_GELU_GRAD = 5,  // z = acc*alpha + bias;  D = bf16(gelu(z));  D2 = bf16(gelu'(z))  — the backward then needs no erf/exp
   EPI_MUL = 6,        // D = bf16((acc*alpha + bias) * aux)
   EPI_GELU_GRAD_Q8 = 7,  // fp8 operands only: z = acc*alpha + bias;  D8 = e4m3(gelu(z) * *out_scale) (+ amax);  D2 = bf16(gelu'(z))
+  EPI_SILU_GRAD = 8,  // z = acc*alpha + bias;  D = bf16(silu(z));  D2 = bf16(silu'(z))  — EPI_GELU_GRAD with SiLU
+  // v = acc*alpha + bias;  D = bf16(v * aux);  D2 = bf16(v * aux2) — the gated FFN: forward up projection (aux = act(g),
+  // aux2 = act'(g): D = act(g)*u, D2 = u*act'(g)) and its dgrad (aux = act(g), aux2 = u*act'(g): D = du, D2 = dg). aux and aux2
+  // are read through the read-only data path, so D / D2 must not overlap them (no in-place update).
+  EPI_MUL2 = 9,
 };
 
 struct GemmArgs {
@@ -25,8 +30,9 @@ struct GemmArgs {
   void* D2 = nullptr;       // second output (EPI_GELU_DUAL / EPI_GELU_GRAD), bf16 [M,N]
   const float* bias = nullptr;
   const void* aux = nullptr;  // bf16 [M,N]
+  const void* aux2 = nullptr; // bf16 [M,N], second multiplier (EPI_MUL2)
   int M = 0, N = 0, K = 0;
-  long long lda = 0, ldb = 0, ldd = 0, ldd2 = 0, ld_aux = 0;
+  long long lda = 0, ldb = 0, ldd = 0, ldd2 = 0, ld_aux = 0, ld_aux2 = 0;
   int a_mn = 0, b_mn = 0;
   int epi = EPI_BF16;
   int accumulate = 0;

@@ -239,6 +239,9 @@ __device__ __forceinline__ float gelu_grad(float x) {
   gelu_cdf_pdf(x, c, d);
   return fmaf(x, d, c);
 }
+// silu(x) = x * s and silu'(x) = s * (1 + x * (1 - s)), s = sigmoid(x): one exp for both
+__device__ __forceinline__ float silu_sigmoid(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
+__device__ __forceinline__ float silu_grad_from(float x, float s) { return s * fmaf(x, 1.0f - s, 1.0f); }
 
 // ---------------------------------------------------------------- cross-GPU flags (sys scope)
 __device__ __forceinline__ void st_release_sys(uint32_t* p, uint32_t v) {

@@ -6,7 +6,9 @@ attention right padding never reaches a valid row, so the padded batch is exact 
 processes one new token per sequence:
 
     embed (per-row position) -> per block: LN -> QKV -> (clip / qk_ln) -> append (RoPE + cache write) -> decode attention
-    -> out-proj + residual -> LN -> up + GELU -> down + residual -> final LN -> LM head -> argmax (on the device)
+    -> out-proj + residual -> LN -> FFN -> down + residual -> final LN -> LM head -> argmax (on the device)
+
+where the FFN is up + activation (GELU or SiLU) or, gated (``mptglu``), gate + activation -> up times that.
 
 The step is captured as one CUDA graph per batch size and replayed; token ids, positions and the cache are static device
 buffers, and the host reads back one int32 per sequence. The GEMMs of a step use the weight-streaming skinny GEMM up to
@@ -73,9 +75,11 @@ class KVDecoder:
         c, dev = self.cfg, self.dev
         bf = lambda *s: torch.empty(*s, dtype=torch.bfloat16, device=dev)  # noqa: E731
         f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
-        d, dff = c.d_model, c.expansion_ratio * c.d_model
+        d, dff = c.d_model, c.ffn_hidden
         x = {"h": bf(n, d) if h is None else h, "ln": bf(n, d), "m": f32(n), "r": f32(n), "qkv": bf(n, c.qkv_dim), "attn": bf(n, d),
              "hmid": bf(n, d), "u": bf(n, dff), "z": bf(n, dff)}
+        if c.ffn_gated and n > SKINNY_MAX_M:   # the training GEMM's gated forward also writes act'(g) and u * act'(g)
+            x.update(ffn_d=bf(n, dff), ffn_c=bf(n, dff))
         if c.qk_ln:
             x.update(qk_pre=bf(n, d), qk_tmp=bf(n, d))
         return x
@@ -94,6 +98,28 @@ class KVDecoder:
             ops.linear_gelu_fwd(x, w, b, pre, out)
         else:
             ops.linear_fwd(x, w, b, out, residual=residual)
+
+    def _ffn(self, w: Any, ln: torch.Tensor, u: torch.Tensor, z: torch.Tensor, out: torch.Tensor, resid: torch.Tensor,
+             dact: torch.Tensor | None = None, cg: torch.Tensor | None = None) -> None:
+        """``out = resid + ffn(ln)``. ``u`` / ``z``: [rows, F] scratch; a gated FFN over more than ``SKINNY_MAX_M`` rows runs the
+        training forward, which also writes act'(g) into ``dact`` and u * act'(g) into ``cg``."""
+        c = self.cfg
+        skinny = ln.shape[0] <= SKINNY_MAX_M
+        if c.ffn_gated:
+            if skinny:   # z = act(gate(ln)); u = up(ln) * z
+                ops.skinny_gemm(ln, w.wgate, z, w.bgate, gelu=c.ffn_act == "gelu", silu=c.ffn_act == "silu")
+                ops.skinny_gemm(ln, w.wup, u, w.bup, mul=z)
+            else:
+                ops.linear_act_grad_fwd(c.ffn_act, ln, w.wgate, w.bgate, dact, z)
+                ops.linear_glu_up_fwd(ln, w.wup, w.bup, z, dact, u, cg)
+        elif c.ffn_act == "silu":
+            if skinny:
+                ops.skinny_gemm(ln, w.wup, u, w.bup, silu=True)
+            else:
+                ops.linear_silu_grad_fwd(ln, w.wup, w.bup, z, u)
+        else:
+            self._linear(ln, w.wup, w.bup, u, gelu=True, pre=z)
+        self._linear(u, w.wdown, w.bdown, out, residual=resid)
 
     def _qkv_post(self, w: Any, qkv: torch.Tensor, pre: torch.Tensor, tmp: torch.Tensor, m: torch.Tensor, r: torch.Tensor) -> None:
         """clip_qkv and qk_ln exactly as the training forward applies them."""
@@ -127,7 +153,8 @@ class KVDecoder:
         f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=self.dev)  # noqa: E731
         h, hmid, ln, qkv, attn = bf(T, d), bf(T, d), bf(T, d), bf(T, W), bf(T, d)
         m, r, lse = f32(T), f32(T), f32(b, H, S)
-        u, z = bf(T, c.expansion_ratio * d), bf(T, c.expansion_ratio * d)
+        u, z = bf(T, c.ffn_hidden), bf(T, c.ffn_hidden)
+        dact, cg = (bf(T, c.ffn_hidden), bf(T, c.ffn_hidden)) if c.ffn_gated else (None, None)
         pre, tmp = (bf(T, d), bf(T, d)) if c.qk_ln else (None, None)
         ops.embed_fwd(ids.reshape(-1), e.wte16, e.wpe16, h, S)
         for i, w in enumerate(e.layers):
@@ -142,8 +169,7 @@ class KVDecoder:
             self.cache[i, 1, :, :, :S].index_copy_(0, dst, v)
             ops.linear_fwd(attn, w.wo, w.bo, hmid, residual=h)
             ops.layernorm_fwd(hmid, w.g2, w.b2, ln, m, r, c.norm_eps)
-            ops.linear_gelu_fwd(ln, w.wup, w.bup, z, u)
-            ops.linear_fwd(u, w.wdown, w.bdown, h, residual=hmid)
+            self._ffn(w, ln, u, z, h, hmid, dact, cg)
         last = torch.tensor([i * S + n - 1 for i, n in enumerate(lens)], dtype=torch.long).to(self.dev, non_blocking=True)
         return torch.index_select(h, 0, last)
 
@@ -191,8 +217,7 @@ class KVDecoder:
                 ops.cache_attention(qkv, kc, vc, tiles, attn, c.n_heads, self.scale, e.alibi, n_kv_heads=c.kv_n_heads)
             self._linear(attn, w.wo, w.bo, hmid, residual=h)
             ops.layernorm_fwd(hmid, w.g2, w.b2, ln, m, r, c.norm_eps)
-            self._linear(ln, w.wup, w.bup, u, gelu=True, pre=z)
-            self._linear(u, w.wdown, w.bdown, h, residual=hmid)
+            self._ffn(w, ln, u, z, h, hmid, x.get("ffn_d"), x.get("ffn_c"))
 
     # --------------------------------------------------------------------- step
     def _step_kernels(self, b: int) -> None:

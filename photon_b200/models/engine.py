@@ -33,14 +33,15 @@ import torch
 import torch.nn.functional as F
 
 from photon_b200 import ops
-from photon_b200.models.mpt import MPTConfig, MPTForCausalLM, check_sequence_id, shift_labels
+from photon_b200.models.mpt import MPTConfig, MPTForCausalLM, check_sequence_id, ffn_desc, nondefault_ffn, shift_labels
 from photon_b200.train.backend import apply_freeze
 from photon_b200.utils.flat import FlatLayout, FlatParams
 
 # One block's backward as stages in execution order, each with the parameters whose gradients it produces (a stage's input
-# gradient feeds the next one; the residual path joins at ln2 / ln1). "attn" is the attention backward with the q/k LayerNorms.
+# gradient feeds the next one; the residual path joins at ln2 / ln1). "attn" is the attention backward with the q/k LayerNorms;
+# "up" covers the gate projection of a gated FFN too (its names are absent from an mptmlp layout).
 BLOCK_STAGES = (("down", ("ffn.down_proj.weight", "ffn.down_proj.bias")),
-                ("up", ("ffn.up_proj.weight", "ffn.up_proj.bias")),
+                ("up", ("ffn.up_proj.weight", "ffn.up_proj.bias", "ffn.gate_proj.weight", "ffn.gate_proj.bias")),
                 ("ln2", ("norm_2.weight", "norm_2.bias")),
                 ("out", ("attn.out_proj.weight", "attn.out_proj.bias")),
                 ("attn", ("attn.q_ln.weight", "attn.q_ln.bias", "attn.k_ln.weight", "attn.k_ln.bias")),
@@ -97,7 +98,7 @@ class _LayerW:
 
     __slots__ = ("wqkv", "bqkv", "wo", "bo", "wup", "bup", "wdown", "bdown", "g1", "b1", "g2", "b2",
                  "d_wqkv", "d_bqkv", "d_wo", "d_bo", "d_wup", "d_bup", "d_wdown", "d_bdown", "d_g1", "d_b1", "d_g2", "d_b2",
-                 "qk_g", "qk_b", "d_qk_g", "d_qk_b")
+                 "qk_g", "qk_b", "d_qk_g", "d_qk_b", "wgate", "bgate", "d_wgate", "d_bgate")
 
 
 class B200Engine:
@@ -121,6 +122,13 @@ class B200Engine:
             raise NotImplementedError(f"B200Engine computes in bf16 (got precision={precision}); use kernels.*=torch for fp32/fp16")
         if (frozen_layers or unfrozen_layers) and zero3 is not None:
             raise NotImplementedError("freeze lists are not covered under full parameter sharding (kernels.*=torch runs them)")
+        if nondefault_ffn(cfg) and (precision == "amp_fp8" or zero3 is not None):
+            raise NotImplementedError(f"{ffn_desc(cfg)} is not covered under amp_fp8 or full parameter sharding "
+                                      "(kernels.*=torch runs it)")
+        if cfg.ffn_hidden % 8:
+            # every GEMM operand / output row and the bias-gradient column sums of the FFN are [*, F] bf16 rows that must
+            # be 16-byte multiples (the TMA row-stride and N % 8 launch checks)
+            raise ValueError(f"the sm_90a engine needs an FFN width that is a multiple of 8, got {cfg.ffn_hidden}")
         ops.ext()  # fail loudly if the extension is missing
         self.precision = precision
         self.zero3 = zero3
@@ -255,6 +263,9 @@ class B200Engine:
             w.qk_b = [v32(p + "attn.q_ln.bias"), v32(p + "attn.k_ln.bias")]
             w.d_qk_g = [vg(p + "attn.q_ln.weight"), vg(p + "attn.k_ln.weight")]
             w.d_qk_b = [vg(p + "attn.q_ln.bias"), vg(p + "attn.k_ln.bias")]
+            gated = self.cfg.ffn_gated   # ffn_config.ffn_type mptglu: gate_proj next to up_proj
+            w.wgate, w.bgate = (v16(p + "ffn.gate_proj.weight"), v32(p + "ffn.gate_proj.bias")) if gated else (None, None)
+            w.d_wgate, w.d_bgate = (vg(p + "ffn.gate_proj.weight"), vg(p + "ffn.gate_proj.bias")) if gated else (None, None)
             self.layers.append(w)
 
     def params_updated(self) -> None:
@@ -381,7 +392,7 @@ class B200Engine:
         self._ws.clear()  # one live shape at a time (activations dominate memory)
         self._graphs.clear()  # captured graphs point into the old workspace
         c, dev = self.cfg, self.device
-        T, d, H, L, W = b * S, c.d_model, c.n_heads, c.n_layers, c.qkv_dim
+        T, d, H, L, W, Fh = b * S, c.d_model, c.n_heads, c.n_layers, c.qkv_dim, c.ffn_hidden
         bf = lambda *s: torch.empty(*s, dtype=torch.bfloat16, device=dev)  # noqa: E731
         f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
         ws: dict[str, Any] = {"h": [bf(T, d) for _ in range(L + 1)], "layers": []}
@@ -393,11 +404,13 @@ class B200Engine:
                 u8 = lambda *s: torch.empty(*s, dtype=torch.uint8, device=dev)  # noqa: E731
                 ws["layers"].append({"ln1": u8(T, d), "m1": f32(T), "r1": f32(T), "qkv": bf(T, W), "attn": bf(T, d), "attn8": u8(T, d),
                                      "lse": f32(b, H, S), "hmid": bf(T, d), "ln2": u8(T, d), "m2": f32(T), "r2": f32(T),
-                                     "z": bf(T, c.expansion_ratio * d), "u": u8(T, c.expansion_ratio * d)})
+                                     "z": bf(T, Fh), "u": u8(T, Fh)})
             else:
                 ws["layers"].append({"ln1": bf(T, d), "m1": f32(T), "r1": f32(T), "qkv": bf(T, W), "attn": bf(T, d),
                                      "lse": f32(b, H, S), "hmid": bf(T, d), "ln2": bf(T, d), "m2": f32(T), "r2": f32(T),
-                                     "z": bf(T, c.expansion_ratio * d), "u": bf(T, c.expansion_ratio * d)})
+                                     "z": bf(T, Fh), "u": bf(T, Fh)})
+                if c.ffn_gated:   # z = u * act'(g), u = act(g) * up (the down projection's input), a = act(g)
+                    ws["layers"][-1]["a"] = bf(T, Fh)
             if c.clip_qkv:
                 ws["layers"][-1]["clipmask"] = torch.empty(T, W, dtype=torch.bool, device=dev)
             if c.qk_ln:   # pre-LayerNorm q / k (inputs of the two LN backward passes) and their row statistics
@@ -405,12 +418,14 @@ class B200Engine:
         if c.qk_ln:   # scratch of the q / k LayerNorms, viewed at the width of the part in use (see _qk_parts)
             ws.update(qk_tmp=bf(T, d), qk_tmp2=bf(T, d))
         ws.update(lnf=bf(T, d), mf=f32(T), rf=f32(T), dlnf=bf(T, d), dh=bf(T, d), dhmid=bf(T, d), dln=bf(T, d),
-                  dqkv=bf(T, W), dattn=bf(T, d), dz=bf(T, c.expansion_ratio * d), delta=f32(b, H, S),
+                  dqkv=bf(T, W), dattn=bf(T, d), dz=bf(T, Fh), delta=f32(b, H, S),
                   logits=bf(min(self.lm_head_chunk, T), c.vocab_size))
         if self.fp8:   # E5M2 copy of the gradient currently flowing backward (one buffer, viewed at the width in use)
-            ws["g8"] = torch.empty(T * max(c.expansion_ratio, 3) * d, dtype=torch.uint8, device=dev)
+            ws["g8"] = torch.empty(T * max(Fh, 3 * d), dtype=torch.uint8, device=dev)
         if c.attn_uses_sequence_id:   # first / last row of each row's document, shared by every layer and both directions
             ws.update(doc_start=torch.empty(T, dtype=torch.int32, device=dev), doc_end=torch.empty(T, dtype=torch.int32, device=dev))
+        if c.ffn_gated:   # the gate's output gradient (the up projection's goes to dz)
+            ws["dg"] = bf(T, Fh)
         ws["sequence_id"] = None      # this microbatch's document ids (set by _forward), None: plain causal
         self._ws[key] = ws
         return ws
@@ -517,7 +532,12 @@ class B200Engine:
             return
         ops.linear_fwd(lw["attn"], w.wo, w.bo, lw["hmid"], residual=h[i])
         ops.layernorm_fwd(lw["hmid"], w.g2, w.b2, lw["ln2"], lw["m2"], lw["r2"], c.norm_eps)
-        ops.linear_gelu_grad_fwd(lw["ln2"], w.wup, w.bup, lw["z"], lw["u"])   # lw["z"] holds gelu'(pre-activation)
+        if c.ffn_gated:
+            # a = act(g), act'(g) into the free dz (a backward buffer); then u = up(ln2): lw["u"] = a * u, lw["z"] = u * act'(g)
+            ops.linear_act_grad_fwd(c.ffn_act, lw["ln2"], w.wgate, w.bgate, ws["dz"], lw["a"])
+            ops.linear_glu_up_fwd(lw["ln2"], w.wup, w.bup, lw["a"], ws["dz"], lw["u"], lw["z"])
+        else:
+            ops.linear_act_grad_fwd(c.ffn_act, lw["ln2"], w.wup, w.bup, lw["z"], lw["u"])   # lw["z"] holds act'(pre-activation)
         ops.linear_fwd(lw["u"], w.wdown, w.bdown, h[i + 1], residual=lw["hmid"])
 
     def _forward(self, ids: torch.Tensor, ws: dict[str, Any], sequence_id: torch.Tensor | None = None) -> None:
@@ -588,6 +608,22 @@ class B200Engine:
             ops.gemm_fp8(dy8, wt if wt is not None else self.w8_views[i][w_role], dx, M, R(g_role, i), R(w_role, i), b_mn=wt is None,
                          epi=ops.EPI_MUL if mul is not None else ops.EPI_BF16, a_fmt=ops.E5M2, b_fmt=ops.E4M3, aux=mul)
 
+    def _glu_bwd(self, i: int, ws: dict[str, Any], d_in: bool, dln: torch.Tensor | None) -> None:
+        """Gated FFN backward (bf16): down's weight / bias gradients and, when ``d_in``, du = (dh W_down) * act(g) and
+        dg = (dh W_down) * c in one dgrad; then the up and gate projections' trainable gradients and, when ``dln`` is given,
+        dln = dg W_gate + du W_up (two dgrads, the second adding the first through its residual epilogue)."""
+        w, lw, dh = self.layers[i], ws["layers"][i], ws["dh"]
+        self._linear_bwd(i, ws, dh, "g_dh", lw["u"], "x_u", "wdown", w.wdown, w.d_wdown, w.d_bdown, None)
+        if not d_in:
+            return
+        du, dg = ws["dz"], ws["dg"]
+        ops.linear_glu_dgrad(dh, w.wdown, lw["a"], lw["z"], du, dg)
+        self._linear_bwd(i, ws, du, "g_dz", lw["ln2"], "x_ln2", "wup", w.wup, w.d_wup, w.d_bup, None)
+        self._linear_bwd(i, ws, dg, "g_dz", lw["ln2"], "x_ln2", "wgate", w.wgate, w.d_wgate, w.d_bgate, None)
+        if dln is not None:
+            ops.linear_dgrad(dg, w.wgate, ws["dattn"])   # dattn is free until the out-projection's dgrad writes it
+            ops.linear_dgrad(du, w.wup, dln, residual=ws["dattn"])
+
     def _backward(self, ids: torch.Tensor, ws: dict[str, Any]) -> None:
         c = self.cfg
         b, S = ids.shape
@@ -618,11 +654,14 @@ class B200Engine:
         c, h, w, lw, P = self.cfg, ws["h"], self.layers[i], ws["layers"][i], self.plan
         dh, dhmid, dln = ws["dh"], ws["dhmid"], ws["dln"]
         dx = lambda s, t: t if P.dx((i, s)) else None  # noqa: E731
-        # ---- FFN: h[i+1] = hmid + down(gelu(up(ln2(hmid))))
-        self._linear_bwd(i, ws, dh, "g_dh", lw["u"], "x_u", "wdown", w.wdown, w.d_wdown, w.d_bdown, dx("down", ws["dz"]), mul=lw["z"])
-        if not P.runs((i, "up")):
-            return
-        self._linear_bwd(i, ws, ws["dz"], "g_dz", lw["ln2"], "x_ln2", "wup", w.wup, w.d_wup, w.d_bup, dx("up", dln))
+        # ---- FFN: h[i+1] = hmid + down(act(up(ln2(hmid))))  or, gated, hmid + down(act(gate(ln2)) * up(ln2))
+        if c.ffn_gated:
+            self._glu_bwd(i, ws, P.dx((i, "down")), dx("up", dln))
+        else:
+            self._linear_bwd(i, ws, dh, "g_dh", lw["u"], "x_u", "wdown", w.wdown, w.d_wdown, w.d_bdown, dx("down", ws["dz"]), mul=lw["z"])
+            if not P.runs((i, "up")):
+                return
+            self._linear_bwd(i, ws, ws["dz"], "g_dz", lw["ln2"], "x_ln2", "wup", w.wup, w.d_wup, w.d_bup, dx("up", dln))
         if not P.runs((i, "ln2")):
             return
         ops.layernorm_bwd(dln, lw["hmid"], w.g2, lw["m2"], lw["r2"], dh, dhmid, w.d_g2, w.d_b2)

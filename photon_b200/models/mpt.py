@@ -7,8 +7,8 @@ photon/utils.py:572,591,602-637; SURVEY Appendix C). The B200 hot path lives in
 :mod:`photon_b200.models.engine`, which runs the same parameters through
 hand-written sm_90a kernels and is tested against this module.
 
-Block: ``x = x + attn(norm_1(x)); x = x + ffn(norm_2(x))``; ``ffn =
-down(gelu_exact(up(x)))``; LM head tied to ``wte``; loss = CE over
+Block: ``x = x + attn(norm_1(x)); x = x + ffn(norm_2(x))``; ``ffn = down(act(up(x)))`` (``mptmlp``) or
+``down(act(gate(x)) * up(x))`` (``mptglu``), ``act`` exact GELU (default) or SiLU; LM head tied to ``wte``; loss = CE over
 ``targets = roll(labels, -1)`` with the last position ignored (-100).
 """
 from __future__ import annotations
@@ -27,7 +27,7 @@ class MPTConfig:
     d_model: int = 768
     n_heads: int = 12
     n_layers: int = 12
-    expansion_ratio: int = 4
+    expansion_ratio: float = 4   # may be fractional, as in llm-foundry: the FFN width is int(d_model * expansion_ratio)
     max_seq_len: int = 2048
     vocab_size: int = 50368
     attn_impl: str = "flash"  # flash | torch | b200
@@ -45,6 +45,11 @@ class MPTConfig:
     # attn_config.attn_type grouped_query_attention / multiquery_attention: K / V have kv_n_heads heads (None: n_heads), query
     # head h attending with kv head h // (n_heads // kv_n_heads)
     kv_n_heads: int | None = None
+    # ffn_config (llm-foundry): ffn_type mptmlp (down(act(up(x)))) or mptglu (down(act(gate(x)) * up(x))); ffn_act_fn gelu
+    # (exact) or silu; ffn_hidden_size overrides the width int(d_model * expansion_ratio)
+    ffn_type: str = "mptmlp"
+    ffn_act: str = "gelu"
+    ffn_hidden_size: int | None = None
     init_std: float | None = None  # None -> kaiming_normal_ (llm-foundry default)
     extra: dict[str, Any] = field(default_factory=dict)
 
@@ -53,6 +58,21 @@ class MPTConfig:
             self.kv_n_heads = self.n_heads
         if self.kv_n_heads < 1 or self.n_heads % self.kv_n_heads:
             raise ValueError(f"kv_n_heads = {self.kv_n_heads} must divide n_heads = {self.n_heads}")
+        if self.ffn_type not in FFN_TYPES:
+            raise ValueError(f"unsupported ffn_config.ffn_type {self.ffn_type!r} (supported: {', '.join(FFN_TYPES)})")
+        if self.ffn_act not in FFN_ACTS:
+            raise ValueError(f"unsupported FFN activation {self.ffn_act!r} (supported: {', '.join(FFN_ACTS)})")
+        if self.ffn_hidden < 1:
+            raise ValueError(f"the FFN width must be positive, got {self.ffn_hidden}")
+
+    @property
+    def ffn_hidden(self) -> int:
+        """Width ``F`` of the feed-forward block: ``ffn_config.ffn_hidden_size``, else ``int(d_model * expansion_ratio)``."""
+        return int(self.ffn_hidden_size) if self.ffn_hidden_size is not None else int(self.d_model * self.expansion_ratio)
+
+    @property
+    def ffn_gated(self) -> bool:
+        return self.ffn_type == "mptglu"
 
     @property
     def d_head(self) -> int:
@@ -106,9 +126,12 @@ class MPTConfig:
             attn_uses_sequence_id=bool(attn.pop("attn_uses_sequence_id", False)), kv_n_heads=kv,
             no_bias=bool(m.pop("no_bias", False)), learned_pos_emb=bool(m.pop("learned_pos_emb", True)),
         )
+        ffn = dict(m.pop("ffn_config", {}) or {})
+        known.update(ffn_type=ffn.pop("ffn_type", "mptmlp"), ffn_act=parse_ffn_act(ffn.pop("ffn_act_fn", None)),
+                     ffn_hidden_size=ffn.pop("ffn_hidden_size", None))
         for k in ("name", "init_device"):
             m.pop(k, None)
-        cfg = cls(**known, extra={**m, **({"attn_config": attn} if attn else {}),
+        cfg = cls(**known, extra={**m, **({"attn_config": attn} if attn else {}), **({"ffn_config": ffn} if ffn else {}),
                                   **({"rope_impl": rope_cfg} if rope_cfg else {})})
         if cfg.d_model % cfg.n_heads:
             raise ValueError("d_model must be divisible by n_heads")
@@ -117,10 +140,12 @@ class MPTConfig:
         return cfg
 
     def num_params(self) -> int:
-        d, L, V, S, e = self.d_model, self.n_layers, self.vocab_size, self.max_seq_len, self.expansion_ratio
+        d, L, V, S, f = self.d_model, self.n_layers, self.vocab_size, self.max_seq_len, self.ffn_hidden
         b = 0 if self.no_bias else 1
         w = self.qkv_dim
-        per_block = (2 * d) * 2 + (w * d + b * w) + (d * d + b * d) + (e * d * d + b * e * d) + (e * d * d + b * d)
+        per_block = (2 * d) * 2 + (w * d + b * w) + (d * d + b * d) + (f * d + b * f) + (f * d + b * d)
+        if self.ffn_gated:
+            per_block += f * d + b * f   # gate_proj
         if self.no_bias:
             per_block -= 2 * d  # LN biases dropped too
         return V * d + (S * d if self.learned_pos_emb else 0) + L * per_block + (2 * d if not self.no_bias else d)
@@ -129,6 +154,38 @@ class MPTConfig:
         """fwd+bwd model FLOPs per token as SpeedMonitor counts them: 6·N + 12·L·d·S."""
         s = seq_len or self.max_seq_len
         return 6.0 * self.num_params() + 12.0 * self.n_layers * self.d_model * s
+
+
+FFN_TYPES = ("mptmlp", "mptglu")
+FFN_ACTS = ("gelu", "silu")
+
+
+def parse_ffn_act(spec: dict[str, Any] | None) -> str:
+    """``ffn_config.ffn_act_fn`` (``{name: <torch.nn.functional name>, **kwargs}``, default exact GELU) -> "gelu" or "silu".
+    Anything else is refused rather than approximated."""
+    if spec is None:
+        return "gelu"
+    given, spec = dict(spec), dict(spec)
+    name = spec.pop("name", None)
+    if name == "gelu" and spec.pop("approximate", "none") == "none" and not spec:
+        return "gelu"
+    if name == "silu" and not spec.pop("inplace", False) and not spec:
+        return "silu"
+    raise ValueError(f"unsupported ffn_config.ffn_act_fn {given!r} (supported: {{name: gelu, approximate: none}}, "
+                     "{name: silu})")
+
+
+def ffn_act(x: torch.Tensor, name: str) -> torch.Tensor:
+    return F.silu(x) if name == "silu" else F.gelu(x)
+
+
+def nondefault_ffn(cfg: MPTConfig) -> bool:
+    """A feed-forward block other than llm-foundry's default ``mptmlp`` with exact GELU (the width does not count)."""
+    return cfg.ffn_type != "mptmlp" or cfg.ffn_act != "gelu"
+
+
+def ffn_desc(cfg: MPTConfig) -> str:
+    return f"ffn_config ffn_type={cfg.ffn_type} ffn_act_fn={cfg.ffn_act}"
 
 
 def alibi_slopes(n_heads: int, bias_max: int = 8) -> torch.Tensor:
@@ -206,14 +263,29 @@ class MPTAttention(nn.Module):
 
 
 class MPTMLP(nn.Module):
+    """``down_proj(act(up_proj(x)))`` at width ``cfg.ffn_hidden``."""
+
     def __init__(self, cfg: MPTConfig) -> None:
         super().__init__()
-        d = cfg.d_model
-        self.up_proj = nn.Linear(d, cfg.expansion_ratio * d, bias=not cfg.no_bias)
-        self.down_proj = nn.Linear(cfg.expansion_ratio * d, d, bias=not cfg.no_bias)
+        d, f = cfg.d_model, cfg.ffn_hidden
+        self.act = cfg.ffn_act
+        self.up_proj = nn.Linear(d, f, bias=not cfg.no_bias)
+        self.down_proj = nn.Linear(f, d, bias=not cfg.no_bias)
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        return self.down_proj(F.gelu(self.up_proj(x)))
+        return self.down_proj(ffn_act(self.up_proj(x), self.act))
+
+
+class MPTGLU(MPTMLP):
+    """``down_proj(act(gate_proj(x)) * up_proj(x))`` (llm-foundry ``mptglu``); ``gate_proj`` is registered after
+    ``up_proj`` / ``down_proj``, as there."""
+
+    def __init__(self, cfg: MPTConfig) -> None:
+        super().__init__(cfg)
+        self.gate_proj = nn.Linear(cfg.d_model, cfg.ffn_hidden, bias=not cfg.no_bias)
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        return self.down_proj(ffn_act(self.gate_proj(x), self.act) * self.up_proj(x))
 
 
 class MPTBlock(nn.Module):
@@ -222,7 +294,7 @@ class MPTBlock(nn.Module):
         self.norm_1 = nn.LayerNorm(cfg.d_model, eps=cfg.norm_eps, bias=not cfg.no_bias)
         self.attn = MPTAttention(cfg)
         self.norm_2 = nn.LayerNorm(cfg.d_model, eps=cfg.norm_eps, bias=not cfg.no_bias)
-        self.ffn = MPTMLP(cfg)
+        self.ffn = MPTGLU(cfg) if cfg.ffn_gated else MPTMLP(cfg)
 
     def forward(self, x: torch.Tensor, rope: Any, alibi: Any, doc_keep: Any = None) -> torch.Tensor:
         x = x + self.attn(self.norm_1(x).to(x.dtype), rope, alibi, doc_keep)

@@ -52,17 +52,19 @@ def add_launch_count(n: int) -> None:
 
 # --------------------------------------------------------------------------------- GEMM
 EPI_BF16, EPI_RESIDUAL, EPI_GELU_DUAL, EPI_DGELU, EPI_F32, EPI_GELU_GRAD, EPI_MUL, EPI_GELU_GRAD_Q8 = 0, 1, 2, 3, 4, 5, 6, 7
+EPI_SILU_GRAD, EPI_MUL2 = 8, 9
 E4M3, E5M2 = 0, 1          # operand formats of the fp8 wgmma GEMMs
 FP8_MAX = (448.0, 57344.0)
 
 
 def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False,
          epi: int = EPI_BF16, bias: torch.Tensor | None = None, aux: torch.Tensor | None = None,
-         out2: torch.Tensor | None = None, accumulate: bool = False, alpha: float = 1.0, cluster: int = 0) -> torch.Tensor:
+         out2: torch.Tensor | None = None, accumulate: bool = False, alpha: float = 1.0, cluster: int = 0,
+         aux2: torch.Tensor | None = None) -> torch.Tensor:
     """``out[M,N] = epilogue(alpha * A @ B^T)`` on wgmma tensor cores.
 
     ``a``: ``[M,K]`` (K-major) or ``[K,M]`` when ``a_mn``; ``b``: ``[N,K]`` or ``[K,N]`` when ``b_mn``."""
-    ext().gemm(a, b, out, int(a_mn), int(b_mn), int(epi), bias, aux, out2, bool(accumulate), float(alpha), int(cluster))
+    ext().gemm(a, b, out, int(a_mn), int(b_mn), int(epi), bias, aux, out2, bool(accumulate), float(alpha), int(cluster), aux2)
     return out
 
 
@@ -85,10 +87,42 @@ def linear_gelu_grad_fwd(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | 
     return gemm(x, w, act, epi=EPI_GELU_GRAD, bias=bias, out2=dact)
 
 
+def linear_silu_grad_fwd(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None, dact: torch.Tensor,
+                         act: torch.Tensor) -> torch.Tensor:
+    """z = x @ w^T + bias ; act = silu(z) = z·σ(z) ; dact = silu'(z) = σ(z)·(1 + z·(1 − σ(z))) — :func:`linear_gelu_grad_fwd`
+    with SiLU (one exp per element for both)."""
+    return gemm(x, w, act, epi=EPI_SILU_GRAD, bias=bias, out2=dact)
+
+
+def linear_act_grad_fwd(act_name: str, x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None, dact: torch.Tensor,
+                        act: torch.Tensor) -> torch.Tensor:
+    """:func:`linear_gelu_grad_fwd` (``act_name`` "gelu") or :func:`linear_silu_grad_fwd` ("silu")."""
+    f = linear_silu_grad_fwd if act_name == "silu" else linear_gelu_grad_fwd
+    return f(x, w, bias, dact, act)
+
+
+def linear_glu_up_fwd(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None, act: torch.Tensor, dact: torch.Tensor,
+                      m: torch.Tensor, c: torch.Tensor) -> torch.Tensor:
+    """Up projection of a gated FFN: u = x @ w^T + bias ; m = u * act ; c = u * dact (``act`` / ``dact`` = act(g) / act'(g) of
+    the gate projection g). ``m`` is the down projection's input, ``c`` the saved factor of the gate's gradient. The
+    outputs must not overlap the multipliers."""
+    return gemm(x, w, m, epi=EPI_MUL2, bias=bias, aux=act, aux2=dact, out2=c)
+
+
+def linear_glu_dgrad(dm: torch.Tensor, w: torch.Tensor, act: torch.Tensor, c: torch.Tensor, du: torch.Tensor,
+                     dg: torch.Tensor) -> torch.Tensor:
+    """dgrad of a gated FFN's down projection: dm' = dm @ w (w stored [N,K], consumed MN-major) ; du = dm' * act(g) ;
+    dg = dm' * c (c = u * act'(g) saved by :func:`linear_glu_up_fwd`): the gradients of the up and gate projections'
+    outputs. The outputs must not overlap the multipliers."""
+    return gemm(dm, w, du, b_mn=True, epi=EPI_MUL2, aux=act, aux2=c, out2=dg)
+
+
 def linear_dgrad(dy: torch.Tensor, w: torch.Tensor, dx: torch.Tensor, gelu_pre: torch.Tensor | None = None,
-                 mul: torch.Tensor | None = None) -> torch.Tensor:
-    """dx = dy @ w  (w stored [N,K] → consumed MN-major, no transpose); optional ``* gelu'(pre)`` (pre-activation given)
-    or ``* mul`` (saved derivative given)."""
+                 mul: torch.Tensor | None = None, residual: torch.Tensor | None = None) -> torch.Tensor:
+    """dx = dy @ w  (w stored [N,K] → consumed MN-major, no transpose); optional ``* gelu'(pre)`` (pre-activation given),
+    ``* mul`` (saved derivative given) or ``+ residual`` (another input gradient to add; not ``dx`` itself)."""
+    if residual is not None:
+        return gemm(dy, w, dx, b_mn=True, epi=EPI_RESIDUAL, aux=residual)
     if mul is not None:
         return gemm(dy, w, dx, b_mn=True, epi=EPI_MUL, aux=mul)
     return gemm(dy, w, dx, b_mn=True, epi=EPI_DGELU if gelu_pre is not None else EPI_BF16, aux=gelu_pre)
@@ -299,15 +333,19 @@ def rope_(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_heads: int,
 
 
 # ---------------------------------------------------------------------------- decoding
-SKINNY_PLAIN, SKINNY_RESIDUAL, SKINNY_GELU = 0, 1, 2
+SKINNY_PLAIN, SKINNY_RESIDUAL, SKINNY_GELU, SKINNY_SILU, SKINNY_MUL = 0, 1, 2, 3, 4
 
 
 def skinny_gemm(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor, bias: torch.Tensor | None = None,
-                residual: torch.Tensor | None = None, gelu: bool = False) -> torch.Tensor:
-    """``out[M,N] = x[M,K] @ w[N,K]^T (+ bias) (+ residual | then exact GELU)`` for 1 <= M <= 64 rows (decode steps): the weight
-    rows stream through the GPU once, K is split when the 64-column tiles cannot fill it, and split partials are summed in a
-    fixed order, so the result is bitwise reproducible."""
-    epi = SKINNY_GELU if gelu else (SKINNY_RESIDUAL if residual is not None else SKINNY_PLAIN)
+                residual: torch.Tensor | None = None, gelu: bool = False, silu: bool = False,
+                mul: torch.Tensor | None = None) -> torch.Tensor:
+    """``out[M,N] = x[M,K] @ w[N,K]^T (+ bias) (+ residual | then exact GELU | then SiLU | then * mul)`` for 1 <= M <= 64 rows
+    (decode steps): the weight rows stream through the GPU once, K is split when the 64-column tiles cannot fill it, and split
+    partials are summed in a fixed order, so the result is bitwise reproducible."""
+    if mul is not None:
+        epi, residual = SKINNY_MUL, mul
+    else:
+        epi = SKINNY_GELU if gelu else SKINNY_SILU if silu else (SKINNY_RESIDUAL if residual is not None else SKINNY_PLAIN)
     ext().skinny_gemm(x, w, out, bias, residual, epi)
     return out
 

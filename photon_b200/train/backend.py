@@ -27,7 +27,7 @@ from typing import Any
 import torch
 import torch.nn.functional as F
 
-from photon_b200.models.mpt import MPTConfig, MPTForCausalLM, check_sequence_id, shift_labels
+from photon_b200.models.mpt import MPTConfig, MPTForCausalLM, check_sequence_id, ffn_desc, nondefault_ffn, shift_labels
 from photon_b200.utils.flat import FlatParams
 
 
@@ -162,6 +162,9 @@ def build_backend(model_cfg: MPTConfig, device: torch.device, precision: str, ke
             unsupported.append(f"precision={precision}")
         if (kw.get("frozen_layers") or kw.get("unfrozen_layers")) and kw.get("zero3") is not None:
             unsupported.append("frozen/unfrozen layers")   # the ZeRO-3 unit plan assumes every block tensor is in the flat
+        if nondefault_ffn(model_cfg) and (precision == "amp_fp8" or kw.get("zero3") is not None):
+            # the fp8 weight roles, the fp8 GELU epilogue and the ZeRO-3 unit plan know the four mptmlp block matrices only
+            unsupported.append(f"{ffn_desc(model_cfg)} with {'amp_fp8' if precision == 'amp_fp8' else 'full parameter sharding'}")
         if unsupported:
             print(f"[backend] {', '.join(unsupported)} not covered by the sm_90a engine -> stock PyTorch backend "
                   "(explicit, logged; set kernels.*=torch to silence)", flush=True)
