@@ -190,33 +190,48 @@ void gemm_mxfp8(const Tensor& a8, const Tensor& b8, Tensor& d, const Tensor& sfa
   pb::gemm_mxfp8_launch(a8.data_ptr(), b8.data_ptr(), d.data_ptr(), sfa.data_ptr(), sfb.data_ptr(), opt_ptr<float>(bias), M, N, K,
                         d.stride(0), num_sms(), stream_of(a8));
 }
-void layernorm_fwd_q8(const Tensor& x, const Tensor& gamma, const c10::optional<Tensor>& beta, Tensor& y8, Tensor& mean, Tensor& rstd,
-                      double eps, Tensor& meta, int role) {
+// the checks of layernorm_fwd_q8 / rmsnorm_fwd_q8 (`mean` is null for RMSNorm); returns meta's role count
+int64_t check_norm_fwd_q8(const char* op, const Tensor& x, const Tensor& gamma, const c10::optional<Tensor>& beta, const Tensor& y8,
+                          const Tensor* mean, const Tensor& rstd, const Tensor& meta, int role) {
   check_bf16(x, "x");
   check_f32(gamma, "gamma");
   check_f32(meta, "meta");
-  TORCH_CHECK(x.is_contiguous() && y8.is_contiguous() && is_byte(y8) && y8.numel() == x.numel(), "layernorm_fwd_q8: y8 must be a contiguous 1-byte tensor shaped like x");
+  TORCH_CHECK(x.is_contiguous() && y8.is_contiguous() && is_byte(y8) && y8.numel() == x.numel(), op, ": y8 must be a contiguous 1-byte tensor shaped like x");
   const int64_t nr = meta.size(1);
   TORCH_CHECK(meta.dim() == 2 && meta.size(0) == 3 && role >= 0 && role < nr, "bad meta / role");
   const int d = int(x.size(-1));
   const int64_t T = x.numel() / d;
-  check_f32(mean, "mean");
+  if (mean) check_f32(*mean, "mean");
   check_f32(rstd, "rstd");
-  check_numel(gamma, d, "layernorm_fwd_q8", "gamma");
-  check_numel(mean, T, "layernorm_fwd_q8", "mean");
-  check_numel(rstd, T, "layernorm_fwd_q8", "rstd");
-  check_vec(x, "layernorm_fwd_q8", "x");
-  check_vec(gamma, "layernorm_fwd_q8", "gamma");
-  check_vec(y8, "layernorm_fwd_q8", "y8", 8);
+  check_numel(gamma, d, op, "gamma");
+  if (mean) check_numel(*mean, T, op, "mean");
+  check_numel(rstd, T, op, "rstd");
+  check_vec(x, op, "x");
+  check_vec(gamma, op, "gamma");
+  check_vec(y8, op, "y8", 8);
   if (beta.has_value()) {
     check_f32(*beta, "beta");
-    check_numel(*beta, d, "layernorm_fwd_q8", "beta");
-    check_vec(*beta, "layernorm_fwd_q8", "beta");
+    check_numel(*beta, d, op, "beta");
+    check_vec(*beta, op, "beta");
   }
+  return nr;
+}
+void layernorm_fwd_q8(const Tensor& x, const Tensor& gamma, const c10::optional<Tensor>& beta, Tensor& y8, Tensor& mean, Tensor& rstd,
+                      double eps, Tensor& meta, int role) {
+  const int64_t nr = check_norm_fwd_q8("layernorm_fwd_q8", x, gamma, beta, y8, &mean, rstd, meta, role);
+  const int d = int(x.size(-1));
   c10::cuda::CUDAGuard guard(x.device());
   float* m = meta.data_ptr<float>();
   pb::layernorm_fwd_q8(x.data_ptr(), gamma.data_ptr<float>(), opt_ptr<float>(beta), y8.data_ptr(),
                        mean.data_ptr<float>(), rstd.data_ptr<float>(), x.numel() / d, d, float(eps), m + role, m + 2 * nr + role, stream_of(x));
+}
+void rmsnorm_fwd_q8(const Tensor& x, const Tensor& gamma, Tensor& y8, Tensor& rstd, double eps, Tensor& meta, int role) {
+  const int64_t nr = check_norm_fwd_q8("rmsnorm_fwd_q8", x, gamma, c10::nullopt, y8, nullptr, rstd, meta, role);
+  const int d = int(x.size(-1));
+  c10::cuda::CUDAGuard guard(x.device());
+  float* m = meta.data_ptr<float>();
+  pb::rmsnorm_fwd_q8(x.data_ptr(), gamma.data_ptr<float>(), y8.data_ptr(), rstd.data_ptr<float>(), x.numel() / d, d, float(eps), m + role,
+                     m + 2 * nr + role, stream_of(x));
 }
 // out_sum[j] += sum_t dy[t,j] and / or y8 = fp8(dy * scale[role]) with amax[role] updated — one read of dy
 void colsum_quant(const Tensor& dy, c10::optional<Tensor> out_sum, c10::optional<Tensor> y8, int fmt, c10::optional<Tensor> meta, int role) {
@@ -592,21 +607,22 @@ void transpose_u8(const Tensor& src, Tensor& dst) {
   c10::cuda::CUDAGuard guard(src.device());
   pb::transpose_u8(src.data_ptr(), src.stride(0), dst.data_ptr(), int(src.size(0)), int(src.size(1)), stream_of(src));
 }
-// gamma / beta: fp32 [d]; mean / rstd: fp32 [T] with T = x.numel() / d; y / dx / dres shaped like x
-void check_layernorm(const char* op, const Tensor& x, const Tensor& gamma, const c10::optional<Tensor>& beta, const Tensor& mean,
+// gamma / beta: fp32 [d]; mean / rstd: fp32 [T] with T = x.numel() / d; y / dx / dres shaped like x. `mean` is null for RMSNorm.
+void check_layernorm(const char* op, const Tensor& x, const Tensor& gamma, const c10::optional<Tensor>& beta, const Tensor* mean,
                      const Tensor& rstd) {
   check_bf16(x, "x");
   check_f32(gamma, "gamma");
-  check_f32(mean, "mean");
+  if (mean) check_f32(*mean, "mean");
   check_f32(rstd, "rstd");
   TORCH_CHECK(x.dim() >= 1 && x.is_contiguous(), op, ": x must be contiguous");
   const int64_t d = x.size(-1);
   TORCH_CHECK(d > 0, op, ": empty rows");
   const int64_t T = x.numel() / d;
   check_numel(gamma, d, op, "gamma");
-  check_numel(mean, T, op, "mean");
+  if (mean) check_numel(*mean, T, op, "mean");
   check_numel(rstd, T, op, "rstd");
-  TORCH_CHECK(gamma.is_contiguous() && mean.is_contiguous() && rstd.is_contiguous(), op, ": gamma, mean and rstd must be contiguous");
+  TORCH_CHECK(gamma.is_contiguous() && (!mean || mean->is_contiguous()) && rstd.is_contiguous(), op,
+              ": gamma, mean and rstd must be contiguous");
   check_vec(x, op, "x");
   check_vec(gamma, op, "gamma");
   if (beta.has_value()) {
@@ -623,7 +639,7 @@ void check_like_x(const char* op, const Tensor& t, const Tensor& x, const char* 
 }
 void layernorm_fwd(const Tensor& x, const Tensor& gamma, const c10::optional<Tensor>& beta, Tensor& y, Tensor& mean, Tensor& rstd,
                    double eps) {
-  check_layernorm("layernorm_fwd", x, gamma, beta, mean, rstd);
+  check_layernorm("layernorm_fwd", x, gamma, beta, &mean, rstd);
   check_like_x("layernorm_fwd", y, x, "y");
   c10::cuda::CUDAGuard guard(x.device());
   const int d = int(x.size(-1));
@@ -632,7 +648,7 @@ void layernorm_fwd(const Tensor& x, const Tensor& gamma, const c10::optional<Ten
 }
 void layernorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& gamma, const Tensor& mean, const Tensor& rstd,
                    const c10::optional<Tensor>& dres, Tensor& dx, c10::optional<Tensor> dgamma, c10::optional<Tensor> dbeta) {
-  check_layernorm("layernorm_bwd", x, gamma, c10::nullopt, mean, rstd);
+  check_layernorm("layernorm_bwd", x, gamma, c10::nullopt, &mean, rstd);
   check_like_x("layernorm_bwd", dy, x, "dy");
   check_like_x("layernorm_bwd", dx, x, "dx");
   if (dres.has_value()) check_like_x("layernorm_bwd", *dres, x, "dres");
@@ -646,6 +662,29 @@ void layernorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& gamma, const
   c10::cuda::CUDAGuard guard(x.device());
   pb::layernorm_bwd(dy.data_ptr(), x.data_ptr(), gamma.data_ptr<float>(), mean.data_ptr<float>(), rstd.data_ptr<float>(), opt_ptr(dres),
                     dx.data_ptr(), opt_ptr<float>(dgamma), opt_ptr<float>(dbeta), x.numel() / d, d, stream_of(x));
+}
+void rmsnorm_fwd(const Tensor& x, const Tensor& gamma, Tensor& y, Tensor& rstd, double eps) {
+  check_layernorm("rmsnorm_fwd", x, gamma, c10::nullopt, nullptr, rstd);
+  check_like_x("rmsnorm_fwd", y, x, "y");
+  c10::cuda::CUDAGuard guard(x.device());
+  const int d = int(x.size(-1));
+  pb::rmsnorm_fwd(x.data_ptr(), gamma.data_ptr<float>(), y.data_ptr(), rstd.data_ptr<float>(), x.numel() / d, d, float(eps), stream_of(x));
+}
+void rmsnorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& gamma, const Tensor& rstd, const c10::optional<Tensor>& dres, Tensor& dx,
+                 c10::optional<Tensor> dgamma) {
+  check_layernorm("rmsnorm_bwd", x, gamma, c10::nullopt, nullptr, rstd);
+  check_like_x("rmsnorm_bwd", dy, x, "dy");
+  check_like_x("rmsnorm_bwd", dx, x, "dx");
+  if (dres.has_value()) check_like_x("rmsnorm_bwd", *dres, x, "dres");
+  const int d = int(x.size(-1));
+  if (dgamma.has_value()) {
+    check_f32(*dgamma, "dgamma");
+    check_numel(*dgamma, d, "rmsnorm_bwd", "dgamma");
+    TORCH_CHECK(dgamma->is_contiguous(), "rmsnorm_bwd: dgamma must be contiguous");
+  }
+  c10::cuda::CUDAGuard guard(x.device());
+  pb::rmsnorm_bwd(dy.data_ptr(), x.data_ptr(), gamma.data_ptr<float>(), rstd.data_ptr<float>(), opt_ptr(dres), dx.data_ptr(),
+                  opt_ptr<float>(dgamma), x.numel() / d, d, stream_of(x));
 }
 void col_sum(const Tensor& dy, Tensor& out) {
   check_bf16(dy, "dy");
@@ -946,6 +985,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("d2") = py::none(), py::arg("accumulate") = false, py::arg("alpha") = 1.0, py::arg("cluster") = 0,
         py::arg("d8") = py::none(), py::arg("role_out") = -1);
   m.def("layernorm_fwd_q8", &layernorm_fwd_q8);
+  m.def("rmsnorm_fwd_q8", &rmsnorm_fwd_q8);
   m.def("mx_quantize", &mx_quantize, py::arg("x"), py::arg("rblk") = 0);
   m.def("gemm_mxfp8", &gemm_mxfp8, py::arg("a8"), py::arg("b8"), py::arg("d"), py::arg("sfa"), py::arg("sfb"), py::arg("bias") = py::none());
   m.def("colsum_quant", &colsum_quant, py::arg("dy"), py::arg("out_sum") = py::none(), py::arg("y8") = py::none(), py::arg("fmt") = 1,
@@ -974,6 +1014,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("transpose_u8", &transpose_u8);
   m.def("layernorm_fwd", &layernorm_fwd);
   m.def("layernorm_bwd", &layernorm_bwd);
+  m.def("rmsnorm_fwd", &rmsnorm_fwd);
+  m.def("rmsnorm_bwd", &rmsnorm_bwd);
   m.def("col_sum", &col_sum);
   m.def("cross_entropy", &cross_entropy);
   m.def("flat_l2_norm", &flat_l2_norm);

@@ -4,7 +4,8 @@
 // E4M3, gradients flowing backward to E5M2; every cast multiplies by the tensor role's scale and saturates; the GEMM epilogue
 // multiplies by 1/(scale_a * scale_b). Nothing here makes an extra pass over an activation just to quantise it:
 //
-//   * ln_fwd_q8_kernel        LayerNorm forward whose ONLY output is the E4M3 tensor the next GEMM (and the wgrad) reads
+//   * ln_fwd_q8_kernel        LayerNorm (or, RMS instance, RMSNorm) forward whose ONLY output is the E4M3 tensor the next GEMM
+//                             (and the wgrad) reads
 //   * colsum_quant_kernel     bias-gradient column sums and the E5M2 copy of dY for dgrad / wgrad from the same read of dY
 //   * (csrc/gemm_tcgen05.cu)  EPI_GELU_GRAD_Q8 writes gelu(z) as E4M3 from the up-projection's epilogue
 //   * seg_amax / seg_quant    the four weight matrices of every block, E4M3 with CURRENT scaling, from the bf16 shadow
@@ -35,8 +36,9 @@ __device__ __forceinline__ float warp_sum_f(float v) {
   return v;
 }
 
-// ------------------------------------------------------------------ LayerNorm forward -> E4M3 (one warp per row)
-template <int LN_NCH>
+// ------------------------------------------------------------------ LayerNorm / RMSNorm forward -> E4M3 (one warp per row)
+// RMS: no mean (not written, may be null) and no beta, as in csrc/fused_ops.cu's ln_fwd_kernel.
+template <int LN_NCH, bool RMS>
 __global__ void __launch_bounds__(256) ln_fwd_q8_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ gamma,
                                                          const float* __restrict__ beta, uint8_t* __restrict__ y8,
                                                          float* __restrict__ mean, float* __restrict__ rstd, long long T, int d,
@@ -58,24 +60,31 @@ __global__ void __launch_bounds__(256) ln_fwd_q8_kernel(const __nv_bfloat16* __r
         float f[8];
         unpack8f(buf[c], f);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) sum += f[k];
+        for (int k = 0; k < 8; ++k) {
+          if constexpr (RMS) sum += f[k] * f[k];
+          else sum += f[k];
+        }
       }
     }
-    const float mu = warp_sum_f(sum) / d;
-    float ss = 0.f;
+    float mu = 0.f, var = warp_sum_f(sum) / d;   // var: mean(x^2) for RMS, otherwise mean(x) until the second pass
+    if constexpr (!RMS) {
+      mu = var;
+      float ss = 0.f;
 #pragma unroll
-    for (int c = 0; c < LN_NCH; ++c) {
-      const int e = c * 256 + lane * 8;
-      if (e < d) {
-        float f[8];
-        unpack8f(buf[c], f);
+      for (int c = 0; c < LN_NCH; ++c) {
+        const int e = c * 256 + lane * 8;
+        if (e < d) {
+          float f[8];
+          unpack8f(buf[c], f);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) ss += (f[k] - mu) * (f[k] - mu);
+          for (int k = 0; k < 8; ++k) ss += (f[k] - mu) * (f[k] - mu);
+        }
       }
+      var = warp_sum_f(ss) / d;
     }
-    const float rs = rsqrtf(warp_sum_f(ss) / d + eps);
+    const float rs = rsqrtf(var + eps);
     if (lane == 0) {
-      mean[row] = mu;
+      if constexpr (!RMS) mean[row] = mu;
       rstd[row] = rs;
     }
     uint2* yr = reinterpret_cast<uint2*>(y8 + row * d);
@@ -86,12 +95,17 @@ __global__ void __launch_bounds__(256) ln_fwd_q8_kernel(const __nv_bfloat16* __r
         float f[8];
         unpack8f(buf[c], f);
         const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma + e)), g1 = __ldg(reinterpret_cast<const float4*>(gamma + e + 4));
-        float4 b0 = make_float4(0, 0, 0, 0), b1 = b0;
-        if (beta) b0 = __ldg(reinterpret_cast<const float4*>(beta + e)), b1 = __ldg(reinterpret_cast<const float4*>(beta + e + 4));
         const float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-        const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+        if constexpr (RMS) {
 #pragma unroll
-        for (int k = 0; k < 8; ++k) f[k] = (f[k] - mu) * rs * g[k] + b[k];
+          for (int k = 0; k < 8; ++k) f[k] = f[k] * rs * g[k];
+        } else {
+          float4 b0 = make_float4(0, 0, 0, 0), b1 = b0;
+          if (beta) b0 = __ldg(reinterpret_cast<const float4*>(beta + e)), b1 = __ldg(reinterpret_cast<const float4*>(beta + e + 4));
+          const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+          for (int k = 0; k < 8; ++k) f[k] = (f[k] - mu) * rs * g[k] + b[k];
+        }
         am = amax8(f, am);
         yr[c * 32 + lane] = quant8<0>(f, s);
       }
@@ -238,16 +252,27 @@ __global__ void update_scales_kernel(float* __restrict__ scale, float* __restric
   if (threadIdx.x == 0) *pos = *pos + 1;
 }
 
+template <bool RMS>
+void norm_fwd_q8(const void* x, const float* gamma, const float* beta, void* y8, float* mean, float* rstd, long long T, int d, float eps,
+                 const float* scale, float* amax, cudaStream_t st) {
+  const char* name = RMS ? "rmsnorm_fwd_q8" : "layernorm_fwd_q8";
+  if (d % 8 || d > 16 * 256) throw std::runtime_error(std::string(name) + ": d must be a multiple of 8 and <= 4096");
+  with_ln_chunks((d + 255) / 256, [&](auto N) {
+    ln_fwd_q8_kernel<N, RMS><<<int((T + 7) / 8), 256, 0, st>>>((const __nv_bfloat16*)x, gamma, beta, (uint8_t*)y8, mean, rstd, T, d, eps,
+                                                               scale, amax);
+  });
+  launched(name);
+}
+
 }  // namespace
 
 void layernorm_fwd_q8(const void* x, const float* gamma, const float* beta, void* y8, float* mean, float* rstd, long long T, int d,
                       float eps, const float* scale, float* amax, cudaStream_t st) {
-  if (d % 8 || d > 16 * 256) throw std::runtime_error("layernorm_fwd_q8: d must be a multiple of 8 and <= 4096");
-  with_ln_chunks((d + 255) / 256, [&](auto N) {
-    ln_fwd_q8_kernel<N><<<int((T + 7) / 8), 256, 0, st>>>((const __nv_bfloat16*)x, gamma, beta, (uint8_t*)y8, mean, rstd, T, d, eps, scale,
-                                                          amax);
-  });
-  launched("layernorm_fwd_q8");
+  norm_fwd_q8<false>(x, gamma, beta, y8, mean, rstd, T, d, eps, scale, amax, st);
+}
+void rmsnorm_fwd_q8(const void* x, const float* gamma, void* y8, float* rstd, long long T, int d, float eps, const float* scale, float* amax,
+                    cudaStream_t st) {
+  norm_fwd_q8<true>(x, gamma, nullptr, y8, nullptr, rstd, T, d, eps, scale, amax, st);
 }
 
 void colsum_quant(const void* dy, long long ld, float* out_sum, void* y8, long long ld8, int fmt, const float* scale, float* amax,

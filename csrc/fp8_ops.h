@@ -9,6 +9,9 @@ namespace pb {
 // y8[T,d] = e4m3(layernorm(x) * *scale); *amax = max(*amax, max|layernorm(x)|); mean / rstd saved for the backward
 void layernorm_fwd_q8(const void* x, const float* gamma, const float* beta, void* y8, float* mean, float* rstd, long long T, int d,
                       float eps, const float* scale, float* amax, cudaStream_t st);
+// the same for RMSNorm (no beta, no mean): y8 = e4m3(x * rstd * gamma * *scale)
+void rmsnorm_fwd_q8(const void* x, const float* gamma, void* y8, float* rstd, long long T, int d, float eps, const float* scale, float* amax,
+                    cudaStream_t st);
 // out_sum[j] += sum_t dy[t,j] (may be null);  y8[t,j] = fp8(dy[t,j] * *scale) (may be null), fmt 0 = E4M3, 1 = E5M2
 void colsum_quant(const void* dy, long long ld, float* out_sum, void* y8, long long ld8, int fmt, const float* scale, float* amax,
                   long long T, int d, cudaStream_t st);

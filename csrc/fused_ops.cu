@@ -1,6 +1,6 @@
 // Memory-bound fused kernels of the MPT training step for sm_90a (everything that is not a GEMM or
-// attention): embedding gather/scatter, LayerNorm fwd/bwd (+residual-gradient add), column reductions for
-// bias / LN-affine gradients, fused cross-entropy (loss + in-place dlogits), flat-buffer L2 norm,
+// attention): embedding gather/scatter, LayerNorm / RMSNorm fwd/bwd (+residual-gradient add), column reductions for
+// bias / norm-affine gradients, fused cross-entropy (loss + in-place dlogits), flat-buffer L2 norm,
 // ADOPT / DecoupledAdamW multi-tensor step with bf16 shadow emit, axpby for the streaming client mean.
 // All are 128-bit vectorised, one pass over HBM; they replace the ATen kernel sequences the reference
 // reaches through torch (SURVEY §2.5 K1, K2, K9, K11, K12, K14).
@@ -109,10 +109,12 @@ __global__ void embed_bwd_wpe_kernel(const __nv_bfloat16* __restrict__ dh, float
   }
 }
 
-// ------------------------------------------------------------------ LayerNorm (one warp per row, row in registers)
+// ------------------------------------------------------------------ LayerNorm / RMSNorm (one warp per row, row in registers)
+// Every row kernel below has an RMS instance (template flag RMS): no mean (xhat = x * rstd, rstd = rsqrt(mean(x^2) + eps)),
+// no beta / dbeta, and a dx without the mean(dy*g) term. mean is neither read nor written there (it may be null).
 constexpr int LN_MAXCH = 16;  // 16 chunks x 32 lanes x 8 elems = d <= 4096
 
-template <int LN_NCH>
+template <int LN_NCH, bool RMS>
 __global__ void __launch_bounds__(256) ln_fwd_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ gamma,
                                                       const float* __restrict__ beta, __nv_bfloat16* __restrict__ y,
                                                       float* __restrict__ mean, float* __restrict__ rstd, long long T,
@@ -131,24 +133,31 @@ __global__ void __launch_bounds__(256) ln_fwd_kernel(const __nv_bfloat16* __rest
       float f[8];
       unpack8(buf[c], f);
 #pragma unroll
-      for (int k = 0; k < 8; ++k) s += f[k];
+      for (int k = 0; k < 8; ++k) {
+        if constexpr (RMS) s += f[k] * f[k];
+        else s += f[k];
+      }
     }
   }
-  const float mu = warp_sum(s) / d;
-  float ss = 0.f;
+  float mu = 0.f, var = warp_sum(s) / d;   // var: mean(x^2) for RMS, otherwise mean(x) until the second pass
+  if constexpr (!RMS) {
+    mu = var;
+    float ss = 0.f;
 #pragma unroll
-  for (int c = 0; c < LN_NCH; ++c) {
-    const int e = c * 256 + lane * 8;
-    if (e < d) {
-      float f[8];
-      unpack8(buf[c], f);
+    for (int c = 0; c < LN_NCH; ++c) {
+      const int e = c * 256 + lane * 8;
+      if (e < d) {
+        float f[8];
+        unpack8(buf[c], f);
 #pragma unroll
-      for (int k = 0; k < 8; ++k) ss += (f[k] - mu) * (f[k] - mu);
+        for (int k = 0; k < 8; ++k) ss += (f[k] - mu) * (f[k] - mu);
+      }
     }
+    var = warp_sum(ss) / d;
   }
-  const float rs = rsqrtf(warp_sum(ss) / d + eps);
+  const float rs = rsqrtf(var + eps);
   if (lane == 0) {
-    mean[row] = mu;
+    if constexpr (!RMS) mean[row] = mu;
     rstd[row] = rs;
   }
   uint4* yr = reinterpret_cast<uint4*>(y + row * d);
@@ -159,19 +168,25 @@ __global__ void __launch_bounds__(256) ln_fwd_kernel(const __nv_bfloat16* __rest
       float f[8];
       unpack8(buf[c], f);
       const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma + e)), g1 = __ldg(reinterpret_cast<const float4*>(gamma + e + 4));
-      float4 b0 = make_float4(0, 0, 0, 0), b1 = b0;
-      if (beta) b0 = __ldg(reinterpret_cast<const float4*>(beta + e)), b1 = __ldg(reinterpret_cast<const float4*>(beta + e + 4));
       const float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-      const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+      if constexpr (RMS) {
 #pragma unroll
-      for (int k = 0; k < 8; ++k) f[k] = (f[k] - mu) * rs * g[k] + b[k];
+        for (int k = 0; k < 8; ++k) f[k] = f[k] * rs * g[k];
+      } else {
+        float4 b0 = make_float4(0, 0, 0, 0), b1 = b0;
+        if (beta) b0 = __ldg(reinterpret_cast<const float4*>(beta + e)), b1 = __ldg(reinterpret_cast<const float4*>(beta + e + 4));
+        const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+        for (int k = 0; k < 8; ++k) f[k] = (f[k] - mu) * rs * g[k] + b[k];
+      }
       yr[c * 32 + lane] = pack8(f);
     }
   }
 }
 
 // dx = rstd * (dy*g - mean(dy*g) - xhat * mean(dy*g*xhat))  [+ dres]   (row-wise part of LN backward)
-template <int LN_NCH>
+// RMS: dx = rstd * (dy*g - xhat * mean(dy*g*xhat))  [+ dres]
+template <int LN_NCH, bool RMS>
 __global__ void __launch_bounds__(256) ln_bwd_dx_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
                                                          const float* __restrict__ gamma, const float* __restrict__ mean,
                                                          const float* __restrict__ rstd, const __nv_bfloat16* __restrict__ dres,
@@ -181,7 +196,7 @@ __global__ void __launch_bounds__(256) ln_bwd_dx_kernel(const __nv_bfloat16* __r
   if (row >= T) return;
   const uint4* xr = reinterpret_cast<const uint4*>(x + row * d);
   const uint4* gr = reinterpret_cast<const uint4*>(dy + row * d);
-  const float mu = mean[row], rs = rstd[row];
+  const float mu = RMS ? 0.f : mean[row], rs = rstd[row];
   uint4 bx[LN_NCH], bg[LN_NCH];
   float c1 = 0.f, c2 = 0.f;
 #pragma unroll
@@ -198,12 +213,12 @@ __global__ void __launch_bounds__(256) ln_bwd_dx_kernel(const __nv_bfloat16* __r
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
         const float dxh = fg[k] * g[k];
-        c1 += dxh;
+        if constexpr (!RMS) c1 += dxh;
         c2 += dxh * (fx[k] - mu) * rs;
       }
     }
   }
-  c1 = warp_sum(c1) / d;
+  if constexpr (!RMS) c1 = warp_sum(c1) / d;
   c2 = warp_sum(c2) / d;
   uint4* outr = reinterpret_cast<uint4*>(dx + row * d);
   const uint4* rr = dres ? reinterpret_cast<const uint4*>(dres + row * d) : nullptr;
@@ -230,7 +245,8 @@ __global__ void __launch_bounds__(256) ln_bwd_dx_kernel(const __nv_bfloat16* __r
 // Same row-wise dx, plus the column reductions dbeta[j] += sum_t dy[t,j], dgamma[j] += sum_t dy[t,j] * xhat[t,j] in the SAME
 // pass (persistent warps keep per-lane column partials in registers; one smem reduction + one atomicAdd per column per
 // block at the end). Saves the second read of dy and x that a separate column-reduce kernel needs. d <= 1024.
-template <int LN_NCH>
+// RMS: the dx above, and dgamma only.
+template <int LN_NCH, bool RMS>
 __global__ void __launch_bounds__(256, 2) ln_bwd_fused_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
                                                             const float* __restrict__ gamma, const float* __restrict__ mean,
                                                             const float* __restrict__ rstd, const __nv_bfloat16* __restrict__ dres,
@@ -257,7 +273,7 @@ __global__ void __launch_bounds__(256, 2) ln_bwd_fused_kernel(const __nv_bfloat1
   for (long long row = (long long)blockIdx.x * 8 + w; row < T; row += nwarps) {
     const uint4* xr = reinterpret_cast<const uint4*>(x + row * d);
     const uint4* gr = reinterpret_cast<const uint4*>(dy + row * d);
-    const float mu = mean[row], rs = rstd[row];
+    const float mu = RMS ? 0.f : mean[row], rs = rstd[row];
     uint4 bx[LN_NCH], bg[LN_NCH];
     float c1 = 0.f, c2 = 0.f;
 #pragma unroll
@@ -280,13 +296,12 @@ __global__ void __launch_bounds__(256, 2) ln_bwd_fused_kernel(const __nv_bfloat1
       for (int k = 0; k < 8; ++k) {
         const float xh = (fx[k] - mu) * rs;
         const float dxh = fg[k] * g[k];
-        c1 += dxh;
+        if constexpr (!RMS) c1 += dxh, ab[c][k] += fg[k];
         c2 += dxh * xh;
-        ab[c][k] += fg[k];
         ag[c][k] += fg[k] * xh;
       }
     }
-    c1 = warp_sum(c1) / d;
+    if constexpr (!RMS) c1 = warp_sum(c1) / d;
     c2 = warp_sum(c2) / d;
     uint4* outr = reinterpret_cast<uint4*>(dx + row * d);
     const uint4* rr = dres ? reinterpret_cast<const uint4*>(dres + row * d) : nullptr;
@@ -308,9 +323,9 @@ __global__ void __launch_bounds__(256, 2) ln_bwd_fused_kernel(const __nv_bfloat1
       }
     }
   }
-  // block reduction of the column partials: dbeta then dgamma through the same smem
+  // block reduction of the column partials: dbeta (not for RMS) then dgamma through the same smem
 #pragma unroll
-  for (int pass = 0; pass < 2; ++pass) {
+  for (int pass = RMS ? 1 : 0; pass < 2; ++pass) {
     __syncthreads();
 #pragma unroll
     for (int c = 0; c < LN_NCH; ++c)
@@ -330,7 +345,9 @@ __global__ void __launch_bounds__(256, 2) ln_bwd_fused_kernel(const __nv_bfloat1
 }
 
 // Column reductions over rows: out_sum[j] += sum_t dy[t,j];  (optional) out_dot[j] += sum_t dy[t,j]*xhat[t,j].
-// Used for bias gradients (x == nullptr) and for LN dgamma/dbeta. Block = 8 warps x 256 columns.
+// Used for bias gradients (x == nullptr) and for LN dgamma/dbeta. Block = 8 warps x 256 columns. RMS: xhat = x * rstd (mean
+// is not read).
+template <bool RMS>
 __global__ void __launch_bounds__(256) col_reduce_kernel(const __nv_bfloat16* __restrict__ dy, long long ld,
                                                           const __nv_bfloat16* __restrict__ x, const float* __restrict__ mean,
                                                           const float* __restrict__ rstd, float* __restrict__ out_sum,
@@ -354,7 +371,7 @@ __global__ void __launch_bounds__(256) col_reduce_kernel(const __nv_bfloat16* __
         q[u] = *reinterpret_cast<const uint4*>(dy + (r + 8 * u) * ld + col);
         if (x) {
           qx[u] = *reinterpret_cast<const uint4*>(x + (r + 8 * u) * (long long)d + col);
-          mu[u] = mean[r + 8 * u], rs[u] = rstd[r + 8 * u];
+          mu[u] = RMS ? 0.f : mean[r + 8 * u], rs[u] = rstd[r + 8 * u];
         }
       }
 #pragma unroll
@@ -377,7 +394,7 @@ __global__ void __launch_bounds__(256) col_reduce_kernel(const __nv_bfloat16* __
       if (x) {
         float fx[8];
         unpack8(*reinterpret_cast<const uint4*>(x + r * (long long)d + col), fx);
-        const float mu = mean[r], rs = rstd[r];
+        const float mu = RMS ? 0.f : mean[r], rs = rstd[r];
 #pragma unroll
         for (int k = 0; k < 8; ++k) ad[k] += g[k] * (fx[k] - mu) * rs;
       }
@@ -663,6 +680,52 @@ inline int grid_for(long long work_items, int block, int max_blocks = 132 * 8) {
   return int(b < max_blocks ? b : max_blocks);
 }
 
+template <bool RMS>
+void norm_fwd(const void* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, long long T, int d, float eps,
+              cudaStream_t st) {
+  if (d % 8 || d > LN_MAXCH * 256)
+    throw std::runtime_error(std::string(RMS ? "rmsnorm" : "layernorm") + ": d must be a multiple of 8 and <= 4096");
+  with_ln_chunks((d + 255) / 256, [&](auto N) {
+    ln_fwd_kernel<N, RMS><<<int((T + 7) / 8), 256, 0, st>>>((const __nv_bfloat16*)x, gamma, beta, (__nv_bfloat16*)y, mean, rstd, T, d, eps);
+  });
+  launched(RMS ? "rmsnorm_fwd" : "layernorm_fwd");
+}
+template <bool RMS>
+void col_reduce_as(const void* dy, long long ld, const void* x, const float* mean, const float* rstd, float* out_sum, float* out_dot,
+                   long long T, int d, cudaStream_t st) {
+  const int col_blocks = (d + 255) / 256;
+  int strips = (132 * 4 + col_blocks - 1) / col_blocks;
+  if (strips > T) strips = int(T);
+  const int rows_per = int((T + strips - 1) / strips);
+  dim3 grid(col_blocks, int((T + rows_per - 1) / rows_per));
+  col_reduce_kernel<RMS><<<grid, 256, 0, st>>>((const __nv_bfloat16*)dy, ld, (const __nv_bfloat16*)x, mean, rstd, out_sum, out_dot, T, d,
+                                               rows_per);
+  launched("col_reduce");
+}
+template <bool RMS>
+void norm_bwd(const void* dy, const void* x, const float* gamma, const float* mean, const float* rstd, const void* dres, void* dx,
+              float* dgamma, float* dbeta, long long T, int d, cudaStream_t st) {
+  if (d % 8 || d > LN_MAXCH * 256)
+    throw std::runtime_error(std::string(RMS ? "rmsnorm" : "layernorm") + ": d must be a multiple of 8 and <= 4096");
+  const int nch = (d + 255) / 256;
+  if ((dgamma || dbeta) && nch <= 4) {
+    // d <= 1024: dx and the dgamma / dbeta column sums in ONE pass over dy and x
+    const int grid = int(std::min<long long>((T + 7) / 8, 132 * 2));   // 2 resident blocks per SM
+    with_ln_chunks<4>(nch, [&](auto N) {
+      ln_bwd_fused_kernel<N, RMS><<<grid, 256, 0, st>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, gamma, mean, rstd,
+                                                        (const __nv_bfloat16*)dres, (__nv_bfloat16*)dx, dgamma, dbeta, T, d);
+    });
+    launched(RMS ? "rmsnorm_bwd_fused" : "layernorm_bwd_fused");
+    return;
+  }
+  with_ln_chunks(nch, [&](auto N) {
+    ln_bwd_dx_kernel<N, RMS><<<int((T + 7) / 8), 256, 0, st>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, gamma, mean, rstd,
+                                                               (const __nv_bfloat16*)dres, (__nv_bfloat16*)dx, T, d);
+  });
+  launched(RMS ? "rmsnorm_bwd_dx" : "layernorm_bwd_dx");
+  if (dgamma || dbeta) col_reduce_as<RMS>(dy, d, x, mean, rstd, dbeta, dgamma, T, d, st);
+}
+
 }  // namespace
 
 void embed_fwd(const int64_t* ids, const void* wte, const void* wpe, void* out, long long T, int S, int d, int V, cudaStream_t st) {
@@ -680,45 +743,25 @@ void embed_bwd(const int64_t* ids, const void* dh, float* dwte, float* dwpe, lon
     launched("embed_bwd_wpe");
   }
 }
+
 void layernorm_fwd(const void* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, long long T, int d,
                    float eps, cudaStream_t st) {
-  if (d % 8 || d > LN_MAXCH * 256) throw std::runtime_error("layernorm: d must be a multiple of 8 and <= 4096");
-  with_ln_chunks((d + 255) / 256, [&](auto N) {
-    ln_fwd_kernel<N><<<int((T + 7) / 8), 256, 0, st>>>((const __nv_bfloat16*)x, gamma, beta, (__nv_bfloat16*)y, mean, rstd, T, d, eps);
-  });
-  launched("layernorm_fwd");
+  norm_fwd<false>(x, gamma, beta, y, mean, rstd, T, d, eps, st);
+}
+void rmsnorm_fwd(const void* x, const float* gamma, void* y, float* rstd, long long T, int d, float eps, cudaStream_t st) {
+  norm_fwd<true>(x, gamma, nullptr, y, nullptr, rstd, T, d, eps, st);
 }
 void col_reduce(const void* dy, long long ld, const void* x, const float* mean, const float* rstd, float* out_sum, float* out_dot,
                 long long T, int d, cudaStream_t st) {
-  const int col_blocks = (d + 255) / 256;
-  int strips = (132 * 4 + col_blocks - 1) / col_blocks;
-  if (strips > T) strips = int(T);
-  const int rows_per = int((T + strips - 1) / strips);
-  dim3 grid(col_blocks, int((T + rows_per - 1) / rows_per));
-  col_reduce_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)dy, ld, (const __nv_bfloat16*)x, mean, rstd, out_sum, out_dot, T, d,
-                                          rows_per);
-  launched("col_reduce");
+  col_reduce_as<false>(dy, ld, x, mean, rstd, out_sum, out_dot, T, d, st);
 }
 void layernorm_bwd(const void* dy, const void* x, const float* gamma, const float* mean, const float* rstd, const void* dres, void* dx,
                    float* dgamma, float* dbeta, long long T, int d, cudaStream_t st) {
-  if (d % 8 || d > LN_MAXCH * 256) throw std::runtime_error("layernorm: d must be a multiple of 8 and <= 4096");
-  const int nch = (d + 255) / 256;
-  if ((dgamma || dbeta) && nch <= 4) {
-    // d <= 1024: dx and the dgamma / dbeta column sums in ONE pass over dy and x
-    const int grid = int(std::min<long long>((T + 7) / 8, 132 * 2));   // 2 resident blocks per SM
-    with_ln_chunks<4>(nch, [&](auto N) {
-      ln_bwd_fused_kernel<N><<<grid, 256, 0, st>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, gamma, mean, rstd,
-                                                   (const __nv_bfloat16*)dres, (__nv_bfloat16*)dx, dgamma, dbeta, T, d);
-    });
-    launched("layernorm_bwd_fused");
-    return;
-  }
-  with_ln_chunks(nch, [&](auto N) {
-    ln_bwd_dx_kernel<N><<<int((T + 7) / 8), 256, 0, st>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, gamma, mean, rstd,
-                                                          (const __nv_bfloat16*)dres, (__nv_bfloat16*)dx, T, d);
-  });
-  launched("layernorm_bwd_dx");
-  if (dgamma || dbeta) col_reduce(dy, d, x, mean, rstd, dbeta, dgamma, T, d, st);
+  norm_bwd<false>(dy, x, gamma, mean, rstd, dres, dx, dgamma, dbeta, T, d, st);
+}
+void rmsnorm_bwd(const void* dy, const void* x, const float* gamma, const float* rstd, const void* dres, void* dx, float* dgamma,
+                 long long T, int d, cudaStream_t st) {
+  norm_bwd<true>(dy, x, gamma, nullptr, rstd, dres, dx, dgamma, nullptr, T, d, st);
 }
 void cross_entropy(void* logits, long long ld, const int64_t* targets, long long rows, int V, float grad_scale, bool write_grad,
                    double* stats, float* row_lse, const float* unigram_logp, cudaStream_t st) {

@@ -21,6 +21,10 @@ void layernorm_fwd(const void* x, const float* gamma, const float* beta, void* y
                    float eps, cudaStream_t st);
 void layernorm_bwd(const void* dy, const void* x, const float* gamma, const float* mean, const float* rstd, const void* dres, void* dx,
                    float* dgamma, float* dbeta, long long T, int d, cudaStream_t st);
+// RMSNorm: y = x * rstd * gamma with rstd = rsqrt(mean(x^2) + eps); the backward's dgamma = sum_t dy * x * rstd (null: skipped)
+void rmsnorm_fwd(const void* x, const float* gamma, void* y, float* rstd, long long T, int d, float eps, cudaStream_t st);
+void rmsnorm_bwd(const void* dy, const void* x, const float* gamma, const float* rstd, const void* dres, void* dx, float* dgamma,
+                 long long T, int d, cudaStream_t st);
 void col_reduce(const void* dy, long long ld, const void* x, const float* mean, const float* rstd, float* out_sum, float* out_dot,
                 long long T, int d, cudaStream_t st);
 void cross_entropy(void* logits, long long ld, const int64_t* targets, long long rows, int V, float grad_scale, bool write_grad,

@@ -132,7 +132,7 @@ class KVDecoder:
                 part = qkv[:, lo:lo + n]
                 p, t = (x.view(-1)[: T * n].view(T, n) for x in (pre, tmp))
                 p.copy_(part)
-                ops.layernorm_fwd(p, w.qk_g[j], w.qk_b[j], t, m, r, c.norm_eps)
+                self.e._norm_fwd(p, w.qk_g[j], w.qk_b[j], t, m, r)  # noqa: SLF001
                 part.copy_(t)
 
     # ------------------------------------------------------------------ prefill
@@ -158,7 +158,7 @@ class KVDecoder:
         pre, tmp = (bf(T, d), bf(T, d)) if c.qk_ln else (None, None)
         ops.embed_fwd(ids.reshape(-1), e.wte16, e.wpe16, h, S)
         for i, w in enumerate(e.layers):
-            ops.layernorm_fwd(h, w.g1, w.b1, ln, m, r, c.norm_eps)
+            e._norm_fwd(h, w.g1, w.b1, ln, m, r)
             ops.linear_fwd(ln, w.wqkv, w.bqkv, qkv)
             self._qkv_post(w, qkv, pre, tmp, m, r)
             if e.rope is not None:
@@ -168,7 +168,7 @@ class KVDecoder:
             self.cache[i, 0, :, :, :S].index_copy_(0, dst, k)   # the kv heads' k / v after clip, qk_ln and RoPE
             self.cache[i, 1, :, :, :S].index_copy_(0, dst, v)
             ops.linear_fwd(attn, w.wo, w.bo, hmid, residual=h)
-            ops.layernorm_fwd(hmid, w.g2, w.b2, ln, m, r, c.norm_eps)
+            e._norm_fwd(hmid, w.g2, w.b2, ln, m, r)
             self._ffn(w, ln, u, z, h, hmid, dact, cg)
         last = torch.tensor([i * S + n - 1 for i, n in enumerate(lens)], dtype=torch.long).to(self.dev, non_blocking=True)
         return torch.index_select(h, 0, last)
@@ -176,7 +176,7 @@ class KVDecoder:
     @torch.no_grad()
     def start(self, prompts: list[list[int]], max_new_tokens: int) -> list[int]:
         """Prefill ``prompts`` (a batch of token lists) and return the first greedy token of each."""
-        c, e = self.cfg, self.e
+        e = self.e
         b = len(prompts)
         if not 1 <= b <= self.max_batch:
             raise ValueError(f"batch of {b} prompts; this decoder runs 1..{self.max_batch}")
@@ -189,7 +189,7 @@ class KVDecoder:
         B = self.buf
         # only the last prompt row of every sequence goes through the final LN and the LM head
         B["h"][:b].copy_(self._prefill(prompts, list(range(b))))
-        ops.layernorm_fwd(B["h"][:b], e.gf, e.bf, B["ln"][:b], B["m"][:b], B["r"][:b], c.norm_eps)
+        e._norm_fwd(B["h"][:b], e.gf, e.bf, B["ln"][:b], B["m"][:b], B["r"][:b])
         self._linear(B["ln"][:b], e.wte16, None, B["logits"][:b])
         self.pos[:b].copy_(torch.tensor(lens, dtype=torch.int32), non_blocking=True)
         ops.argmax_advance(B["logits"][:b], self.tok[:b])
@@ -207,7 +207,7 @@ class KVDecoder:
         h, ln, m, r, qkv, attn, hmid, u, z = (x[k] for k in ("h", "ln", "m", "r", "qkv", "attn", "hmid", "u", "z"))
         for i, w in enumerate(e.layers):
             kc, vc = self.cache[i, 0], self.cache[i, 1]
-            ops.layernorm_fwd(h, w.g1, w.b1, ln, m, r, c.norm_eps)
+            e._norm_fwd(h, w.g1, w.b1, ln, m, r)
             self._linear(ln, w.wqkv, w.bqkv, qkv)
             self._qkv_post(w, qkv, x.get("qk_pre"), x.get("qk_tmp"), m, r)
             ops.decode_append(qkv, pos, kc, vc, e.rope, c.n_heads, slot, n_kv_heads=c.kv_n_heads)
@@ -216,16 +216,16 @@ class KVDecoder:
             else:
                 ops.cache_attention(qkv, kc, vc, tiles, attn, c.n_heads, self.scale, e.alibi, n_kv_heads=c.kv_n_heads)
             self._linear(attn, w.wo, w.bo, hmid, residual=h)
-            ops.layernorm_fwd(hmid, w.g2, w.b2, ln, m, r, c.norm_eps)
+            e._norm_fwd(hmid, w.g2, w.b2, ln, m, r)
             self._ffn(w, ln, u, z, h, hmid, x.get("ffn_d"), x.get("ffn_c"))
 
     # --------------------------------------------------------------------- step
     def _step_kernels(self, b: int) -> None:
-        c, e, B = self.cfg, self.e, self.buf
+        e, B = self.e, self.buf
         x = {k: v[:b] for k, v in B.items() if k != "logits"}
         ops.embed_pos(self.tok, self.pos, e.wte16, e.wpe16, x["h"])
         self._blocks(x, self.pos)
-        ops.layernorm_fwd(x["h"], e.gf, e.bf, x["ln"], x["m"], x["r"], c.norm_eps)
+        e._norm_fwd(x["h"], e.gf, e.bf, x["ln"], x["m"], x["r"])
         self._linear(x["ln"], e.wte16, None, B["logits"][:b])
         ops.argmax_advance(B["logits"][:b], self.tok, self.pos)
 
@@ -304,7 +304,7 @@ class KVDecoder:
             self._blocks(x, pos_t, i32([s for s, _, n, _ in runs for _ in range(n)]), ops.cache_tiles(runs, self.dev))
         ln = torch.empty_like(hid)
         m, r = (torch.empty(R, dtype=torch.float32, device=self.dev) for _ in range(2))
-        ops.layernorm_fwd(hid, e.gf, e.bf, ln, m, r, c.norm_eps)
+        e._norm_fwd(hid, e.gf, e.bf, ln, m, r)
         logits = torch.empty(R, c.vocab_size, dtype=torch.bfloat16, device=self.dev)
         self._linear(ln, e.wte16, None, logits)
         # scored token k of pair i is predicted by its group's last context row (k = 0) or by extend row first[i] + k - 1

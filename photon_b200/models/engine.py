@@ -14,7 +14,7 @@ master parameters/gradients and a flat bf16 compute shadow
 * LM head + cross-entropy chunked over tokens so the ``[T, 50368]`` logits are
   never materialised (``[chunk, V]`` scratch that stays L2/HBM friendly);
   the chunk's dlogits feed the dgrad/wgrad GEMMs immediately;
-* LayerNorm fwd/bwd (+ residual-gradient add), embedding gather/scatter,
+* LayerNorm / RMSNorm fwd/bwd (+ residual-gradient add), embedding gather/scatter,
   bias-gradient column sums, loss statistics: ``csrc/fused_ops.cu``;
 * attention: ``csrc/attention_tcgen05.cu`` (``attention: b200``) or, when
   ``kernels.attention: torch``, cuDNN/FA2 SDPA as an explicit library fallback.
@@ -38,8 +38,9 @@ from photon_b200.train.backend import apply_freeze
 from photon_b200.utils.flat import FlatLayout, FlatParams
 
 # One block's backward as stages in execution order, each with the parameters whose gradients it produces (a stage's input
-# gradient feeds the next one; the residual path joins at ln2 / ln1). "attn" is the attention backward with the q/k LayerNorms;
-# "up" covers the gate projection of a gated FFN too (its names are absent from an mptmlp layout).
+# gradient feeds the next one; the residual path joins at ln2 / ln1). "ln2" / "ln1" and the q/k norms of "attn" (the attention
+# backward with them) are LayerNorms or RMSNorms (cfg.norm_type). Names absent from a layout are never trainable: a norm's bias
+# under RMSNorm or no_bias, and the gate projection ("up" covers it in a gated FFN) in an mptmlp one.
 BLOCK_STAGES = (("down", ("ffn.down_proj.weight", "ffn.down_proj.bias")),
                 ("up", ("ffn.up_proj.weight", "ffn.up_proj.bias", "ffn.gate_proj.weight", "ffn.gate_proj.bias")),
                 ("ln2", ("norm_2.weight", "norm_2.bias")),
@@ -395,6 +396,7 @@ class B200Engine:
         T, d, H, L, W, Fh = b * S, c.d_model, c.n_heads, c.n_layers, c.qkv_dim, c.ffn_hidden
         bf = lambda *s: torch.empty(*s, dtype=torch.bfloat16, device=dev)  # noqa: E731
         f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
+        mean = (lambda: None) if c.rmsnorm else (lambda: f32(T))   # a LayerNorm's row means (RMSNorm keeps rstd only)  # noqa: E731
         ws: dict[str, Any] = {"h": [bf(T, d) for _ in range(L + 1)], "layers": []}
         for i in range(L):
             if self.activation_checkpointing and i > 0:
@@ -402,22 +404,22 @@ class B200Engine:
                 continue
             if self.fp8:   # the GEMM inputs exist only as E4M3 (1 byte): 7·T·d instead of 12·T·d bytes of saved activations
                 u8 = lambda *s: torch.empty(*s, dtype=torch.uint8, device=dev)  # noqa: E731
-                ws["layers"].append({"ln1": u8(T, d), "m1": f32(T), "r1": f32(T), "qkv": bf(T, W), "attn": bf(T, d), "attn8": u8(T, d),
-                                     "lse": f32(b, H, S), "hmid": bf(T, d), "ln2": u8(T, d), "m2": f32(T), "r2": f32(T),
+                ws["layers"].append({"ln1": u8(T, d), "m1": mean(), "r1": f32(T), "qkv": bf(T, W), "attn": bf(T, d), "attn8": u8(T, d),
+                                     "lse": f32(b, H, S), "hmid": bf(T, d), "ln2": u8(T, d), "m2": mean(), "r2": f32(T),
                                      "z": bf(T, Fh), "u": u8(T, Fh)})
             else:
-                ws["layers"].append({"ln1": bf(T, d), "m1": f32(T), "r1": f32(T), "qkv": bf(T, W), "attn": bf(T, d),
-                                     "lse": f32(b, H, S), "hmid": bf(T, d), "ln2": bf(T, d), "m2": f32(T), "r2": f32(T),
+                ws["layers"].append({"ln1": bf(T, d), "m1": mean(), "r1": f32(T), "qkv": bf(T, W), "attn": bf(T, d),
+                                     "lse": f32(b, H, S), "hmid": bf(T, d), "ln2": bf(T, d), "m2": mean(), "r2": f32(T),
                                      "z": bf(T, Fh), "u": bf(T, Fh)})
                 if c.ffn_gated:   # z = u * act'(g), u = act(g) * up (the down projection's input), a = act(g)
                     ws["layers"][-1]["a"] = bf(T, Fh)
             if c.clip_qkv:
                 ws["layers"][-1]["clipmask"] = torch.empty(T, W, dtype=torch.bool, device=dev)
-            if c.qk_ln:   # pre-LayerNorm q / k (inputs of the two LN backward passes) and their row statistics
-                ws["layers"][-1].update(qk_pre=[bf(T, d), bf(T, c.kv_dim)], qk_m=[f32(T), f32(T)], qk_r=[f32(T), f32(T)])
-        if c.qk_ln:   # scratch of the q / k LayerNorms, viewed at the width of the part in use (see _qk_parts)
+            if c.qk_ln:   # pre-norm q / k (inputs of the two norm backward passes) and their row statistics
+                ws["layers"][-1].update(qk_pre=[bf(T, d), bf(T, c.kv_dim)], qk_m=[mean(), mean()], qk_r=[f32(T), f32(T)])
+        if c.qk_ln:   # scratch of the q / k norms, viewed at the width of the part in use (see _qk_parts)
             ws.update(qk_tmp=bf(T, d), qk_tmp2=bf(T, d))
-        ws.update(lnf=bf(T, d), mf=f32(T), rf=f32(T), dlnf=bf(T, d), dh=bf(T, d), dhmid=bf(T, d), dln=bf(T, d),
+        ws.update(lnf=bf(T, d), mf=mean(), rf=f32(T), dlnf=bf(T, d), dh=bf(T, d), dhmid=bf(T, d), dln=bf(T, d),
                   dqkv=bf(T, W), dattn=bf(T, d), dz=bf(T, Fh), delta=f32(b, H, S),
                   logits=bf(min(self.lm_head_chunk, T), c.vocab_size))
         if self.fp8:   # E5M2 copy of the gradient currently flowing backward (one buffer, viewed at the width in use)
@@ -429,6 +431,30 @@ class B200Engine:
         ws["sequence_id"] = None      # this microbatch's document ids (set by _forward), None: plain causal
         self._ws[key] = ws
         return ws
+
+    # ------------------------------------------------------------ normalisation
+    # Every norm of the model (norm_1, norm_2, norm_f, q_ln, k_ln) runs through these three, LayerNorm or RMSNorm by
+    # cfg.norm_type. ``b`` (beta), ``db`` and ``m`` (row means) belong to LayerNorm only: RMSNorm ignores them (None there).
+    def _norm_fwd(self, x: torch.Tensor, g: torch.Tensor, b: torch.Tensor | None, y: torch.Tensor, m: torch.Tensor | None,
+                  r: torch.Tensor) -> None:
+        if self.cfg.rmsnorm:
+            ops.rmsnorm_fwd(x, g, y, r, self.cfg.norm_eps)
+        else:
+            ops.layernorm_fwd(x, g, b, y, m, r, self.cfg.norm_eps)
+
+    def _norm_fwd_q8(self, x: torch.Tensor, g: torch.Tensor, b: torch.Tensor | None, y8: torch.Tensor, m: torch.Tensor | None,
+                     r: torch.Tensor, role: int) -> None:
+        if self.cfg.rmsnorm:
+            ops.rmsnorm_fwd_q8(x, g, y8, r, self.cfg.norm_eps, self.fp8_meta, role)
+        else:
+            ops.layernorm_fwd_q8(x, g, b, y8, m, r, self.cfg.norm_eps, self.fp8_meta, role)
+
+    def _norm_bwd(self, dy: torch.Tensor, x: torch.Tensor, g: torch.Tensor, m: torch.Tensor | None, r: torch.Tensor,
+                  dres: torch.Tensor | None, dx: torch.Tensor, dg: torch.Tensor | None, db: torch.Tensor | None) -> None:
+        if self.cfg.rmsnorm:
+            ops.rmsnorm_bwd(dy, x, g, r, dres, dx, dg)
+        else:
+            ops.layernorm_bwd(dy, x, g, m, r, dres, dx, dg, db)
 
     # ------------------------------------------------------------------ forward
     def _kernel_attention(self, S: int) -> bool:
@@ -503,10 +529,10 @@ class B200Engine:
         c, h, w, lw = self.cfg, ws["h"], self.layers[i], ws["layers"][i]
         if self.fp8:
             M, w8, R = self.fp8_meta, self.w8_views[i], self._role
-            ops.layernorm_fwd_q8(h[i], w.g1, w.b1, lw["ln1"], lw["m1"], lw["r1"], c.norm_eps, M, R("x_ln1", i))
+            self._norm_fwd_q8(h[i], w.g1, w.b1, lw["ln1"], lw["m1"], lw["r1"], R("x_ln1", i))
             ops.gemm_fp8(lw["ln1"], w8["wqkv"], lw["qkv"], M, R("x_ln1", i), R("wqkv", i), bias=w.bqkv)
         else:
-            ops.layernorm_fwd(h[i], w.g1, w.b1, lw["ln1"], lw["m1"], lw["r1"], c.norm_eps)
+            self._norm_fwd(h[i], w.g1, w.b1, lw["ln1"], lw["m1"], lw["r1"])
             ops.linear_fwd(lw["ln1"], w.wqkv, w.bqkv, lw["qkv"])
         if c.clip_qkv:   # attn_config.clip_qkv: clamp the fused projection; remember where the gradient passes
             torch.logical_and(lw["qkv"] > -c.clip_qkv, lw["qkv"] < c.clip_qkv, out=lw["clipmask"])
@@ -516,7 +542,7 @@ class B200Engine:
             for j, (lo, n) in enumerate(self._qk_parts()):
                 part, tmp = lw["qkv"][:, lo:lo + n], ws["qk_tmp"].view(-1)[: T * n].view(T, n)
                 lw["qk_pre"][j].copy_(part)
-                ops.layernorm_fwd(lw["qk_pre"][j], w.qk_g[j], w.qk_b[j], tmp, lw["qk_m"][j], lw["qk_r"][j], c.norm_eps)
+                self._norm_fwd(lw["qk_pre"][j], w.qk_g[j], w.qk_b[j], tmp, lw["qk_m"][j], lw["qk_r"][j])
                 part.copy_(tmp)
         if self.rope is not None:
             ops.rope_(lw["qkv"].view(b, S, c.qkv_dim), self.rope[0], self.rope[1], c.n_heads, n_kv_heads=c.kv_n_heads)
@@ -524,14 +550,14 @@ class B200Engine:
         if self.fp8:
             ops.colsum_quant(lw["attn"], None, lw["attn8"], ops.E4M3, M, R("x_attn", i))
             ops.gemm_fp8(lw["attn8"], w8["wo"], lw["hmid"], M, R("x_attn", i), R("wo", i), epi=ops.EPI_RESIDUAL, bias=w.bo, aux=h[i])
-            ops.layernorm_fwd_q8(lw["hmid"], w.g2, w.b2, lw["ln2"], lw["m2"], lw["r2"], c.norm_eps, M, R("x_ln2", i))
+            self._norm_fwd_q8(lw["hmid"], w.g2, w.b2, lw["ln2"], lw["m2"], lw["r2"], R("x_ln2", i))
             # gelu(z) leaves the epilogue as E4M3 (the down-projection's operand), gelu'(z) as bf16 (the dgrad multiplier)
             ops.gemm_fp8(lw["ln2"], w8["wup"], lw["z"], M, R("x_ln2", i), R("wup", i), epi=ops.EPI_GELU_GRAD_Q8, bias=w.bup, out2=lw["z"],
                          out8=lw["u"], role_out=R("x_u", i))
             ops.gemm_fp8(lw["u"], w8["wdown"], h[i + 1], M, R("x_u", i), R("wdown", i), epi=ops.EPI_RESIDUAL, bias=w.bdown, aux=lw["hmid"])
             return
         ops.linear_fwd(lw["attn"], w.wo, w.bo, lw["hmid"], residual=h[i])
-        ops.layernorm_fwd(lw["hmid"], w.g2, w.b2, lw["ln2"], lw["m2"], lw["r2"], c.norm_eps)
+        self._norm_fwd(lw["hmid"], w.g2, w.b2, lw["ln2"], lw["m2"], lw["r2"])
         if c.ffn_gated:
             # a = act(g), act'(g) into the free dz (a backward buffer); then u = up(ln2): lw["u"] = a * u, lw["z"] = u * act'(g)
             ops.linear_act_grad_fwd(c.ffn_act, lw["ln2"], w.wgate, w.bgate, ws["dz"], lw["a"])
@@ -562,7 +588,7 @@ class B200Engine:
                 x = h[i + 1][:S].float()
                 self.activation_stats[f"l2_norm/block_{i}"] = float(x.norm(dim=-1).mean())
                 self.activation_stats[f"max/block_{i}"] = float(x.abs().max())
-        ops.layernorm_fwd(h[c.n_layers], self.gf, self.bf, ws["lnf"], ws["mf"], ws["rf"], c.norm_eps)
+        self._norm_fwd(h[c.n_layers], self.gf, self.bf, ws["lnf"], ws["mf"], ws["rf"])
 
     def _head(self, ws: dict[str, Any], targets: torch.Tensor, grad_scale: float, train: bool) -> None:
         """Chunked LM head + fused CE (+ immediate head backward when training)."""
@@ -631,7 +657,7 @@ class B200Engine:
         dh = ws["dh"]
         z, P = self.zero3, self.plan
         if P.runs("norm_f"):
-            ops.layernorm_bwd(ws["dlnf"], h[c.n_layers], self.gf, ws["mf"], ws["rf"], None, dh, self.d_gf, self.d_bf)
+            self._norm_bwd(ws["dlnf"], h[c.n_layers], self.gf, ws["mf"], ws["rf"], None, dh, self.d_gf, self.d_bf)
         # blocks below the lowest one with a trainable tensor (and their recompute) are skipped: see BackwardPlan
         for i in range(c.n_layers - 1, P.lowest_block - 1, -1):
             if z is not None:
@@ -664,7 +690,7 @@ class B200Engine:
             self._linear_bwd(i, ws, ws["dz"], "g_dz", lw["ln2"], "x_ln2", "wup", w.wup, w.d_wup, w.d_bup, dx("up", dln))
         if not P.runs((i, "ln2")):
             return
-        ops.layernorm_bwd(dln, lw["hmid"], w.g2, lw["m2"], lw["r2"], dh, dhmid, w.d_g2, w.d_b2)
+        self._norm_bwd(dln, lw["hmid"], w.g2, lw["m2"], lw["r2"], dh, dhmid, w.d_g2, w.d_b2)
         if not P.runs((i, "out")):
             return
         # ---- attention: hmid = h[i] + out_proj(attn(qkv(ln1(h[i]))))
@@ -679,7 +705,7 @@ class B200Engine:
                 part = ws["dqkv"][:, lo:lo + n]
                 tmp, tmp2 = (ws[k].view(-1)[: T * n].view(T, n) for k in ("qk_tmp", "qk_tmp2"))
                 tmp.copy_(part)
-                ops.layernorm_bwd(tmp, lw["qk_pre"][j], w.qk_g[j], lw["qk_m"][j], lw["qk_r"][j], None, tmp2, w.d_qk_g[j], w.d_qk_b[j])
+                self._norm_bwd(tmp, lw["qk_pre"][j], w.qk_g[j], lw["qk_m"][j], lw["qk_r"][j], None, tmp2, w.d_qk_g[j], w.d_qk_b[j])
                 part.copy_(tmp2)
         if c.clip_qkv:
             ws["dqkv"].mul_(lw["clipmask"])
@@ -688,7 +714,7 @@ class B200Engine:
         self._linear_bwd(i, ws, ws["dqkv"], "g_dqkv", lw["ln1"], "x_ln1", "wqkv", w.wqkv, w.d_wqkv, w.d_bqkv, dx("qkv", dln))
         if not P.runs((i, "ln1")):
             return
-        ops.layernorm_bwd(dln, h[i], w.g1, lw["m1"], lw["r1"], dhmid, dh, w.d_g1, w.d_b1)
+        self._norm_bwd(dln, h[i], w.g1, lw["m1"], lw["r1"], dhmid, dh, w.d_g1, w.d_b1)
 
     # ---------------------------------------------------------------- protocol
     def _fwd_bwd_eager(self, ids: torch.Tensor, grad_scale: float, sequence_id: torch.Tensor | None = None) -> None:

@@ -8,8 +8,8 @@ photon/utils.py:572,591,602-637; SURVEY Appendix C). The B200 hot path lives in
 hand-written sm_90a kernels and is tested against this module.
 
 Block: ``x = x + attn(norm_1(x)); x = x + ffn(norm_2(x))``; ``ffn = down(act(up(x)))`` (``mptmlp``) or
-``down(act(gate(x)) * up(x))`` (``mptglu``), ``act`` exact GELU (default) or SiLU; LM head tied to ``wte``; loss = CE over
-``targets = roll(labels, -1)`` with the last position ignored (-100).
+``down(act(gate(x)) * up(x))`` (``mptglu``), ``act`` exact GELU (default) or SiLU; every norm LayerNorm (default) or RMSNorm
+(``norm_type``); LM head tied to ``wte``; loss = CE over ``targets = roll(labels, -1)`` with the last position ignored (-100).
 """
 from __future__ import annotations
 
@@ -40,6 +40,9 @@ class MPTConfig:
     no_bias: bool = False
     learned_pos_emb: bool = True
     norm_eps: float = 1e-5
+    # model.norm_type: "layernorm" (LayerNorm, weight + bias unless no_bias) or "rmsnorm" (RMSNorm, weight only) for norm_1,
+    # norm_2, norm_f and, under qk_ln, q_ln / k_ln; any name of NORM_TYPES is accepted and stored as one of the two
+    norm_type: str = "layernorm"
     # attn_config.attn_uses_sequence_id: attention stays inside each document of a packed row (the collator's sequence_id)
     attn_uses_sequence_id: bool = False
     # attn_config.attn_type grouped_query_attention / multiquery_attention: K / V have kv_n_heads heads (None: n_heads), query
@@ -64,6 +67,14 @@ class MPTConfig:
             raise ValueError(f"unsupported FFN activation {self.ffn_act!r} (supported: {', '.join(FFN_ACTS)})")
         if self.ffn_hidden < 1:
             raise ValueError(f"the FFN width must be positive, got {self.ffn_hidden}")
+        norm = str(self.norm_type).lower()
+        if norm not in NORM_TYPES:
+            raise ValueError(f"unsupported model.norm_type {self.norm_type!r} (supported: {', '.join(NORM_TYPES)})")
+        self.norm_type = NORM_TYPES[norm]
+
+    @property
+    def rmsnorm(self) -> bool:
+        return self.norm_type == "rmsnorm"
 
     @property
     def ffn_hidden(self) -> int:
@@ -125,6 +136,7 @@ class MPTConfig:
             qk_ln=bool(attn.pop("qk_ln", False)), clip_qkv=attn.pop("clip_qkv", None),
             attn_uses_sequence_id=bool(attn.pop("attn_uses_sequence_id", False)), kv_n_heads=kv,
             no_bias=bool(m.pop("no_bias", False)), learned_pos_emb=bool(m.pop("learned_pos_emb", True)),
+            norm_type=m.pop("norm_type", "low_precision_layernorm"), norm_eps=float(m.pop("norm_eps", 1e-5)),
         )
         ffn = dict(m.pop("ffn_config", {}) or {})
         known.update(ffn_type=ffn.pop("ffn_type", "mptmlp"), ffn_act=parse_ffn_act(ffn.pop("ffn_act_fn", None)),
@@ -142,13 +154,12 @@ class MPTConfig:
     def num_params(self) -> int:
         d, L, V, S, f = self.d_model, self.n_layers, self.vocab_size, self.max_seq_len, self.ffn_hidden
         b = 0 if self.no_bias else 1
+        n = 1 if self.no_bias or self.rmsnorm else 2   # tensors per norm: weight, and a LayerNorm's bias unless no_bias
         w = self.qkv_dim
-        per_block = (2 * d) * 2 + (w * d + b * w) + (d * d + b * d) + (f * d + b * f) + (f * d + b * d)
+        per_block = 2 * n * d + (w * d + b * w) + (d * d + b * d) + (f * d + b * f) + (f * d + b * d)
         if self.ffn_gated:
             per_block += f * d + b * f   # gate_proj
-        if self.no_bias:
-            per_block -= 2 * d  # LN biases dropped too
-        return V * d + (S * d if self.learned_pos_emb else 0) + L * per_block + (2 * d if not self.no_bias else d)
+        return V * d + (S * d if self.learned_pos_emb else 0) + L * per_block + n * d
 
     def flops_per_token(self, seq_len: int | None = None) -> float:
         """fwd+bwd model FLOPs per token as SpeedMonitor counts them: 6·N + 12·L·d·S."""
@@ -157,6 +168,10 @@ class MPTConfig:
 
 
 FFN_TYPES = ("mptmlp", "mptglu")
+# llm-foundry's norm registry -> the normalisation built for it (the low-precision and Triton variants compute the same
+# function with the same parameters)
+NORM_TYPES = {"layernorm": "layernorm", "low_precision_layernorm": "layernorm", "rmsnorm": "rmsnorm",
+              "low_precision_rmsnorm": "rmsnorm", "triton_rmsnorm": "rmsnorm"}
 FFN_ACTS = ("gelu", "silu")
 
 
@@ -211,6 +226,25 @@ def apply_rope(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor) -> torch.T
     return torch.cat([x1 * c - x2 * s, x2 * c + x1 * s], dim=-1)
 
 
+class RMSNorm(nn.Module):
+    """llm-foundry's ``RMSNorm``: ``y = x · rsqrt(mean(x²) + eps) · weight`` in fp32, cast back to the input dtype; ``weight``
+    only, initialised to ones."""
+
+    def __init__(self, d: int, eps: float) -> None:
+        super().__init__()
+        self.eps = float(eps)
+        self.weight = nn.Parameter(torch.ones(d))
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        xf = x.float()
+        return (xf * torch.rsqrt(xf.pow(2).mean(-1, keepdim=True) + self.eps) * self.weight.float()).to(x.dtype)
+
+
+def build_norm(cfg: MPTConfig, d: int, bias: bool) -> nn.Module:
+    """The normalisation of ``cfg.norm_type`` over ``d`` features (``bias``: whether a LayerNorm has one)."""
+    return RMSNorm(d, cfg.norm_eps) if cfg.rmsnorm else nn.LayerNorm(d, eps=cfg.norm_eps, bias=bias)
+
+
 class MPTAttention(nn.Module):
     def __init__(self, cfg: MPTConfig) -> None:
         super().__init__()
@@ -219,8 +253,8 @@ class MPTAttention(nn.Module):
         self.Wqkv = nn.Linear(d, cfg.qkv_dim, bias=not cfg.no_bias)
         self.out_proj = nn.Linear(d, d, bias=not cfg.no_bias)
         if cfg.qk_ln:
-            self.q_ln = nn.LayerNorm(d, eps=cfg.norm_eps)
-            self.k_ln = nn.LayerNorm(cfg.kv_dim, eps=cfg.norm_eps)
+            self.q_ln = build_norm(cfg, d, bias=True)
+            self.k_ln = build_norm(cfg, cfg.kv_dim, bias=True)
 
     def forward(self, x: torch.Tensor, rope: tuple[torch.Tensor, torch.Tensor] | None,
                 alibi: torch.Tensor | None, doc_keep: torch.Tensor | None = None) -> torch.Tensor:
@@ -291,9 +325,9 @@ class MPTGLU(MPTMLP):
 class MPTBlock(nn.Module):
     def __init__(self, cfg: MPTConfig) -> None:
         super().__init__()
-        self.norm_1 = nn.LayerNorm(cfg.d_model, eps=cfg.norm_eps, bias=not cfg.no_bias)
+        self.norm_1 = build_norm(cfg, cfg.d_model, bias=not cfg.no_bias)
         self.attn = MPTAttention(cfg)
-        self.norm_2 = nn.LayerNorm(cfg.d_model, eps=cfg.norm_eps, bias=not cfg.no_bias)
+        self.norm_2 = build_norm(cfg, cfg.d_model, bias=not cfg.no_bias)
         self.ffn = MPTGLU(cfg) if cfg.ffn_gated else MPTMLP(cfg)
 
     def forward(self, x: torch.Tensor, rope: Any, alibi: Any, doc_keep: Any = None) -> torch.Tensor:
@@ -308,7 +342,7 @@ class MPTTransformer(nn.Module):
         if cfg.learned_pos_emb:
             self.wpe = nn.Embedding(cfg.max_seq_len, cfg.d_model)
         self.blocks = nn.ModuleList([MPTBlock(cfg) for _ in range(cfg.n_layers)])
-        self.norm_f = nn.LayerNorm(cfg.d_model, eps=cfg.norm_eps, bias=not cfg.no_bias)
+        self.norm_f = build_norm(cfg, cfg.d_model, bias=not cfg.no_bias)
 
 
 class MPTForCausalLM(nn.Module):
@@ -357,6 +391,8 @@ class MPTForCausalLM(nn.Module):
                 mod.weight.fill_(1.0)
                 if mod.bias is not None:
                     mod.bias.zero_()
+            elif isinstance(mod, RMSNorm):
+                mod.weight.fill_(1.0)
 
     # -- forward ----------------------------------------------------------------
     def _aux(self, S: int, device: torch.device) -> tuple[Any, Any]:

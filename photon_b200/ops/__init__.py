@@ -170,6 +170,13 @@ def layernorm_fwd_q8(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor | 
     return y8
 
 
+def rmsnorm_fwd_q8(x: torch.Tensor, gamma: torch.Tensor, y8: torch.Tensor, rstd: torch.Tensor, eps: float, meta: torch.Tensor,
+                   role: int) -> torch.Tensor:
+    """:func:`layernorm_fwd_q8` for RMSNorm (:func:`rmsnorm_fwd`): E4M3 ``x · rstd · gamma`` and ``rstd``."""
+    ext().rmsnorm_fwd_q8(x, gamma, y8, rstd, float(eps), meta, int(role))
+    return y8
+
+
 def colsum_quant(dy: torch.Tensor, out_sum: torch.Tensor | None, y8: torch.Tensor | None, fmt: int = E5M2,
                  meta: torch.Tensor | None = None, role: int = -1) -> None:
     """One read of ``dy`` [T,N]: ``out_sum[j] += Σ_t dy[t,j]`` (bias gradient) and ``y8 = fp8(dy * scale[role])``."""
@@ -212,6 +219,20 @@ def layernorm_fwd(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor | Non
 def layernorm_bwd(dy: torch.Tensor, x: torch.Tensor, gamma: torch.Tensor, mean: torch.Tensor, rstd: torch.Tensor,
                   dres: torch.Tensor | None, dx: torch.Tensor, dgamma: torch.Tensor | None, dbeta: torch.Tensor | None) -> torch.Tensor:
     ext().layernorm_bwd(dy, x, gamma, mean, rstd, dres, dx, dgamma, dbeta)
+    return dx
+
+
+def rmsnorm_fwd(x: torch.Tensor, gamma: torch.Tensor, y: torch.Tensor, rstd: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
+    """``y = x · rstd · gamma`` per row, ``rstd = rsqrt(mean(x²) + eps)`` in fp32 (llm-foundry's ``rms_norm``); ``rstd`` [T] is
+    kept for :func:`rmsnorm_bwd`."""
+    ext().rmsnorm_fwd(x, gamma, y, rstd, float(eps))
+    return y
+
+
+def rmsnorm_bwd(dy: torch.Tensor, x: torch.Tensor, gamma: torch.Tensor, rstd: torch.Tensor, dres: torch.Tensor | None,
+                dx: torch.Tensor, dgamma: torch.Tensor | None) -> torch.Tensor:
+    """``dx = rstd · (dy·gamma − x̂ · mean(dy·gamma·x̂)) (+ dres)`` with ``x̂ = x · rstd``; ``dgamma += Σ_t dy·x̂`` unless None."""
+    ext().rmsnorm_bwd(dy, x, gamma, rstd, dres, dx, dgamma)
     return dx
 
 

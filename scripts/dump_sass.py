@@ -34,7 +34,7 @@ PICKS = [
     ("comm.cu.o", r"ddp_allreduce_kernel", "ddp_allreduce"),
     ("comm.cu.o", r"ddp_zero_step_kernel", "ddp_zero_step"),
     ("comm.cu.o", r"zero3_reduce_kernel", "zero3_reduce"),
-    ("fp8_ops.cu.o", r"ln_fwd_q8_kernel<3>", "layernorm_fwd_q8_d768"),
+    ("fp8_ops.cu.o", r"ln_fwd_q8_kernel<3, false>", "layernorm_fwd_q8_d768"),
     ("fp8_ops.cu.o", r"colsum_quant_kernel<1>", "colsum_quant_e5m2"),
     ("fused_ops.cu.o", r"optim_kernel", "fused_optimizer"),
     ("fused_ops.cu.o", r"ce_kernel", "cross_entropy"),
