@@ -58,13 +58,15 @@ __device__ __forceinline__ void wgmma_pv(float (&o)[DH / 2], const uint32_t (&a)
   else wgmma_bf16_rs_n128<1>(o, a, db, 1u);
 }
 
-// DOC (document mask): doc_start [B*S] holds the first row of each row's document (rows of one sequence). Query q sees key k
-// iff doc_start[q] <= k <= q. Key tiles that end before the document of the tile's first row are never loaded.
+// BOUND: every query row q has a lower bound lo(q) on its keys, and query q sees key k iff lo(q) <= k <= q (causal only).
+// lo(q) = max(doc_start[q], q - window): doc_start [B*S] (optional, the document mask) holds the first row of each row's
+// document (rows of one sequence); window is the sliding-window size (>= S when off). lo is non-decreasing along a sequence,
+// so key tiles that end before lo of the tile's first row are never loaded.
 // GQA: HKV < H (grouped-query attention); false compiles the multi-head kernel (HKV == H, the kv head is the query head).
-template <int DH, bool ALIBI, bool DOC, bool GQA>
+template <int DH, bool ALIBI, bool BOUND, bool GQA>
 __global__ void __launch_bounds__(384, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __restrict__ out, float* __restrict__ lse, int S, int H,
-                float scale, int causal, const float* __restrict__ alibi_slopes, const int* __restrict__ doc_start, int HKV) {
+                float scale, int causal, const float* __restrict__ alibi_slopes, const int* __restrict__ doc_start, int HKV, int window) {
   using C = FwdCfg<DH>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -86,7 +88,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __rest
   const int k_col = GQA ? d_model + h / (H / HKV) * DH : d_model + h * DH;
   const int v_col = GQA ? k_col + HKV * DH : 2 * d_model + h * DH;
   const int n_kv = causal ? qt + 1 : S / BKV;
-  const int j0 = DOC ? doc_start[b * S + qt * BQ] / BKV : 0;   // first key tile any row of this query tile sees
+  const auto lo_of = [&](int q) { return max(doc_start ? doc_start[b * S + q] : 0, q - window); };
+  const int j0 = BOUND ? lo_of(qt * BQ) / BKV : 0;   // first key tile any row of this query tile sees
   const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
 
@@ -140,12 +143,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __rest
 #pragma unroll
   for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
   float sacc[64];
-  // DOC: first visible key of this thread's two rows, and of the tile's last row (the largest, ids being runs): key tiles
-  // starting at or after the latter need no document mask
+  // BOUND: first visible key of this thread's two rows, and of the tile's last row (the largest): key tiles starting at or
+  // after the latter need no mask below the diagonal
   int dstart[2] = {0, 0}, dstart_last = 0;
-  if (DOC) {
-    dstart[0] = doc_start[b * S + qrow0], dstart[1] = doc_start[b * S + qrow0 + 8];
-    dstart_last = doc_start[b * S + qt * BQ + BQ - 1];
+  if (BOUND) {
+    dstart[0] = lo_of(qrow0), dstart[1] = lo_of(qrow0 + 8);
+    dstart_last = lo_of(qt * BQ + BQ - 1);
   }
   mbar_wait(q_full, 0);
   for (int j = j0; j < n_kv; ++j) {
@@ -167,7 +170,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __rest
     if (lane == 0) mbar_arrive(&k_empty[st]);
     // scaled (log2-domain) scores, causal mask on the diagonal tile, ALiBi bias slope * (key - query)
     const bool diag = causal && j == qt;
-    const bool dmask = DOC && j * BKV < dstart_last;
+    const bool dmask = BOUND && j * BKV < dstart_last;
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int j8 = 0; j8 < 16; ++j8) {
@@ -191,7 +194,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __rest
       mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffff, mx[hh], 1));
       mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffff, mx[hh], 2));
       const float m_new = fmaxf(m[hh], mx[hh]);
-      if constexpr (DOC) {
+      if constexpr (BOUND) {
         // a row can meet a tile with no visible key before its first one (m_new = -inf); subtracting 0 there keeps
         // exp2(-inf - -inf) = NaN out of alpha and P (both become 0, and l, O are still 0)
         msub[hh] = m_new == -INFINITY ? 0.f : m_new;
@@ -207,7 +210,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __rest
     for (int j8 = 0; j8 < 16; ++j8) {
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const float pv = exp2f(sacc[4 * j8 + e] - (DOC ? msub[e >> 1] : m[e >> 1]));
+        const float pv = exp2f(sacc[4 * j8 + e] - (BOUND ? msub[e >> 1] : m[e >> 1]));
         sacc[4 * j8 + e] = pv;
         l[e >> 1] += pv;
       }
@@ -319,14 +322,15 @@ __device__ __forceinline__ void wgmma_ss_kmajor(float (&d)[N / 2], uint64_t da, 
   else wgmma_bf16_ss_n64<0, 0>(d, da, db, scale_d);
 }
 
-// DOC: as in the forward; doc_end [B*S] holds the last row of each row's document, so the query walk of a key tile stops at
-// the step holding the end of its last key's document. GQA: as in the forward.
-template <int DH, bool ALIBI, bool DOC, bool GQA>
+// BOUND: as in the forward, read from the key's side: key k is seen by queries k .. hi(k), hi(k) = min(doc_end[k], k + window),
+// with doc_end [B*S] (present iff doc_start is) the last row of each row's document, so the query walk of a key tile stops at
+// the step holding hi of its last key. GQA: as in the forward.
+template <int DH, bool ALIBI, bool BOUND, bool GQA>
 __global__ void __launch_bounds__(384, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
                 const __grid_constant__ CUtensorMap tmDQ, const float* __restrict__ lse, const float* __restrict__ delta,
                 __nv_bfloat16* __restrict__ dqkv, int S, int H, float scale, int causal, const float* __restrict__ alibi_slopes,
-                const int* __restrict__ doc_start, const int* __restrict__ doc_end, int HKV) {
+                const int* __restrict__ doc_start, const int* __restrict__ doc_end, int HKV, int window) {
   using C = BwdCfg<DH>;
   constexpr int BQS = C::BQS;
   extern __shared__ uint8_t smem_raw[];
@@ -350,7 +354,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
   const int d_model = H * DH;
   const int k_col = d_model + hk * DH, v_col = GQA ? k_col + HKV * DH : 2 * d_model + hk * DH;
   const int i0 = causal ? jt * (128 / BQS) : 0;            // query steps of BQS rows
-  const int n_q = DOC ? doc_end[b * S + jt * 128 + 127] / BQS + 1 : S / BQS;
+  const int n_q = BOUND ? min(doc_end ? doc_end[b * S + jt * 128 + 127] : S - 1, jt * 128 + 127 + window) / BQS + 1 : S / BQS;
+  const bool doc = BOUND && doc_start != nullptr;
   const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
 
@@ -381,7 +386,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
         for (int i = i0; i < n_q; ++i) {
           const int n = (h - h0) * (n_q - i0) + i - i0, st = n & 1;   // (query head, query step) items in walk order
           mbar_wait(&q_empty[st], ((n >> 1) & 1) ^ 1);
-          mbar_expect_tx(&q_full[st], 2 * C::QT + (DOC ? 3 : 2) * BQS * 4);
+          mbar_expect_tx(&q_full[st], 2 * C::QT + (doc ? 3 : 2) * BQS * 4);
 #pragma unroll
           for (int c = 0; c < C::CH; ++c) {
             tma_load_2d(sQ + st * C::QT + c * C::QC, &tmQ, &q_full[st], h * DH + c * 64, b * S + i * BQS);
@@ -391,7 +396,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
           uint8_t* rs_st = sRS + st * C::RS;
           bulk_load(rs_st, lse + row, BQS * 4, &q_full[st]);
           bulk_load(rs_st + BQS * 4, delta + row, BQS * 4, &q_full[st]);
-          if (DOC) bulk_load(rs_st + 2 * BQS * 4, doc_start + (long long)b * S + i * BQS, BQS * 4, &q_full[st]);
+          if (doc) bulk_load(rs_st + 2 * BQS * 4, doc_start + (long long)b * S + i * BQS, BQS * 4, &q_full[st]);
         }
       }
     }
@@ -448,7 +453,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
         const int qa = q0 + 8 * j8 + 2 * t4;
         const float2 L = ld_shared_f32x2(rs + 32 * j8);
         const float2 D = ld_shared_f32x2(rs + BQS * 4 + 32 * j8);
-        const int2 DS = DOC ? ld_shared_s32x2(rs + 2 * BQS * 4 + 32 * j8) : make_int2(0, 0);
+        const int2 DS = doc ? ld_shared_s32x2(rs + 2 * BQS * 4 + 32 * j8) : make_int2(0, 0);
         float pv[4], dsv[4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
@@ -457,11 +462,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant_
           if (ALIBI) x = fmaf(slope2, float(key - q), x);
           float pr = exp2f(x);
           if (diag && q < key) pr = 0.f;
-          if (DOC && ((e & 1) ? DS.y : DS.x) > key) pr = 0.f;
+          if (BOUND && max((e & 1) ? DS.y : DS.x, q - window) > key) pr = 0.f;
           pv[e] = pr;
           dsv[e] = pr * (dp[4 * j8 + e] - ((e & 1) ? D.y : D.x));
-          // a masked query of another document may carry a non-finite delta (its own keys' fault): keep it out of dK
-          if (DOC && pr == 0.f) dsv[e] = 0.f;
+          // a masked query (another document, or past the key's window) may carry a non-finite delta (its own keys' fault):
+          // keep it out of dK
+          if (BOUND && pr == 0.f) dsv[e] = 0.f;
         }
         // accumulator columns 16 kc .. 16 kc + 15 (queries) are the A fragment of k-step kc
         const int kc = j8 >> 1, hi = (j8 & 1) * 2;
@@ -596,10 +602,16 @@ __global__ void __launch_bounds__(DOC_THREADS) doc_bounds_kernel(const long long
 
 }  // namespace
 
+// a window that leaves some query a key it cannot see (window < S - 1) runs the bounded instances; a wider one is plain
+// causal attention and runs the causal instances. The kernels take the window as >= S when it is off.
+static bool window_binds(int window, int S) { return window >= 0 && window < S - 1; }
+
 void attention_fwd_launch(const void* qkv, void* out, float* lse, int B, int S, int H, int Hkv, int dh, float scale, bool causal,
-                          cudaStream_t st, const float* alibi_slopes, const int* doc_start) {
+                          cudaStream_t st, const float* alibi_slopes, const int* doc_start, int window) {
   if (S % 128) throw std::runtime_error("photon_b200 attention: sequence length must be a multiple of 128");
   if (dh != 64 && dh != 128) throw std::runtime_error("photon_b200 attention: d_head must be 64 or 128");
+  if (window >= 0 && !causal) throw std::runtime_error("photon_b200 attention: a sliding window needs the causal mask");
+  const bool win = window_binds(window, S);
   const uint64_t w = uint64_t(H + 2 * Hkv) * dh;   // fused qkv row width
   CUtensorMap tm = make_tmap_2d(qkv, 2, false, w, uint64_t(B) * S, w * 2, 64, 128);
   const dim3 grid(S / 128, B * H);
@@ -607,16 +619,19 @@ void attention_fwd_launch(const void* qkv, void* out, float* lse, int B, int S, 
     constexpr int DHV = wide ? 128 : 64;
     auto kern = attn_fwd_kernel<DHV, alibi, doc, gqa>;
     opt_in_smem(kern, FwdCfg<DHV>::SMEM);
-    kern<<<grid, 384, FwdCfg<DHV>::SMEM, st>>>(tm, (__nv_bfloat16*)out, lse, S, H, scale, causal ? 1 : 0, alibi_slopes, doc_start, Hkv);
-  }, Hkv != H, alibi_slopes != nullptr, dh == 128, doc_start != nullptr);
+    kern<<<grid, 384, FwdCfg<DHV>::SMEM, st>>>(tm, (__nv_bfloat16*)out, lse, S, H, scale, causal ? 1 : 0, alibi_slopes, doc_start, Hkv,
+                                               win ? window : S);
+  }, Hkv != H, alibi_slopes != nullptr, dh == 128, doc_start != nullptr || win);
   launched("attention fwd");
 }
 
 void attention_bwd_launch(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta, float* dq_acc,
                           int B, int S, int H, int Hkv, int dh, float scale, bool causal, int num_sms, cudaStream_t st, const float* alibi_slopes,
-                          const int* doc_start, const int* doc_end) {
+                          const int* doc_start, const int* doc_end, int window) {
   if (S % 128) throw std::runtime_error("photon_b200 attention: sequence length must be a multiple of 128");
   if (dh != 64 && dh != 128) throw std::runtime_error("photon_b200 attention backward: d_head must be 64 or 128");
+  if (window >= 0 && !causal) throw std::runtime_error("photon_b200 attention backward: a sliding window needs the causal mask");
+  const bool win = window_binds(window, S);
   const int sms = num_sms > 0 ? num_sms : 132;
   const int d = H * dh;
   const uint64_t w = uint64_t(H + 2 * Hkv) * dh;   // fused qkv row width
@@ -642,8 +657,8 @@ void attention_bwd_launch(const void* qkv, const void* out, const void* dout, co
     auto kern = attn_bwd_kernel<DHV, alibi, doc, gqa>;
     opt_in_smem(kern, C::SMEM);
     kern<<<grid, 384, C::SMEM, st>>>(tmKV, tmQ, tmDO, tmDQ, lse, delta, (__nv_bfloat16*)dqkv, S, H, scale, causal ? 1 : 0, alibi_slopes,
-                                     doc_start, doc_end, Hkv);
-  }, Hkv != H, alibi_slopes != nullptr, dh == 128, doc_start != nullptr);
+                                     doc_start, doc_end, Hkv, win ? window : S);
+  }, Hkv != H, alibi_slopes != nullptr, dh == 128, doc_start != nullptr || win);
   launched("attention bwd");
   attn_bwd_dq_convert_kernel<<<sms * 8, 256, 0, st>>>(dq_acc, (__nv_bfloat16*)dqkv, rows, d, int(w), scale);
   launched("attention bwd dq convert");

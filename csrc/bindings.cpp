@@ -328,22 +328,28 @@ void check_doc_args(const Tensor& qkv, bool causal, const c10::optional<Tensor>&
   check_doc_bound(doc_start, "doc_start", qkv);
   check_doc_bound(doc_end, "doc_end", qkv);
 }
+// sliding window: -1 = off, otherwise query q sees keys q - window .. q; only with the causal mask
+void check_window(int window, bool causal, const char* op) {
+  TORCH_CHECK(window >= -1, op, ": sliding window ", window, " must be -1 (off) or >= 0");
+  TORCH_CHECK(window == -1 || causal, op, ": a sliding window is only supported with the causal mask");
+}
 void attention_fwd(const Tensor& qkv, Tensor& out, Tensor& lse, int n_heads, double scale, bool causal,
-                   const c10::optional<Tensor>& alibi_slopes, const c10::optional<Tensor>& doc_start, int n_kv_heads) {
+                   const c10::optional<Tensor>& alibi_slopes, const c10::optional<Tensor>& doc_start, int n_kv_heads, int window) {
   check_bf16(qkv, "qkv");
   check_bf16(out, "out");
   check_f32(lse, "lse");
   n_kv_heads = kv_heads(n_heads, n_kv_heads);
   check_attention_args(qkv, out, lse, n_heads, n_kv_heads, causal, alibi_slopes);
   check_doc_args(qkv, causal, doc_start, c10::nullopt);
+  check_window(window, causal, "attention_fwd");
   c10::cuda::CUDAGuard guard(qkv.device());
   const int B = int(qkv.size(0)), S = int(qkv.size(1)), dh = int(qkv.size(2) / (n_heads + 2 * n_kv_heads));
   pb::attention_fwd_launch(qkv.data_ptr(), out.data_ptr(), lse.data_ptr<float>(), B, S, n_heads, n_kv_heads, dh, float(scale), causal,
-                           stream_of(qkv), opt_ptr<float>(alibi_slopes), opt_ptr<int>(doc_start));
+                           stream_of(qkv), opt_ptr<float>(alibi_slopes), opt_ptr<int>(doc_start), window);
 }
 void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, const Tensor& lse, Tensor& dqkv, Tensor& delta,
                    int n_heads, double scale, bool causal, const c10::optional<Tensor>& alibi_slopes,
-                   const c10::optional<Tensor>& doc_start, const c10::optional<Tensor>& doc_end, int n_kv_heads) {
+                   const c10::optional<Tensor>& doc_start, const c10::optional<Tensor>& doc_end, int n_kv_heads, int window) {
   check_bf16(qkv, "qkv");
   check_bf16(out, "out");
   check_bf16(dout, "dout");
@@ -354,6 +360,7 @@ void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, con
   check_attention_args(qkv, out, lse, n_heads, n_kv_heads, causal, alibi_slopes);
   check_doc_args(qkv, causal, doc_start, doc_end);
   TORCH_CHECK(doc_start.has_value() == doc_end.has_value(), "attention_bwd: doc_start needs doc_end");
+  check_window(window, causal, "attention_bwd");
   TORCH_CHECK(dout.is_contiguous() && dout.sizes() == out.sizes(), "dout must be contiguous [B,S,d]");
   TORCH_CHECK(delta.is_contiguous() && delta.sizes() == lse.sizes(), "delta must be contiguous float32 [B,H,S]");
   TORCH_CHECK(dqkv.is_contiguous() && dqkv.sizes() == qkv.sizes(), "dqkv must be contiguous and shaped like qkv");
@@ -364,7 +371,7 @@ void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, con
   Tensor dq_acc = at::empty({(int64_t)B * S, d}, qkv.options().dtype(at::kFloat));
   pb::attention_bwd_launch(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr<float>(), dqkv.data_ptr(), delta.data_ptr<float>(),
                            dq_acc.data_ptr<float>(), B, S, n_heads, n_kv_heads, dh, float(scale), causal, num_sms(), stream_of(qkv),
-                           opt_ptr<float>(alibi_slopes), opt_ptr<int>(doc_start), opt_ptr<int>(doc_end));
+                           opt_ptr<float>(alibi_slopes), opt_ptr<int>(doc_start), opt_ptr<int>(doc_end), window);
 }
 // sequence_id int64 [B,S] -> doc_start / doc_end int32 [B*S] (first / last row of each row's document)
 void doc_bounds(const Tensor& sequence_id, Tensor& doc_start, Tensor& doc_end) {
@@ -450,7 +457,7 @@ void skinny_gemm(const Tensor& x, const Tensor& w, Tensor& y, const c10::optiona
 }
 // kc / vc: one layer of the cache, [B_max, Hkv, S_max, dh]; q: rows of [B, >= H*dh] (the q heads of the fused qkv)
 void decode_attention(const Tensor& q, const Tensor& kc, const Tensor& vc, const Tensor& pos, Tensor& out, int n_heads, double scale,
-                      const c10::optional<Tensor>& alibi_slopes, int n_kv_heads) {
+                      const c10::optional<Tensor>& alibi_slopes, int n_kv_heads, int window) {
   check_bf16(q, "q");
   check_bf16(out, "out");
   check_i32(pos, "pos");
@@ -465,13 +472,14 @@ void decode_attention(const Tensor& q, const Tensor& kc, const Tensor& vc, const
     check_f32(*alibi_slopes, "alibi_slopes");
     TORCH_CHECK(alibi_slopes->numel() == n_heads, "alibi_slopes must have n_heads elements");
   }
+  check_window(window, true, "decode_attention");
   c10::cuda::CUDAGuard guard(q.device());
   const int splits = pb::decode_attention_splits(S);
   Tensor po = torch::empty({(long long)B * H * splits * dh}, q.options().dtype(at::kFloat));
   Tensor pml = torch::empty({(long long)B * H * splits * 2}, q.options().dtype(at::kFloat));
   pb::decode_attention_launch(q.data_ptr(), q.stride(0), kc.data_ptr(), vc.data_ptr(), pos.data_ptr<int>(), out.data_ptr(), out.stride(0),
                               po.data_ptr<float>(), pml.data_ptr<float>(), B, H, Hkv, dh, S, float(scale), opt_ptr<float>(alibi_slopes),
-                              stream_of(q));
+                              stream_of(q), window);
 }
 void decode_append(Tensor& qkv, const Tensor& pos, Tensor& kc, Tensor& vc, const c10::optional<Tensor>& cos_t,
                    const c10::optional<Tensor>& sin_t, int n_heads, const c10::optional<Tensor>& slot, int n_kv_heads) {
@@ -502,7 +510,7 @@ void decode_append(Tensor& qkv, const Tensor& pos, Tensor& kc, Tensor& vc, const
 }
 // query rows of qkv [N, (H+2*Hkv)*dh] in tiles (int32 [T, 4]: slot, first_row, n_rows <= 64, first_pos) against one cache layer
 void cache_attention(const Tensor& qkv, const Tensor& kc, const Tensor& vc, const Tensor& tiles, Tensor& out, int n_heads, double scale,
-                     const c10::optional<Tensor>& alibi_slopes, int n_kv_heads) {
+                     const c10::optional<Tensor>& alibi_slopes, int n_kv_heads, int window) {
   check_bf16(qkv, "qkv");
   check_bf16(out, "out");
   check_i32(tiles, "tiles");
@@ -520,10 +528,11 @@ void cache_attention(const Tensor& qkv, const Tensor& kc, const Tensor& vc, cons
     check_f32(*alibi_slopes, "alibi_slopes");
     TORCH_CHECK(alibi_slopes->numel() == n_heads, "alibi_slopes must have n_heads elements");
   }
+  check_window(window, true, "cache_attention");
   c10::cuda::CUDAGuard guard(qkv.device());
   pb::cache_attention_launch(qkv.data_ptr(), qkv.stride(0), qkv.size(0), kc.data_ptr(), vc.data_ptr(), tiles.data_ptr<int>(),
                              int(tiles.size(0)), out.data_ptr(), out.stride(0), Bm, H, Hkv, dh, S, float(scale), opt_ptr<float>(alibi_slopes),
-                             stream_of(qkv));
+                             stream_of(qkv), window);
 }
 void embed_pos(const Tensor& ids, const Tensor& pos, const Tensor& wte, const c10::optional<Tensor>& wpe, Tensor& out) {
   check_i32(ids, "ids");
@@ -993,21 +1002,22 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fp8_quantize_segments", &fp8_quantize_segments);
   m.def("fp8_update_scales", &fp8_update_scales);
   m.def("attention_fwd", &attention_fwd, py::arg("qkv"), py::arg("out"), py::arg("lse"), py::arg("n_heads"), py::arg("scale"),
-        py::arg("causal"), py::arg("alibi_slopes") = py::none(), py::arg("doc_start") = py::none(), py::arg("n_kv_heads") = -1);
+        py::arg("causal"), py::arg("alibi_slopes") = py::none(), py::arg("doc_start") = py::none(), py::arg("n_kv_heads") = -1,
+        py::arg("window") = -1);
   m.def("attention_bwd", &attention_bwd, py::arg("qkv"), py::arg("out"), py::arg("dout"), py::arg("lse"), py::arg("dqkv"), py::arg("delta"),
         py::arg("n_heads"), py::arg("scale"), py::arg("causal"), py::arg("alibi_slopes") = py::none(), py::arg("doc_start") = py::none(),
-        py::arg("doc_end") = py::none(), py::arg("n_kv_heads") = -1);
+        py::arg("doc_end") = py::none(), py::arg("n_kv_heads") = -1, py::arg("window") = -1);
   m.def("doc_bounds", &doc_bounds, py::arg("sequence_id"), py::arg("doc_start"), py::arg("doc_end"));
   m.def("rope", &rope, py::arg("qkv"), py::arg("cos"), py::arg("sin"), py::arg("n_heads"), py::arg("inverse"), py::arg("n_kv_heads") = -1);
   m.def("embed_fwd", &embed_fwd);
   m.def("skinny_gemm", &skinny_gemm, py::arg("x"), py::arg("w"), py::arg("y"), py::arg("bias") = py::none(), py::arg("residual") = py::none(),
         py::arg("epi") = 0);
   m.def("decode_attention", &decode_attention, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("pos"), py::arg("out"),
-        py::arg("n_heads"), py::arg("scale"), py::arg("alibi_slopes") = py::none(), py::arg("n_kv_heads") = -1);
+        py::arg("n_heads"), py::arg("scale"), py::arg("alibi_slopes") = py::none(), py::arg("n_kv_heads") = -1, py::arg("window") = -1);
   m.def("decode_append", &decode_append, py::arg("qkv"), py::arg("pos"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cos") = py::none(),
         py::arg("sin") = py::none(), py::arg("n_heads") = 1, py::arg("slot") = py::none(), py::arg("n_kv_heads") = -1);
   m.def("cache_attention", &cache_attention, py::arg("qkv"), py::arg("k_cache"), py::arg("v_cache"), py::arg("tiles"), py::arg("out"),
-        py::arg("n_heads"), py::arg("scale"), py::arg("alibi_slopes") = py::none(), py::arg("n_kv_heads") = -1);
+        py::arg("n_heads"), py::arg("scale"), py::arg("alibi_slopes") = py::none(), py::arg("n_kv_heads") = -1, py::arg("window") = -1);
   m.def("embed_pos", &embed_pos, py::arg("ids"), py::arg("pos"), py::arg("wte"), py::arg("wpe"), py::arg("out"));
   m.def("argmax_advance", &argmax_advance, py::arg("logits"), py::arg("ids"), py::arg("pos") = py::none());
   m.def("embed_bwd", &embed_bwd);

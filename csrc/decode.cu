@@ -205,11 +205,13 @@ __device__ __forceinline__ float da_warp_sum(float v) {
 // One CTA = one (chunk, kv head, sequence). The G = H / HKV query heads of the kv head are taken NG at a time: each pass loads
 // the chunk's key rows once and scores them against the pass's NG queries, then its value rows once for the NG weighted sums
 // (G <= NG: every cached row of the chunk is read once). Per query head the arithmetic is that of one head alone.
-template <int DH, bool ALIBI, int NG>
+// WIN: sliding window, the query sees keys lo .. pos[b] with lo = max(0, pos[b] - window); chunks wholly below lo return at
+// once, and the chunk holding lo masks the keys below it.
+template <int DH, bool ALIBI, int NG, bool WIN>
 __global__ void __launch_bounds__(DA_THREADS)
 decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __nv_bfloat16* __restrict__ kc,
                    const __nv_bfloat16* __restrict__ vc, const int* __restrict__ pos, float* __restrict__ po, float* __restrict__ pml,
-                   int H, int HKV, int s_max, int n_split, float sc, const float* __restrict__ slopes) {
+                   int H, int HKV, int s_max, int n_split, float sc, const float* __restrict__ slopes, int window) {
   __shared__ float qs[NG][DH];
   __shared__ float ps[NG][DA_CHUNK];
   __shared__ float red[2][NG][4];
@@ -219,6 +221,8 @@ decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __n
   const int len = pos[b] + 1;
   const int j0 = s * DA_CHUNK, j1 = min(len, j0 + DA_CHUNK);
   if (j0 >= j1) return;   // chunk past the sequence: the combine kernel reads only the chunks below pos[b] + 1
+  const int lo = WIN ? max(0, pos[b] - window) : 0;
+  if (WIN && j1 <= lo) return;   // chunk below the window: the combine kernel reads only the chunks from lo on
   const int G = H / HKV;
   const long long head = (long long)(b * HKV + hk) * s_max * DH;
   constexpr int PER = DH / 32;
@@ -241,7 +245,7 @@ decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __n
       float x[NG];
 #pragma unroll
       for (int g = 0; g < NG; ++g) x[g] = -INFINITY;
-      if (j < j1) {
+      if (j < j1 && (!WIN || j >= lo)) {
         const uint4* kr = reinterpret_cast<const uint4*>(kc + head + (long long)j * DH);
         float acc[NG];
 #pragma unroll
@@ -288,7 +292,7 @@ decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __n
     for (int jj = tid; jj < DA_CHUNK; jj += DA_THREADS) {
 #pragma unroll
       for (int g = 0; g < NG; ++g) {
-        const float pv = (j0 + jj < j1) ? exp2f(ps[g][jj] - m[g]) : 0.f;
+        const float pv = (j0 + jj < j1 && (!WIN || j0 + jj >= lo)) ? exp2f(ps[g][jj] - m[g]) : 0.f;
         ps[g][jj] = pv;
         l[g] += pv;
       }
@@ -305,7 +309,7 @@ decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __n
     for (int g = 0; g < NG; ++g)
 #pragma unroll
       for (int i = 0; i < PER; ++i) o[g][i] = 0.f;
-    for (int jj = warp; jj < j1 - j0; jj += 4) {
+    for (int jj = (WIN ? max(lo - j0, 0) : 0) + warp; jj < j1 - j0; jj += 4) {
       const __nv_bfloat16* vr = vc + head + (long long)(j0 + jj) * DH + lane * PER;
       float f[PER];
       if constexpr (PER == 2) {
@@ -342,17 +346,18 @@ decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __n
   }
 }
 
-template <int DH>
+template <int DH, bool WIN>
 __global__ void __launch_bounds__(DH) decode_combine_kernel(const float* __restrict__ po, const float* __restrict__ pml,
                                                             const int* __restrict__ pos, __nv_bfloat16* __restrict__ out, long long ldo,
-                                                            int H, int n_split) {
+                                                            int H, int n_split, int window) {
   const int h = blockIdx.x, b = blockIdx.y, t = threadIdx.x;
   const int used = (pos[b] + 1 + DA_CHUNK - 1) / DA_CHUNK;
+  const int first = WIN ? max(0, pos[b] - window) / DA_CHUNK : 0;   // the chunk holding the window's first key
   const long long slot0 = (long long)(b * H + h) * n_split;
   float M = -INFINITY;
-  for (int s = 0; s < used; ++s) M = fmaxf(M, pml[2 * (slot0 + s)]);
+  for (int s = first; s < used; ++s) M = fmaxf(M, pml[2 * (slot0 + s)]);
   float L = 0.f, o = 0.f;
-  for (int s = 0; s < used; ++s) {
+  for (int s = first; s < used; ++s) {
     const float w = exp2f(pml[2 * (slot0 + s)] - M);
     L = fmaf(w, pml[2 * (slot0 + s) + 1], L);
     o = fmaf(w, po[(slot0 + s) * DH + t], o);
@@ -378,12 +383,14 @@ struct CaCfg {
   static_assert(SMEM <= 232448, "smem budget");
 };
 
-template <int DH, bool ALIBI>
+// WIN: sliding window, the row at position p sees keys max(0, p - window) .. p; the key-tile walk starts at the tile holding
+// the first row's first key.
+template <int DH, bool ALIBI, bool WIN>
 __global__ void __launch_bounds__(CA_THREADS)
 cache_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                   const int4* __restrict__ tiles, __nv_bfloat16* __restrict__ out, long long ldo, long long n_q, int H, int HKV, int s_max,
                   float sc,
-                  const float* __restrict__ slopes) {
+                  const float* __restrict__ slopes, int window) {
   using C = CaCfg<DH>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -399,6 +406,7 @@ cache_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   const int4 tile = tiles[blockIdx.x];  // (slot, first_row, n_rows, first_pos)
   const int h = blockIdx.y;
   const int n_kv = (tile.w + tile.z - 1) / CA_BKV + 1;   // key tiles up to the last row's position
+  const int j0 = WIN ? max(0, tile.w - window) / CA_BKV : 0;
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
     for (int s = 0; s < 2; ++s) {
@@ -421,9 +429,9 @@ cache_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
       mbar_expect_tx(q_full, C::Q_BYTES);   // rows past the last qkv row arrive as zeros
 #pragma unroll
       for (int c = 0; c < C::CH; ++c) tma_load_2d(sQ + c * 8192, &tmQ, q_full, h * DH + c * 64, tile.y);
-      for (int j = 0; j < n_kv; ++j) {
-        const int st = j & 1;
-        const uint32_t ph = ((j >> 1) & 1) ^ 1;
+      for (int j = j0; j < n_kv; ++j) {
+        const int st = (j - j0) & 1;
+        const uint32_t ph = (((j - j0) >> 1) & 1) ^ 1;
         mbar_wait(&k_empty[st], ph);
         mbar_expect_tx(&k_full[st], C::KV_BYTES);
 #pragma unroll
@@ -448,9 +456,9 @@ cache_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
   float s[64];
   mbar_wait(q_full, 0);
-  for (int j = 0; j < n_kv; ++j) {
-    const int st = j & 1;
-    const uint32_t ph = (j >> 1) & 1;
+  for (int j = j0; j < n_kv; ++j) {
+    const int st = (j - j0) & 1;
+    const uint32_t ph = ((j - j0) >> 1) & 1;
     mbar_wait(&k_full[st], ph);
     wgmma_fence();
 #pragma unroll
@@ -464,7 +472,8 @@ cache_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
     wgmma_fence_regs(s);
     __syncwarp();
     if (lane == 0) mbar_arrive(&k_empty[st]);
-    // row r (position first_pos + r) sees keys 0 .. first_pos + r; key 0 is always visible, so m is finite after tile 0
+    // row r (position first_pos + r) sees keys 0 .. first_pos + r; key 0 is always visible, so m is finite after tile 0.
+    // WIN: keys from first_pos + r - window on; a row can meet a tile with none of them (guarded below)
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int j8 = 0; j8 < 16; ++j8) {
@@ -476,17 +485,25 @@ cache_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
         float x = s[4 * j8 + e] * sc;
         if (ALIBI) x = fmaf(slope2, float(key - qpos), x);
         if (key > qpos) x = -INFINITY;
+        if (WIN && key < qpos - window) x = -INFINITY;
         s[4 * j8 + e] = x;
         mx[hh] = fmaxf(mx[hh], x);
       }
     }
     float alpha[2];
+    [[maybe_unused]] float msub[2];
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffff, mx[hh], 1));
       mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffff, mx[hh], 2));
       const float m_new = fmaxf(m[hh], mx[hh]);
-      alpha[hh] = exp2f(m[hh] - m_new);
+      if constexpr (WIN) {
+        // no visible key yet (m_new = -inf): subtracting 0 keeps exp2(-inf - -inf) = NaN out of alpha and P
+        msub[hh] = m_new == -INFINITY ? 0.f : m_new;
+        alpha[hh] = exp2f(m[hh] - msub[hh]);
+      } else {
+        alpha[hh] = exp2f(m[hh] - m_new);
+      }
       m[hh] = m_new;
       l[hh] *= alpha[hh];
     }
@@ -496,8 +513,8 @@ cache_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
     for (int kc = 0; kc < 8; ++kc) {
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        const float p0 = exp2f(s[8 * kc + 2 * q] - m[q & 1]);
-        const float p1 = exp2f(s[8 * kc + 2 * q + 1] - m[q & 1]);
+        const float p0 = exp2f(s[8 * kc + 2 * q] - (WIN ? msub[q & 1] : m[q & 1]));
+        const float p1 = exp2f(s[8 * kc + 2 * q + 1] - (WIN ? msub[q & 1] : m[q & 1]));
         l[q & 1] += p0 + p1;
         pa[kc][q] = pack_bf16(p0, p1);
       }
@@ -682,7 +699,7 @@ int decode_attention_splits(int s_max) { return (s_max + DA_CHUNK - 1) / DA_CHUN
 
 void decode_attention_launch(const void* q, long long ldq, const void* kc, const void* vc, const int* pos, void* out, long long ldo,
                              float* partial_o, float* partial_ml, int B, int H, int Hkv, int dh, int s_max, float scale,
-                             const float* alibi_slopes, cudaStream_t st) {
+                             const float* alibi_slopes, cudaStream_t st, int window) {
   if (B < 1) return;
   const int n_split = decode_attention_splits(s_max);
   const dim3 grid(n_split, Hkv, B);
@@ -691,21 +708,21 @@ void decode_attention_launch(const void* q, long long ldq, const void* kc, const
   const auto* kk = (const __nv_bfloat16*)kc;
   const auto* vv = (const __nv_bfloat16*)vc;
   const float sc = scale * LOG2E;
-  with_bools([&](auto alibi, auto wide) {
+  with_bools([&](auto alibi, auto wide, auto win) {
     constexpr int D = wide ? 128 : 64;
     // the G query heads of a kv head are scored NG at a time
     const auto attn = [&](auto NG) {
-      decode_attn_kernel<D, alibi, NG><<<grid, DA_THREADS, 0, st>>>(qq, ldq, kk, vv, pos, partial_o, partial_ml, H, Hkv, s_max, n_split, sc,
-                                                                   alibi_slopes);
+      decode_attn_kernel<D, alibi, NG, win><<<grid, DA_THREADS, 0, st>>>(qq, ldq, kk, vv, pos, partial_o, partial_ml, H, Hkv, s_max, n_split,
+                                                                        sc, alibi_slopes, window);
     };
     if (G == 1) attn(std::integral_constant<int, 1>{});
     else if (G == 2) attn(std::integral_constant<int, 2>{});
     else if (G <= 4) attn(std::integral_constant<int, 4>{});
     else attn(std::integral_constant<int, 8>{});
     launched("decode attention");
-    decode_combine_kernel<D><<<dim3(H, B), D, 0, st>>>(partial_o, partial_ml, pos, (__nv_bfloat16*)out, ldo, H, n_split);
+    decode_combine_kernel<D, win><<<dim3(H, B), D, 0, st>>>(partial_o, partial_ml, pos, (__nv_bfloat16*)out, ldo, H, n_split, window);
     launched("decode attention combine");
-  }, alibi_slopes != nullptr, dh == 128);
+  }, alibi_slopes != nullptr, dh == 128, window >= 0 && window < s_max - 1);   // a wider window sees every cached key
 }
 
 void decode_append_launch(void* qkv, long long ldqkv, const int* pos, void* kc, void* vc, const float* cosT, const float* sinT, int B,
@@ -719,7 +736,7 @@ void decode_append_launch(void* qkv, long long ldqkv, const int* pos, void* kc, 
 
 void cache_attention_launch(const void* qkv, long long ldq, long long n_q, const void* kc, const void* vc, const int* tiles, int n_tiles,
                             void* out, long long ldo, int B_max, int H, int Hkv, int dh, int s_max, float scale,
-                            const float* alibi_slopes, cudaStream_t st) {
+                            const float* alibi_slopes, cudaStream_t st, int window) {
   if (n_tiles < 1 || n_q < 1) return;
   const long long kv_rows = (long long)B_max * Hkv * s_max;
   if (kv_rows >= (1LL << 31)) throw std::runtime_error("photon_b200 cache attention: the cache has more than 2^31 rows per layer");
@@ -729,12 +746,12 @@ void cache_attention_launch(const void* qkv, long long ldq, long long n_q, const
   const dim3 grid(n_tiles, H);
   const auto* tt = reinterpret_cast<const int4*>(tiles);
   const float sc = scale * LOG2E;
-  with_bools([&](auto alibi, auto wide) {
+  with_bools([&](auto alibi, auto wide, auto win) {
     constexpr int D = wide ? 128 : 64;
-    auto kern = cache_attn_kernel<D, alibi>;
+    auto kern = cache_attn_kernel<D, alibi, win>;
     opt_in_smem(kern, CaCfg<D>::SMEM);
-    kern<<<grid, CA_THREADS, CaCfg<D>::SMEM, st>>>(tq, tk, tv, tt, (__nv_bfloat16*)out, ldo, n_q, H, Hkv, s_max, sc, alibi_slopes);
-  }, alibi_slopes != nullptr, dh == 128);
+    kern<<<grid, CA_THREADS, CaCfg<D>::SMEM, st>>>(tq, tk, tv, tt, (__nv_bfloat16*)out, ldo, n_q, H, Hkv, s_max, sc, alibi_slopes, window);
+  }, alibi_slopes != nullptr, dh == 128, window >= 0 && window < s_max - 1);   // a wider window sees every cached key
   launched("cache attention");
 }
 

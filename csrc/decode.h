@@ -44,11 +44,12 @@ void skinny_gemm_launch(const SkinnyArgs& a, float* partials, cudaStream_t st);
 
 // Number of KV chunks (one CTA each per sequence and kv head) for a cache of s_max positions.
 int decode_attention_splits(int s_max);
-// out[b, h*dh:(h+1)*dh] = softmax(q k^T * scale + alibi) v over keys 0..pos[b] of the cache.
+// out[b, h*dh:(h+1)*dh] = softmax(q k^T * scale + alibi) v over keys 0..pos[b] of the cache (window >= 0: keys
+// max(0, pos[b] - window)..pos[b], the sliding window; -1 = off).
 // q: row b at q + b*ldq (head h at +h*dh); partial_o: fp32 [B, H, splits, dh]; partial_ml: fp32 [B, H, splits, 2].
 void decode_attention_launch(const void* q, long long ldq, const void* kc, const void* vc, const int* pos, void* out, long long ldo,
                              float* partial_o, float* partial_ml, int B, int H, int Hkv, int dh, int s_max, float scale,
-                             const float* alibi_slopes, cudaStream_t st);
+                             const float* alibi_slopes, cudaStream_t st, int window = -1);
 
 // For each row b of the fused qkv [B, (H + 2*Hkv)*dh]: rotate q and k (rotate-half tables cos / sin [>= s_max, dh/2], nullptr = no RoPE)
 // at position pos[b] (q in place), and write k, v into the cache at position pos[b] of slot slot[b] (slot == nullptr: slot b).
@@ -59,11 +60,12 @@ void decode_append_launch(void* qkv, long long ldqkv, const int* pos, void* kc, 
 // (slot, first_row, n_rows <= 64, first_pos): query rows first_row .. first_row + n_rows - 1 of qkv [n_q, (H + 2*Hkv)*dh] (q, after
 // RoPE) sit at positions first_pos + i of that slot, and row i attends to keys 0 .. first_pos + i of the slot:
 //   out[first_row + i, h*dh:(h+1)*dh] = softmax(q k^T * scale + alibi) v.
+// window >= 0 (sliding window) starts row i's keys at max(0, first_pos + i - window); -1 = off.
 // Rows outside every tile are not written. The keys of all tile rows must already be in the cache (decode_append first).
 // qkv and out rows must be 16-byte aligned (TMA); d_head 64 or 128.
 void cache_attention_launch(const void* qkv, long long ldq, long long n_q, const void* kc, const void* vc, const int* tiles, int n_tiles,
                             void* out, long long ldo, int B_max, int H, int Hkv, int dh, int s_max, float scale,
-                            const float* alibi_slopes, cudaStream_t st);
+                            const float* alibi_slopes, cudaStream_t st, int window = -1);
 
 // h[b,:] = wte[ids[b],:] + wpe[pos[b],:] (wpe may be nullptr)
 void embed_pos_launch(const int* ids, const int* pos, const void* wte, const void* wpe, void* out, int B, int d, int V, cudaStream_t st);

@@ -26,7 +26,6 @@ wgmma kernel over the slot's keys, causal at each row's own position) in place o
 """
 from __future__ import annotations
 
-import math
 from typing import Any
 
 import torch
@@ -50,7 +49,7 @@ class KVDecoder:
         self.max_batch, self.max_seq_len = int(max_batch), int(c.max_seq_len)
         self.use_graph = bool(use_graph)
         self.dev = engine.device
-        self.scale = 1.0 / math.sqrt(c.d_head)
+        self.scale, self.window = c.attn_scale, c.sliding_window_size
         self._cap = 0
         self._graphs: dict[int, torch.cuda.CUDAGraph] = {}
         self._b = 0
@@ -163,7 +162,8 @@ class KVDecoder:
             self._qkv_post(w, qkv, pre, tmp, m, r)
             if e.rope is not None:
                 ops.rope_(qkv.view(b, S, W), e.rope[0], e.rope[1], H, n_kv_heads=Hkv)
-            ops.attention_fwd(qkv.view(b, S, W), attn.view(b, S, d), lse, H, self.scale, True, e.alibi, n_kv_heads=Hkv)
+            ops.attention_fwd(qkv.view(b, S, W), attn.view(b, S, d), lse, H, self.scale, True, e.alibi, n_kv_heads=Hkv,
+                              window=self.window)
             _, k, v = e._sdpa_heads(qkv, b, S)  # noqa: SLF001
             self.cache[i, 0, :, :, :S].index_copy_(0, dst, k)   # the kv heads' k / v after clip, qk_ln and RoPE
             self.cache[i, 1, :, :, :S].index_copy_(0, dst, v)
@@ -212,9 +212,11 @@ class KVDecoder:
             self._qkv_post(w, qkv, x.get("qk_pre"), x.get("qk_tmp"), m, r)
             ops.decode_append(qkv, pos, kc, vc, e.rope, c.n_heads, slot, n_kv_heads=c.kv_n_heads)
             if tiles is None:
-                ops.decode_attention(qkv, kc, vc, pos, attn, c.n_heads, self.scale, e.alibi, n_kv_heads=c.kv_n_heads)
+                ops.decode_attention(qkv, kc, vc, pos, attn, c.n_heads, self.scale, e.alibi, n_kv_heads=c.kv_n_heads,
+                                     window=self.window)
             else:
-                ops.cache_attention(qkv, kc, vc, tiles, attn, c.n_heads, self.scale, e.alibi, n_kv_heads=c.kv_n_heads)
+                ops.cache_attention(qkv, kc, vc, tiles, attn, c.n_heads, self.scale, e.alibi, n_kv_heads=c.kv_n_heads,
+                                    window=self.window)
             self._linear(attn, w.wo, w.bo, hmid, residual=h)
             e._norm_fwd(hmid, w.g2, w.b2, ln, m, r)
             self._ffn(w, ln, u, z, h, hmid, x.get("ffn_d"), x.get("ffn_c"))

@@ -26,14 +26,14 @@ backend and the two are directly comparable in tests.
 """
 from __future__ import annotations
 
-import math
 from typing import Any
 
 import torch
 import torch.nn.functional as F
 
 from photon_b200 import ops
-from photon_b200.models.mpt import MPTConfig, MPTForCausalLM, check_sequence_id, ffn_desc, nondefault_ffn, shift_labels
+from photon_b200.models.mpt import (MPTConfig, MPTForCausalLM, check_sequence_id, ffn_desc, nondefault_ffn, shift_labels,
+                                    window_keep)
 from photon_b200.train.backend import apply_freeze
 from photon_b200.utils.flat import FlatLayout, FlatParams
 
@@ -476,11 +476,11 @@ class B200Engine:
 
     def _attention_fwd(self, lw: dict[str, Any], ws: dict[str, Any], b: int, S: int) -> None:
         c = self.cfg
-        scale = 1.0 / math.sqrt(c.d_head)
+        scale = c.attn_scale
         doc = ws["sequence_id"] is not None
         if self._kernel_attention(S):
             ops.attention_fwd(lw["qkv"].view(b, S, c.qkv_dim), lw["attn"].view(b, S, c.d_model), lw["lse"], c.n_heads, scale, True,
-                              self.alibi, ws["doc_start"] if doc else None, n_kv_heads=c.kv_n_heads)
+                              self.alibi, ws["doc_start"] if doc else None, n_kv_heads=c.kv_n_heads, window=c.sliding_window_size)
             return
         # library attention: kernels.attention=torch, an unsupported d_head, or a sequence length that is not a multiple
         # of the 128-row tiles (the shipped configs use 2048)
@@ -492,11 +492,14 @@ class B200Engine:
         return {"enable_gqa": True} if self.cfg.kv_n_heads != self.cfg.n_heads else {}
 
     def _sdpa_mask(self, S: int, dtype: torch.dtype, sequence_id: torch.Tensor | None = None) -> dict[str, Any]:
-        if self.alibi is None and sequence_id is None:
+        win = window_keep(S, self.cfg.sliding_window_size, self.device)
+        if self.alibi is None and sequence_id is None and win is None:
             return {"is_causal": True}
         keep = torch.ones(S, S, dtype=torch.bool, device=self.device).tril()
         if sequence_id is not None:   # the same equality mask as the torch module: [b, 1, S, S]
             keep = keep & (sequence_id[:, :, None] == sequence_id[:, None, :])[:, None]
+        if win is not None:
+            keep = keep & win
         if self.alibi is None:
             return {"attn_mask": keep}
         pos = torch.arange(S, device=self.device)
@@ -505,13 +508,13 @@ class B200Engine:
 
     def _attention_bwd(self, lw: dict[str, Any], ws: dict[str, Any], b: int, S: int) -> None:
         c = self.cfg
-        scale = 1.0 / math.sqrt(c.d_head)
+        scale = c.attn_scale
         doc = ws["sequence_id"] is not None
         if self._kernel_attention(S):
             ops.attention_bwd(lw["qkv"].view(b, S, c.qkv_dim), lw["attn"].view(b, S, c.d_model),
                               ws["dattn"].view(b, S, c.d_model), lw["lse"], ws["dqkv"].view(b, S, c.qkv_dim), ws["delta"],
                               c.n_heads, scale, True, self.alibi, ws["doc_start"] if doc else None, ws["doc_end"] if doc else None,
-                              n_kv_heads=c.kv_n_heads)
+                              n_kv_heads=c.kv_n_heads, window=c.sliding_window_size)
             if self.rope is not None:   # gradients w.r.t. the un-rotated q, k
                 ops.rope_(ws["dqkv"].view(b, S, c.qkv_dim), self.rope[0], self.rope[1], c.n_heads, inverse=True, n_kv_heads=c.kv_n_heads)
             return

@@ -14,6 +14,7 @@ Block: ``x = x + attn(norm_1(x)); x = x + ffn(norm_2(x))``; ``ffn = down(act(up(
 from __future__ import annotations
 
 import math
+import numbers
 from dataclasses import dataclass, field
 from typing import Any
 
@@ -48,6 +49,11 @@ class MPTConfig:
     # attn_config.attn_type grouped_query_attention / multiquery_attention: K / V have kv_n_heads heads (None: n_heads), query
     # head h attending with kv head h // (n_heads // kv_n_heads)
     kv_n_heads: int | None = None
+    # attn_config.sliding_window_size W: query i sees keys i - W .. i only (W + 1 keys, intersected with the document mask;
+    # positions stay absolute); -1 is off. Unrelated to the ICL evaluator's context truncation.
+    sliding_window_size: int = -1
+    # attn_config.softmax_scale: the factor on q·k in every attention path (None: 1 / sqrt(d_head))
+    softmax_scale: float | None = None
     # ffn_config (llm-foundry): ffn_type mptmlp (down(act(up(x)))) or mptglu (down(act(gate(x)) * up(x))); ffn_act_fn gelu
     # (exact) or silu; ffn_hidden_size overrides the width int(d_model * expansion_ratio)
     ffn_type: str = "mptmlp"
@@ -71,6 +77,20 @@ class MPTConfig:
         if norm not in NORM_TYPES:
             raise ValueError(f"unsupported model.norm_type {self.norm_type!r} (supported: {', '.join(NORM_TYPES)})")
         self.norm_type = NORM_TYPES[norm]
+        w = self.sliding_window_size
+        if isinstance(w, bool) or not isinstance(w, numbers.Integral) or w < -1:
+            raise ValueError(f"attn_config.sliding_window_size must be an integer >= 0, or -1 (off); got {w!r}")
+        self.sliding_window_size = int(w)
+        sc = self.softmax_scale
+        if sc is not None:
+            if isinstance(sc, bool) or not isinstance(sc, numbers.Real) or not math.isfinite(sc) or sc <= 0:
+                raise ValueError(f"attn_config.softmax_scale must be a positive number or None; got {sc!r}")
+            self.softmax_scale = float(sc)
+
+    @property
+    def attn_scale(self) -> float:
+        """The attention score scale: ``softmax_scale``, else ``1 / sqrt(d_head)``."""
+        return 1.0 / math.sqrt(self.d_head) if self.softmax_scale is None else self.softmax_scale
 
     @property
     def rmsnorm(self) -> bool:
@@ -135,6 +155,7 @@ class MPTConfig:
             rope=bool(attn.pop("rope", False)), rope_theta=float(attn.pop("rope_theta", 10000.0)),
             qk_ln=bool(attn.pop("qk_ln", False)), clip_qkv=attn.pop("clip_qkv", None),
             attn_uses_sequence_id=bool(attn.pop("attn_uses_sequence_id", False)), kv_n_heads=kv,
+            sliding_window_size=attn.pop("sliding_window_size", -1), softmax_scale=attn.pop("softmax_scale", None),
             no_bias=bool(m.pop("no_bias", False)), learned_pos_emb=bool(m.pop("learned_pos_emb", True)),
             norm_type=m.pop("norm_type", "low_precision_layernorm"), norm_eps=float(m.pop("norm_eps", 1e-5)),
         )
@@ -213,6 +234,14 @@ def alibi_slopes(n_heads: int, bias_max: int = 8) -> torch.Tensor:
     return slopes
 
 
+def window_keep(S: int, window: int, device: Any = None) -> torch.Tensor | None:
+    """The sliding window's part of the attention mask: bool [S, S], True where key ``j >= i - window`` (the causal part is
+    separate). None when the window is off or wide enough (``window >= S - 1``) to leave causal attention unchanged."""
+    if window < 0 or window >= S - 1:
+        return None
+    return torch.ones(S, S, dtype=torch.bool, device=device).triu(-window)
+
+
 def rope_tables(seq_len: int, d_head: int, theta: float, device: Any = None) -> tuple[torch.Tensor, torch.Tensor]:
     inv = 1.0 / (theta ** (torch.arange(0, d_head, 2, dtype=torch.float32, device=device) / d_head))
     ang = torch.outer(torch.arange(seq_len, dtype=torch.float32, device=device), inv)
@@ -272,7 +301,8 @@ class MPTAttention(nn.Module):
         k, v = (t.view(B, S, Hkv, dh).transpose(1, 2) for t in (k, v))
         if rope is not None:
             q, k = apply_rope(q, rope[0][:S], rope[1][:S]), apply_rope(k, rope[0][:S], rope[1][:S])
-        scale = 1.0 / math.sqrt(dh)
+        scale = cfg.attn_scale
+        win = window_keep(S, cfg.sliding_window_size, x.device)
         if cfg.attn_impl == "torch" or (alibi is not None and cfg.attn_impl != "flash"):
             if Hkv != H:   # query head h reads kv head h // (H // Hkv)
                 k, v = k.repeat_interleave(H // Hkv, dim=1), v.repeat_interleave(H // Hkv, dim=1)
@@ -282,14 +312,18 @@ class MPTAttention(nn.Module):
             mask = torch.ones(S, S, dtype=torch.bool, device=x.device).tril()
             if doc_keep is not None:
                 mask = mask & doc_keep
+            if win is not None:
+                mask = mask & win
             att = att.masked_fill(~mask, float("-inf"))
             o = torch.softmax(att.float(), dim=-1).to(v.dtype) @ v
         else:
             bias = None
-            if alibi is not None or doc_keep is not None:
+            if alibi is not None or doc_keep is not None or win is not None:
                 mask = torch.ones(S, S, dtype=torch.bool, device=x.device).tril()
                 if doc_keep is not None:
                     mask = mask & doc_keep
+                if win is not None:
+                    mask = mask & win
                 bias = mask if alibi is None else alibi[:, :, :S, :S].to(q.dtype).masked_fill(~mask, float("-inf"))
             gqa = {"enable_gqa": True} if Hkv != H else {}
             o = F.scaled_dot_product_attention(q, k, v, attn_mask=bias, is_causal=bias is None, scale=scale, **gqa)

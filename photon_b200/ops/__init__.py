@@ -320,23 +320,27 @@ def _kv(n_heads: int, n_kv_heads: int | None) -> int:
 
 def attention_fwd(qkv: torch.Tensor, out: torch.Tensor, lse: torch.Tensor, n_heads: int, scale: float, causal: bool = True,
                   alibi_slopes: torch.Tensor | None = None, doc_start: torch.Tensor | None = None,
-                  n_kv_heads: int | None = None) -> None:
+                  n_kv_heads: int | None = None, window: int = -1) -> None:
     """``qkv`` [B, S, (n_heads + 2 * n_kv_heads) * d_head]: the q heads, then the k heads, then the v heads; query head ``h``
     attends with kv head ``h // (n_heads // n_kv_heads)`` (grouped-query attention; None: ``n_heads``, multi-head).
     ``alibi_slopes``: optional fp32 [n_heads]; adds ``slope_h * (key - query)`` to the scores (MPT ``attn_config.alibi``).
     ``doc_start``: optional int32 [B*S] from :func:`doc_bounds` (causal only); query ``q`` then sees key ``k`` iff
-    ``doc_start[q] <= k <= q``, and key tiles before a query tile's first document are skipped."""
-    ext().attention_fwd(qkv, out, lse, int(n_heads), float(scale), bool(causal), alibi_slopes, doc_start, _kv(n_heads, n_kv_heads))
+    ``doc_start[q] <= k <= q``, and key tiles before a query tile's first document are skipped.
+    ``window``: sliding window (causal only; -1: off). Query ``q`` then sees keys ``q - window .. q`` only (intersected with
+    the document mask), and key tiles before a query tile's window are skipped."""
+    ext().attention_fwd(qkv, out, lse, int(n_heads), float(scale), bool(causal), alibi_slopes, doc_start, _kv(n_heads, n_kv_heads),
+                        int(window))
 
 
 def attention_bwd(qkv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor, dqkv: torch.Tensor,
                   delta: torch.Tensor, n_heads: int, scale: float, causal: bool = True,
                   alibi_slopes: torch.Tensor | None = None, doc_start: torch.Tensor | None = None,
-                  doc_end: torch.Tensor | None = None, n_kv_heads: int | None = None) -> None:
-    """``doc_start`` / ``doc_end`` (both or neither): the document mask of :func:`attention_fwd`. ``dqkv`` is shaped like
-    ``qkv``; with grouped-query attention the dK / dV of a kv head are summed over its query heads."""
+                  doc_end: torch.Tensor | None = None, n_kv_heads: int | None = None, window: int = -1) -> None:
+    """``doc_start`` / ``doc_end`` (both or neither) and ``window``: the document mask and sliding window of
+    :func:`attention_fwd`. ``dqkv`` is shaped like ``qkv``; with grouped-query attention the dK / dV of a kv head are summed
+    over its query heads."""
     ext().attention_bwd(qkv, out, dout, lse, dqkv, delta, int(n_heads), float(scale), bool(causal), alibi_slopes, doc_start, doc_end,
-                        _kv(n_heads, n_kv_heads))
+                        _kv(n_heads, n_kv_heads), int(window))
 
 
 def doc_bounds(sequence_id: torch.Tensor, doc_start: torch.Tensor, doc_end: torch.Tensor) -> None:
@@ -372,11 +376,14 @@ def skinny_gemm(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor, bias: torch
 
 
 def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, pos: torch.Tensor, out: torch.Tensor, n_heads: int,
-                     scale: float, alibi_slopes: torch.Tensor | None = None, n_kv_heads: int | None = None) -> torch.Tensor:
+                     scale: float, alibi_slopes: torch.Tensor | None = None, n_kv_heads: int | None = None,
+                     window: int = -1) -> torch.Tensor:
     """One query row per sequence (``q`` [B, >= H*dh]) against one layer of the cache (``k_cache`` / ``v_cache``
-    [B_max, n_kv_heads, S_max, dh]) over keys ``0..pos[b]`` (int32 on the device); ``out`` [B, H*dh]. One CTA serves all query
-    heads of a kv head, so each cached row is read once per group."""
-    ext().decode_attention(q, k_cache, v_cache, pos, out, int(n_heads), float(scale), alibi_slopes, _kv(n_heads, n_kv_heads))
+    [B_max, n_kv_heads, S_max, dh]) over keys ``0..pos[b]`` (int32 on the device; ``window`` >= 0: keys
+    ``max(0, pos[b] - window)..pos[b]``); ``out`` [B, H*dh]. One CTA serves all query heads of a kv head, so each cached row is
+    read once per group."""
+    ext().decode_attention(q, k_cache, v_cache, pos, out, int(n_heads), float(scale), alibi_slopes, _kv(n_heads, n_kv_heads),
+                           int(window))
     return out
 
 
@@ -391,12 +398,15 @@ def decode_append(qkv: torch.Tensor, pos: torch.Tensor, k_cache: torch.Tensor, v
 
 
 def cache_attention(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, tiles: torch.Tensor, out: torch.Tensor,
-                    n_heads: int, scale: float, alibi_slopes: torch.Tensor | None = None, n_kv_heads: int | None = None) -> torch.Tensor:
+                    n_heads: int, scale: float, alibi_slopes: torch.Tensor | None = None, n_kv_heads: int | None = None,
+                    window: int = -1) -> torch.Tensor:
     """Several query rows per cache slot on the tensor cores. ``tiles`` int32 [T, 4] on the device, one row per tile
     ``(slot, first_row, n_rows <= 64, first_pos)``: rows ``first_row + i`` of ``qkv`` [N, (n_heads + 2 * n_kv_heads) * d_head]
     (q after RoPE) sit at positions ``first_pos + i`` of that slot and attend to its keys ``0 .. first_pos + i`` (query head
-    ``h`` to kv head ``h // (n_heads // n_kv_heads)``). Writes those rows of ``out`` [N, d] only."""
-    ext().cache_attention(qkv, k_cache, v_cache, tiles, out, int(n_heads), float(scale), alibi_slopes, _kv(n_heads, n_kv_heads))
+    ``h`` to kv head ``h // (n_heads // n_kv_heads)``; ``window`` >= 0: keys from ``first_pos + i - window`` on). Writes
+    those rows of ``out`` [N, d] only."""
+    ext().cache_attention(qkv, k_cache, v_cache, tiles, out, int(n_heads), float(scale), alibi_slopes, _kv(n_heads, n_kv_heads),
+                          int(window))
     return out
 
 
