@@ -708,7 +708,7 @@ void col_sum(const Tensor& dy, Tensor& out) {
                  stream_of(dy));
 }
 void cross_entropy(Tensor& logits, const Tensor& targets, double grad_scale, bool write_grad, Tensor& stats,
-                   c10::optional<Tensor> row_lse, const c10::optional<Tensor>& unigram_logp) {
+                   c10::optional<Tensor> row_lse, const c10::optional<Tensor>& unigram_logp, double head_scale, double head_cap) {
   check_bf16(logits, "logits");
   TORCH_CHECK(logits.dim() == 2 && logits.stride(1) == 1, "logits must be [rows,V]");
   TORCH_CHECK(targets.scalar_type() == at::kLong && targets.is_contiguous(), "targets must be contiguous int64");
@@ -725,9 +725,12 @@ void cross_entropy(Tensor& logits, const Tensor& targets, double grad_scale, boo
     check_f32(*unigram_logp, "unigram_logp");
     TORCH_CHECK(unigram_logp->is_contiguous() && unigram_logp->numel() >= logits.size(1), "cross_entropy: unigram_logp must be contiguous [>=V]");
   }
+  TORCH_CHECK(head_scale > 0 && std::isfinite(head_scale), "cross_entropy: the logit scale must be positive and finite");
+  TORCH_CHECK(head_cap >= 0 && std::isfinite(head_cap), "cross_entropy: the logit cap must be 0 (none) or positive and finite");
   c10::cuda::CUDAGuard guard(logits.device());
   pb::cross_entropy(logits.data_ptr(), logits.stride(0), targets.data_ptr<int64_t>(), logits.size(0), int(logits.size(1)), float(grad_scale),
-                    write_grad, stats.data_ptr<double>(), opt_ptr<float>(row_lse), opt_ptr<float>(unigram_logp), stream_of(logits));
+                    write_grad, stats.data_ptr<double>(), opt_ptr<float>(row_lse), opt_ptr<float>(unigram_logp), float(head_scale),
+                    float(head_cap), stream_of(logits));
 }
 // any length: the kernel reads float4s and then the last numel % 4 elements
 void flat_l2_norm(const Tensor& x, Tensor& scratch_f64, Tensor& out_f32) {

@@ -9,9 +9,11 @@
 #include <stdint.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 
 #include "fused_ops.h"
 #include "launch.h"
@@ -422,9 +424,39 @@ __global__ void __launch_bounds__(256) col_reduce_kernel(const __nv_bfloat16* __
 // One block per row of logits[Tc, V] (bf16). Pass 1: online max / sum-exp (+argmax). Pass 2 (training):
 // overwrite the row with dlogits = (softmax - onehot) * grad_scale (zero for ignored rows).
 // stats[0] += sum loss, stats[1] += #valid, stats[2] += #correct, stats[3] += sum unigram loss  (fp64)
+//
+// HT, the LM head's logit transform (llm-foundry logit_scale / final_logit_softcapping): the softmax is taken over y = T(x)
+// instead of the stored logits x, with T(x) = s·x (HT 1) or c·tanh(s·x / c) (HT 2), applied to each logit as it is read. Max,
+// sum-exp, the target logit and row_lse are those of y; pass 2 writes dL/dx = (softmax(y) - onehot) · T'(x) · grad_scale. The
+// argmax stays on x: T is strictly increasing (s, c > 0) and rounding could tie saturated values of y that x tells apart, so the
+// running max of x (m) is kept next to that of y (my). HT 0 is the identity: my is m, and the instance computes what the kernel
+// without the transform did (ce_smem_kernel<0> compiles to its SASS; ce_kernel<0> to the same operations with other registers).
+struct HeadTf {
+  float s;   // scale s
+  float a;   // 2 s / c: with e = exp(-a·|x|), |tanh(s·x / c)| = (1 - e) / (1 + e)
+  float c;   // cap c
+};
+// y = T(x) and, for D, dy/dx. The tanh comes from e = exp(-2|u|) and one rcp: t = (1 - e) / (1 + e) and
+// 1 - t² = 4e / (1 + e)², so the gradient factor keeps its relative accuracy where the cap saturates (e -> 0 gives exactly t = 1,
+// 1 - t² = 0). The MUFU tanh.approx would save the rcp, at a 2^-11 relative error (about 0.015 at a cap of 30).
+template <int HT, bool D = false>
+__device__ __forceinline__ float head_y(float x, const HeadTf& h, float* dydx = nullptr) {
+  if constexpr (HT == 0) {
+    return x;
+  } else if constexpr (HT == 1) {
+    if constexpr (D) *dydx = h.s;
+    return h.s * x;
+  } else {
+    const float e = __expf(-h.a * fabsf(x)), q = __fdividef(1.f, 1.f + e);
+    if constexpr (D) *dydx = h.s * 4.f * e * q * q;
+    return copysignf(h.c * (1.f - e) * q, x);
+  }
+}
+
+template <int HT>
 __global__ void __launch_bounds__(256) ce_kernel(__nv_bfloat16* __restrict__ logits, long long ld, const int64_t* __restrict__ targets,
                                                   int V, float grad_scale, int write_grad, double* __restrict__ stats,
-                                                  float* __restrict__ row_lse, const float* __restrict__ unigram_logp) {
+                                                  float* __restrict__ row_lse, const float* __restrict__ unigram_logp, const HeadTf ht) {
   __shared__ float sm[8], ss[8];
   __shared__ int si[8];
   __shared__ float bm, bs;
@@ -434,8 +466,10 @@ __global__ void __launch_bounds__(256) ce_kernel(__nv_bfloat16* __restrict__ log
   const long long tgt = targets[row];
   const bool valid = tgt >= 0 && tgt < V;
   const int vec = V / 8;
+  float my_ = -INFINITY;
   float m = -INFINITY, s = 0.f;
   int am = 0;
+  float& my = HT ? my_ : m;
   for (int i = threadIdx.x; i < vec; i += blockDim.x) {
     float f[8];
     unpack8(reinterpret_cast<const uint4*>(lr)[i], f);
@@ -445,12 +479,18 @@ __global__ void __launch_bounds__(256) ce_kernel(__nv_bfloat16* __restrict__ log
     for (int k = 1; k < 8; ++k)
       if (f[k] > cm) cm = f[k], ci = k;
     if (cm > m) {
-      s *= __expf(m - cm);
+      if constexpr (HT == 0) {
+        s *= __expf(m - cm);
+      } else {
+        const float cy = head_y<HT>(cm, ht);
+        s *= __expf(my - cy);
+        my = cy;
+      }
       m = cm;
       am = i * 8 + ci;
     }
 #pragma unroll
-    for (int k = 0; k < 8; ++k) s += __expf(f[k] - m);
+    for (int k = 0; k < 8; ++k) s += __expf(head_y<HT>(f[k], ht) - my);
   }
   // warp + block combine of (m, s, argmax)
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -458,27 +498,36 @@ __global__ void __launch_bounds__(256) ce_kernel(__nv_bfloat16* __restrict__ log
   for (int o = 16; o > 0; o >>= 1) {
     const float om = __shfl_xor_sync(0xffffffff, m, o), os = __shfl_xor_sync(0xffffffff, s, o);
     const int oi = __shfl_xor_sync(0xffffffff, am, o);
-    const float nm = fmaxf(m, om);
-    s = (m == -INFINITY ? 0.f : s * __expf(m - nm)) + (om == -INFINITY ? 0.f : os * __expf(om - nm));
+    const float omy = HT ? __shfl_xor_sync(0xffffffff, my, o) : om;
+    const float nmy = fmaxf(my, omy);
+    s = (my == -INFINITY ? 0.f : s * __expf(my - nmy)) + (omy == -INFINITY ? 0.f : os * __expf(omy - nmy));
     if (om > m || (om == m && oi < am)) am = oi;
-    m = nm;
+    if constexpr (HT != 0) m = fmaxf(m, om);
+    my = nmy;
   }
-  if (lane == 0) sm[w] = m, ss[w] = s, si[w] = am;
+  __shared__ float smy_[HT ? 16 : 1];
+  float* const smy = HT ? smy_ : sm;
+  if (lane == 0) {
+    sm[w] = m, ss[w] = s, si[w] = am;
+    if constexpr (HT != 0) smy[w] = my;
+  }
   __syncthreads();
   if (threadIdx.x == 0) {
-    float M = sm[0], S = ss[0];
+    float M = sm[0], MY_ = smy[0], S = ss[0];
+    float& MY = HT ? MY_ : M;
     int I = si[0];
     for (int i = 1; i < 8; ++i) {
-      const float nm = fmaxf(M, sm[i]);
-      S = (M == -INFINITY ? 0.f : S * __expf(M - nm)) + (sm[i] == -INFINITY ? 0.f : ss[i] * __expf(sm[i] - nm));
+      const float nmy = fmaxf(MY, smy[i]);
+      S = (MY == -INFINITY ? 0.f : S * __expf(MY - nmy)) + (smy[i] == -INFINITY ? 0.f : ss[i] * __expf(smy[i] - nmy));
       if (sm[i] > M || (sm[i] == M && si[i] < I)) I = si[i];
-      M = nm;
+      if constexpr (HT != 0) M = fmaxf(M, sm[i]);
+      MY = nmy;
     }
-    bm = M, bs = S, bi = I;
-    const float lse = M + __logf(S);
+    bm = MY, bs = S, bi = I;
+    const float lse = MY + __logf(S);
     if (row_lse) row_lse[row] = lse;
     if (valid) {
-      const float lt = __bfloat162float(lr[tgt]);
+      const float lt = head_y<HT>(__bfloat162float(lr[tgt]), ht);
       atomicAdd(stats + 0, double(lse - lt));
       atomicAdd(stats + 1, 1.0);
       if (I == tgt) atomicAdd(stats + 2, 1.0);
@@ -494,9 +543,10 @@ __global__ void __launch_bounds__(256) ce_kernel(__nv_bfloat16* __restrict__ log
     unpack8(*p, f);
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-      float g = valid ? __expf(f[k] - M) * inv : 0.f;
+      float dy = 0.f;   // set by head_y on valid rows only; an ignored row's gradient is 0 · 0
+      float g = valid ? __expf(head_y<HT, true>(f[k], ht, &dy) - M) * inv : 0.f;
       if (valid && i * 8 + k == tgt) g -= grad_scale;
-      f[k] = g;
+      f[k] = HT ? g * dy : g;
     }
     *p = pack8(f);
   }
@@ -505,9 +555,11 @@ __global__ void __launch_bounds__(256) ce_kernel(__nv_bfloat16* __restrict__ log
 // Same contract, ONE read of the logits: the whole row (V bf16 = 100 KB for the GPT-NeoX vocabulary) is pulled into shared
 // memory by bulk async copies (cp.async.bulk on an mbarrier), both passes run out of shared memory and only the gradient goes back
 // to HBM — 2 instead of 3 row transfers per row. Two CTAs fit on an SM, so one row's copy overlaps the other's arithmetic.
+template <int HT>
 __global__ void __launch_bounds__(512) ce_smem_kernel(__nv_bfloat16* __restrict__ logits, long long ld, const int64_t* __restrict__ targets,
                                                        int V, float grad_scale, int write_grad, double* __restrict__ stats,
-                                                       float* __restrict__ row_lse, const float* __restrict__ unigram_logp) {
+                                                       float* __restrict__ row_lse, const float* __restrict__ unigram_logp,
+                                                       const HeadTf ht) {
   extern __shared__ __align__(128) uint8_t ce_smem[];
   uint4* srow = reinterpret_cast<uint4*>(ce_smem);
   __shared__ uint64_t bar;
@@ -533,8 +585,10 @@ __global__ void __launch_bounds__(512) ce_smem_kernel(__nv_bfloat16* __restrict_
   }
   __syncthreads();
   mbar_wait(&bar, 0);
+  float my_ = -INFINITY;
   float m = -INFINITY, s = 0.f;
   int am = 0;
+  float& my = HT ? my_ : m;
   for (int i = threadIdx.x; i < vec; i += blockDim.x) {
     float f[8];
     unpack8(srow[i], f);
@@ -544,39 +598,54 @@ __global__ void __launch_bounds__(512) ce_smem_kernel(__nv_bfloat16* __restrict_
     for (int k = 1; k < 8; ++k)
       if (f[k] > cm) cm = f[k], ci = k;
     if (cm > m) {
-      s *= __expf(m - cm);
+      if constexpr (HT == 0) {
+        s *= __expf(m - cm);
+      } else {
+        const float cy = head_y<HT>(cm, ht);
+        s *= __expf(my - cy);
+        my = cy;
+      }
       m = cm;
       am = i * 8 + ci;
     }
 #pragma unroll
-    for (int k = 0; k < 8; ++k) s += __expf(f[k] - m);
+    for (int k = 0; k < 8; ++k) s += __expf(head_y<HT>(f[k], ht) - my);
   }
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     const float om = __shfl_xor_sync(0xffffffff, m, o), os = __shfl_xor_sync(0xffffffff, s, o);
     const int oi = __shfl_xor_sync(0xffffffff, am, o);
-    const float nm = fmaxf(m, om);
-    s = (m == -INFINITY ? 0.f : s * __expf(m - nm)) + (om == -INFINITY ? 0.f : os * __expf(om - nm));
+    const float omy = HT ? __shfl_xor_sync(0xffffffff, my, o) : om;
+    const float nmy = fmaxf(my, omy);
+    s = (my == -INFINITY ? 0.f : s * __expf(my - nmy)) + (omy == -INFINITY ? 0.f : os * __expf(omy - nmy));
     if (om > m || (om == m && oi < am)) am = oi;
-    m = nm;
+    if constexpr (HT != 0) m = fmaxf(m, om);
+    my = nmy;
   }
-  if (lane == 0) sm[w] = m, ss[w] = s, si[w] = am;
+  __shared__ float smy_[HT ? 16 : 1];
+  float* const smy = HT ? smy_ : sm;
+  if (lane == 0) {
+    sm[w] = m, ss[w] = s, si[w] = am;
+    if constexpr (HT != 0) smy[w] = my;
+  }
   __syncthreads();
   if (threadIdx.x == 0) {
-    float M = sm[0], S = ss[0];
+    float M = sm[0], MY_ = smy[0], S = ss[0];
+    float& MY = HT ? MY_ : M;
     int I = si[0];
     for (int i = 1; i < nw; ++i) {
-      const float nm = fmaxf(M, sm[i]);
-      S = (M == -INFINITY ? 0.f : S * __expf(M - nm)) + (sm[i] == -INFINITY ? 0.f : ss[i] * __expf(sm[i] - nm));
+      const float nmy = fmaxf(MY, smy[i]);
+      S = (MY == -INFINITY ? 0.f : S * __expf(MY - nmy)) + (smy[i] == -INFINITY ? 0.f : ss[i] * __expf(smy[i] - nmy));
       if (sm[i] > M || (sm[i] == M && si[i] < I)) I = si[i];
-      M = nm;
+      if constexpr (HT != 0) M = fmaxf(M, sm[i]);
+      MY = nmy;
     }
-    bm = M, bs = S;
-    const float lse = M + __logf(S);
+    bm = MY, bs = S;
+    const float lse = MY + __logf(S);
     if (row_lse) row_lse[row] = lse;
     if (valid) {
-      const float lt = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(ce_smem)[tgt]);
+      const float lt = head_y<HT>(__bfloat162float(reinterpret_cast<const __nv_bfloat16*>(ce_smem)[tgt]), ht);
       atomicAdd(stats + 0, double(lse - lt));
       atomicAdd(stats + 1, 1.0);
       if (I == tgt) atomicAdd(stats + 2, 1.0);
@@ -591,9 +660,10 @@ __global__ void __launch_bounds__(512) ce_smem_kernel(__nv_bfloat16* __restrict_
     unpack8(srow[i], f);
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-      float g = valid ? __expf(f[k] - M) * inv : 0.f;
+      float dy = 0.f;   // set by head_y on valid rows only; an ignored row's gradient is 0 · 0
+      float g = valid ? __expf(head_y<HT, true>(f[k], ht, &dy) - M) * inv : 0.f;
       if (valid && i * 8 + k == tgt) g -= grad_scale;
-      f[k] = g;
+      f[k] = HT ? g * dy : g;
     }
     reinterpret_cast<uint4*>(lr)[i] = pack8(f);
   }
@@ -764,22 +834,32 @@ void rmsnorm_bwd(const void* dy, const void* x, const float* gamma, const float*
   norm_bwd<true>(dy, x, gamma, nullptr, rstd, dres, dx, dgamma, nullptr, T, d, st);
 }
 void cross_entropy(void* logits, long long ld, const int64_t* targets, long long rows, int V, float grad_scale, bool write_grad,
-                   double* stats, float* row_lse, const float* unigram_logp, cudaStream_t st) {
+                   double* stats, float* row_lse, const float* unigram_logp, float head_scale, float head_cap, cudaStream_t st) {
   if (V % 8) throw std::runtime_error("cross_entropy: V must be a multiple of 8");
+  if (!(head_scale > 0.f) || !std::isfinite(head_scale) || !(head_cap >= 0.f) || !std::isfinite(head_cap))
+    throw std::runtime_error("cross_entropy: the logit scale must be positive and finite, the cap zero (none) or positive and finite");
+  // the transform instance: none (scale 1, no cap), scale only, or scale and cap
+  const int ht = head_cap > 0.f ? 2 : head_scale != 1.f ? 1 : 0;
+  const HeadTf tf{head_scale, head_cap > 0.f ? 2.f * head_scale / head_cap : 0.f, head_cap};
   const size_t row_bytes = size_t(V) * 2;
   static const bool smem_path = [] { const char* e = std::getenv("PB_CE_SMEM"); return !(e && e[0] == '0'); }();
   // Both kernels move the row in 16-byte pieces, so the binding has already required a 16-byte aligned base and a row stride
   // that is a multiple of 8. ce_kernel (two reads of the row from HBM) therefore runs only for rows over 200 KiB (V > 102400)
   // or under PB_CE_SMEM=0.
-  if (smem_path && row_bytes <= 200 * 1024) {
-    // the row lives in shared memory between the two passes: one HBM read of the logits instead of two
-    opt_in_smem(ce_smem_kernel, 200 * 1024);
-    ce_smem_kernel<<<int(rows), 512, row_bytes, st>>>((__nv_bfloat16*)logits, ld, targets, V, grad_scale, write_grad ? 1 : 0, stats, row_lse,
-                                                      unigram_logp);
-  } else {
-    ce_kernel<<<int(rows), 256, 0, st>>>((__nv_bfloat16*)logits, ld, targets, V, grad_scale, write_grad ? 1 : 0, stats, row_lse,
-                                         unigram_logp);
-  }
+  auto run = [&](auto HT) {
+    if (smem_path && row_bytes <= 200 * 1024) {
+      // the row lives in shared memory between the two passes: one HBM read of the logits instead of two
+      opt_in_smem(ce_smem_kernel<HT>, 200 * 1024);
+      ce_smem_kernel<HT><<<int(rows), 512, row_bytes, st>>>((__nv_bfloat16*)logits, ld, targets, V, grad_scale, write_grad ? 1 : 0, stats,
+                                                            row_lse, unigram_logp, tf);
+    } else {
+      ce_kernel<HT><<<int(rows), 256, 0, st>>>((__nv_bfloat16*)logits, ld, targets, V, grad_scale, write_grad ? 1 : 0, stats, row_lse,
+                                               unigram_logp, tf);
+    }
+  };
+  if (ht == 2) run(std::integral_constant<int, 2>{});
+  else if (ht == 1) run(std::integral_constant<int, 1>{});
+  else run(std::integral_constant<int, 0>{});
   launched("cross_entropy");
 }
 void flat_sqnorm(const float* x, long long n, double* out_accum, cudaStream_t st) {

@@ -27,8 +27,10 @@ void rmsnorm_bwd(const void* dy, const void* x, const float* gamma, const float*
                  long long T, int d, cudaStream_t st);
 void col_reduce(const void* dy, long long ld, const void* x, const float* mean, const float* rstd, float* out_sum, float* out_dot,
                 long long T, int d, cudaStream_t st);
+// head_scale / head_cap: the LM head's logit transform y = cap·tanh(head_scale·x / cap) (head_cap 0: y = head_scale·x), taken
+// before the softmax; 1 / 0 is none
 void cross_entropy(void* logits, long long ld, const int64_t* targets, long long rows, int V, float grad_scale, bool write_grad,
-                   double* stats, float* row_lse, const float* unigram_logp, cudaStream_t st);
+                   double* stats, float* row_lse, const float* unigram_logp, float head_scale, float head_cap, cudaStream_t st);
 void flat_sqnorm(const float* x, long long n, double* out_accum, cudaStream_t st);
 void sqrt_finalize(const double* in, float* out, cudaStream_t st);
 void axpby(float* acc, const float* x, float a, float b, long long n, cudaStream_t st);

@@ -8,6 +8,9 @@ processes one new token per sequence:
     embed (per-row position) -> per block: LN -> QKV -> (clip / qk_ln) -> append (RoPE + cache write) -> decode attention
     -> out-proj + residual -> LN -> FFN -> down + residual -> final LN -> LM head -> argmax (on the device)
 
+The LM head is ``wte`` or, untied, ``lm_head``. Greedy decoding takes the argmax of its raw logits: the head's transform
+(``logit_scale``, ``final_logit_softcapping``) is strictly increasing, so it cannot change the argmax.
+
 where the FFN is up + activation (GELU or SiLU) or, gated (``mptglu``), gate + activation -> up times that.
 
 The step is captured as one CUDA graph per batch size and replayed; token ids, positions and the cache are static device
@@ -31,6 +34,7 @@ from typing import Any
 import torch
 
 from photon_b200 import ops
+from photon_b200.models.mpt import head_transform
 
 # Up to this many rows a step's GEMMs run on the skinny (weight-streaming) GEMM, above it on the training GEMM; the
 # skinny kernel covers M <= 64. Measured crossover: docs/KERNELS.md ("Decoding").
@@ -190,7 +194,7 @@ class KVDecoder:
         # only the last prompt row of every sequence goes through the final LN and the LM head
         B["h"][:b].copy_(self._prefill(prompts, list(range(b))))
         e._norm_fwd(B["h"][:b], e.gf, e.bf, B["ln"][:b], B["m"][:b], B["r"][:b])
-        self._linear(B["ln"][:b], e.wte16, None, B["logits"][:b])
+        self._linear(B["ln"][:b], e.head16, None, B["logits"][:b])
         self.pos[:b].copy_(torch.tensor(lens, dtype=torch.int32), non_blocking=True)
         ops.argmax_advance(B["logits"][:b], self.tok[:b])
         self._pos_host = list(lens)
@@ -228,7 +232,7 @@ class KVDecoder:
         ops.embed_pos(self.tok, self.pos, e.wte16, e.wpe16, x["h"])
         self._blocks(x, self.pos)
         e._norm_fwd(x["h"], e.gf, e.bf, x["ln"], x["m"], x["r"])
-        self._linear(x["ln"], e.wte16, None, B["logits"][:b])
+        self._linear(x["ln"], e.head16, None, B["logits"][:b])
         ops.argmax_advance(B["logits"][:b], self.tok, self.pos)
 
     @torch.no_grad()
@@ -308,19 +312,22 @@ class KVDecoder:
         m, r = (torch.empty(R, dtype=torch.float32, device=self.dev) for _ in range(2))
         e._norm_fwd(hid, e.gf, e.bf, ln, m, r)
         logits = torch.empty(R, c.vocab_size, dtype=torch.bfloat16, device=self.dev)
-        self._linear(ln, e.wte16, None, logits)
+        self._linear(ln, e.head16, None, logits)
         # scored token k of pair i is predicted by its group's last context row (k = 0) or by extend row first[i] + k - 1
         group = {i: gi for gi, g in enumerate(members) for i in g}
         rows = [group[i] if k == 0 else first[i] + k - 1 for i, (_, sc) in enumerate(pairs) for k in range(len(sc))]
         tgts = [t for _, sc in pairs for t in sc]
         lse = torch.empty(R, dtype=torch.float32, device=self.dev)
         stats = torch.zeros(4, dtype=torch.float64, device=self.dev)
-        ops.cross_entropy(logits, torch.full((R,), -1, dtype=torch.long, device=self.dev), 0.0, False, stats, row_lse=lse)
+        # log p = T(logit) - lse(T(logits)) with the head's transform T (logit_scale / final_logit_softcapping); the argmax of
+        # the raw logits is that of T(logits): T is strictly increasing
+        ops.cross_entropy(logits, torch.full((R,), -1, dtype=torch.long, device=self.dev), 0.0, False, stats, row_lse=lse,
+                          logit_scale=e.head_scale, softcap=e.head_cap)
         top = torch.empty(R, dtype=torch.int32, device=self.dev)
         ops.argmax_advance(logits, top)
         row_t = torch.tensor(rows, dtype=torch.long).to(self.dev, non_blocking=True)
         tgt_t = torch.tensor(tgts, dtype=torch.long).to(self.dev, non_blocking=True)
-        logp = logits[row_t, tgt_t].float() - lse[row_t]
+        logp = head_transform(logits[row_t, tgt_t].float(), e.head_scale, e.head_cap) - lse[row_t]
         host = torch.stack([logp, (top[row_t].long() == tgt_t).float()]).cpu().tolist()
         out, k = [], 0
         for _, sc in pairs:

@@ -54,16 +54,18 @@ class BackwardPlan:
     """Which parts of the backward run, given the trainable parameter names (a pure function of the config and that set).
 
     The backward is one chain of stages: LM head, final LayerNorm, the blocks from the last down to the first
-    (:data:`BLOCK_STAGES` each), embeddings. A stage runs when it, or any stage after it, has a trainable parameter; its input
+    (:data:`BLOCK_STAGES` each), embeddings. The head stage owns ``transformer.wte.weight`` when the head is tied (``tied``) and
+    ``lm_head.weight`` otherwise; ``wte`` then belongs to the embedding stage only. A stage runs when it, or any stage after it, has a trainable parameter; its input
     gradient (the dgrad GEMM, the LayerNorm dx) is computed only when a later stage has one. So the backward stops right after the
     last stage that produces a trainable gradient, and weight / bias / LayerNorm-parameter gradients run for trainable names
     only. With every parameter trainable this is the full schedule."""
 
-    def __init__(self, n_layers: int, trainable: Any) -> None:
+    def __init__(self, n_layers: int, trainable: Any, tied: bool = True) -> None:
         self.n_layers = int(n_layers)
         self.trainable = frozenset(trainable)
+        self.head_weight = "transformer.wte.weight" if tied else "lm_head.weight"
         t = lambda names, pre="transformer.": any(pre + n in self.trainable for n in names)  # noqa: E731
-        chain = [("head", t(("wte.weight",))), ("norm_f", t(("norm_f.weight", "norm_f.bias")))]
+        chain = [("head", t((self.head_weight,), "")), ("norm_f", t(("norm_f.weight", "norm_f.bias")))]
         for i in range(self.n_layers - 1, -1, -1):
             chain += [((i, s), t(names, f"transformer.blocks.{i}.")) for s, names in BLOCK_STAGES]
         chain.append(("embed", t(("wte.weight", "wpe.weight"))))
@@ -83,7 +85,7 @@ class BackwardPlan:
 
     @property
     def head_wgrad(self) -> bool:
-        return self.grad("transformer.wte.weight")
+        return self.grad(self.head_weight)
 
     @property
     def lowest_block(self) -> int:
@@ -174,7 +176,9 @@ class B200Engine:
             if self.bf16_params.numel() != self.flat.layout.total or self.bf16_params.dtype != torch.bfloat16:
                 raise ValueError("shadow_storage must be a bf16 tensor with layout.total elements")
         self._init_frozen_planes()
-        self.plan = BackwardPlan(cfg.n_layers, self.flat.layout.names)
+        self.plan = BackwardPlan(cfg.n_layers, self.flat.layout.names, tied=cfg.tie_word_embeddings)
+        # the LM head's logit transform (logit_scale, final_logit_softcapping), applied by the fused cross-entropy kernel
+        self.head_scale, self.head_cap = cfg.head_scale, cfg.final_logit_softcapping
         self.unigram_log_probs = unigram_log_probs.to(self.device) if unigram_log_probs is not None else None
         self.lm_head_chunk = int(lm_head_chunk)
         # positional variants of the MPT attention block (ref: SURVEY §5.7): ALiBi slopes enter the attention kernels,
@@ -229,21 +233,27 @@ class B200Engine:
             n = "transformer." + n
             return lay.view(P, n) if n in have else flay.view(FP, n) if n in frozen else None
 
-        def v16(n: str) -> torch.Tensor:
-            n = "transformer." + n
+        def v16(n: str, pre: str = "transformer.") -> torch.Tensor:
+            n = pre + n
             return flay.view(F16, n) if n in frozen else lay.view(Sd, n)
 
-        vg = lambda n: lay.view(G, "transformer." + n) if "transformer." + n in have else None  # noqa: E731
+        vg = lambda n, pre="transformer.": lay.view(G, pre + n) if pre + n in have else None  # noqa: E731
         if self.zero3 is not None:
-            # weights: views into the two rotating block buffers (block i -> buffer i % 2) / the resident embedding buffer;
-            # 1-D fp32 parameters: the packed resident buffer; gradients: the block's staging plane (reduced after its backward)
+            # weights: views into the two rotating block buffers (block i -> buffer i % 2) / the resident embedding (and untied
+            # head) buffers; 1-D fp32 parameters: the packed resident buffer; gradients: the unit's staging plane (reduced after
+            # its backward)
             z = self.zero3
             v32 = lambda n: z.small("transformer." + n) if "transformer." + n in have else None  # noqa: E731
-            vg = lambda n: z.grad("transformer." + n) if "transformer." + n in have else None  # noqa: E731
-            v16 = lambda n: z.weight("transformer." + n)  # noqa: E731
+            vg = lambda n, pre="transformer.": z.grad(pre + n) if pre + n in have else None  # noqa: E731
+            v16 = lambda n, pre="transformer.": z.weight(pre + n)  # noqa: E731
         has_wpe = self.cfg.learned_pos_emb
         self.wte16, self.wpe16 = v16("wte.weight"), (v16("wpe.weight") if has_wpe else None)
         self.d_wte, self.d_wpe = vg("wte.weight"), (vg("wpe.weight") if has_wpe else None)
+        # the LM head's weight: wte when tied, else lm_head (bf16 also under amp_fp8; a frozen one reads the frozen planes)
+        if self.cfg.tie_word_embeddings:
+            self.head16, self.d_head16 = self.wte16, self.d_wte
+        else:
+            self.head16, self.d_head16 = v16("lm_head.weight", ""), vg("lm_head.weight", "")
         self.gf, self.bf, self.d_gf, self.d_bf = v32("norm_f.weight"), v32("norm_f.bias"), vg("norm_f.weight"), vg("norm_f.bias")
         self.layers: list[_LayerW] = []
         for i in range(self.cfg.n_layers):
@@ -600,13 +610,14 @@ class B200Engine:
         for lo in range(0, T, step):
             hi = min(T, lo + step)
             logits = ws["logits"][: hi - lo]
-            ops.gemm(ws["lnf"][lo:hi], self.wte16, logits)
-            ops.cross_entropy(logits, targets[lo:hi], grad_scale, train, self._stats, None, self.unigram_log_probs)
+            ops.gemm(ws["lnf"][lo:hi], self.head16, logits)
+            ops.cross_entropy(logits, targets[lo:hi], grad_scale, train, self._stats, None, self.unigram_log_probs, self.head_scale,
+                              self.head_cap)
             if train:
                 if self.plan.dx("head"):
-                    ops.linear_dgrad(logits, self.wte16, ws["dlnf"][lo:hi])
-                if self.plan.head_wgrad:
-                    ops.linear_wgrad(logits, ws["lnf"][lo:hi], self.d_wte, accumulate=True)
+                    ops.linear_dgrad(logits, self.head16, ws["dlnf"][lo:hi])
+                if self.plan.head_wgrad:   # accumulates over the chunks into wte's or lm_head's gradient
+                    ops.linear_wgrad(logits, ws["lnf"][lo:hi], self.d_head16, accumulate=True)
 
     # ----------------------------------------------------------------- backward
     def _linear_bwd(self, i: int, ws: dict[str, Any], dy: torch.Tensor, g_role: str, x: torch.Tensor, x_role: str, w_role: str,
@@ -727,10 +738,15 @@ class B200Engine:
         self._stats.zero_()
         if self.fp8:
             self._fp8_prologue(train=True)
-        if self.zero3 is not None:
-            self.zero3.zero_stage(self.zero3.plan.rest)   # embeddings + final norm collect gradients over the whole backward
+        z = self.zero3
+        if z is not None:
+            z.zero_stage(z.plan.rest)     # embeddings + final norm collect gradients over the whole backward
+            if z.plan.head is not None:
+                z.zero_stage(z.plan.head)     # the untied LM head's gradient of this microbatch
         self._forward(ids, ws, sequence_id)
         self._head(ws, targets, grad_scale, train=True)
+        if z is not None and z.plan.head is not None:
+            z.reduce(z.plan.head)         # complete after the head's wgrad over every chunk
         self._backward(ids, ws)
 
     def fwd_bwd(self, ids: torch.Tensor, denom: float, scale: float = 1.0,

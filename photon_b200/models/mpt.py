@@ -9,7 +9,9 @@ hand-written sm_90a kernels and is tested against this module.
 
 Block: ``x = x + attn(norm_1(x)); x = x + ffn(norm_2(x))``; ``ffn = down(act(up(x)))`` (``mptmlp``) or
 ``down(act(gate(x)) * up(x))`` (``mptglu``), ``act`` exact GELU (default) or SiLU; every norm LayerNorm (default) or RMSNorm
-(``norm_type``); LM head tied to ``wte``; loss = CE over ``targets = roll(labels, -1)`` with the last position ignored (-100).
+(``norm_type``); LM head tied to ``wte`` (default) or its own ``lm_head`` (``tie_word_embeddings: false``), its logits optionally
+scaled (``logit_scale``) and soft-capped (``final_logit_softcapping``, see :func:`head_transform`); loss = CE over
+``targets = roll(labels, -1)`` with the last position ignored (-100).
 """
 from __future__ import annotations
 
@@ -18,6 +20,7 @@ import numbers
 from dataclasses import dataclass, field
 from typing import Any
 
+import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -59,6 +62,12 @@ class MPTConfig:
     ffn_type: str = "mptmlp"
     ffn_act: str = "gelu"
     ffn_hidden_size: int | None = None
+    # LM head (llm-foundry MPTForCausalLM): tie_word_embeddings false gives it its own weight lm_head.weight [V, d] (no bias);
+    # logit_scale (None, a number or "inv_sqrt_d_model") and final_logit_softcapping c (None or a number) transform its logits
+    # as c · tanh(scale · x / c), see head_transform
+    tie_word_embeddings: bool = True
+    logit_scale: float | str | None = None
+    final_logit_softcapping: float | None = None
     init_std: float | None = None  # None -> kaiming_normal_ (llm-foundry default)
     extra: dict[str, Any] = field(default_factory=dict)
 
@@ -86,6 +95,30 @@ class MPTConfig:
             if isinstance(sc, bool) or not isinstance(sc, numbers.Real) or not math.isfinite(sc) or sc <= 0:
                 raise ValueError(f"attn_config.softmax_scale must be a positive number or None; got {sc!r}")
             self.softmax_scale = float(sc)
+        if not isinstance(self.tie_word_embeddings, (bool, np.bool_)):
+            raise ValueError(f"tie_word_embeddings must be true or false; got {self.tie_word_embeddings!r}")
+        self.tie_word_embeddings = bool(self.tie_word_embeddings)
+        ls = self.logit_scale
+        if isinstance(ls, str):
+            if ls != "inv_sqrt_d_model":
+                raise ValueError(f"logit_scale must be a positive number, 'inv_sqrt_d_model' or None; got {ls!r}")
+        elif ls is not None:
+            self.logit_scale = _positive(ls, "logit_scale")
+        if self.final_logit_softcapping is not None:
+            self.final_logit_softcapping = _positive(self.final_logit_softcapping, "final_logit_softcapping")
+
+    @property
+    def head_scale(self) -> float | None:
+        """The factor on the LM head's logits: ``logit_scale`` as a number (``inv_sqrt_d_model`` = ``1 / sqrt(d_model)``), None
+        without one."""
+        if self.logit_scale == "inv_sqrt_d_model":
+            return 1.0 / math.sqrt(self.d_model)
+        return self.logit_scale
+
+    @property
+    def head_transformed(self) -> bool:
+        """Whether the LM head's logits go through :func:`head_transform` (a scale or a cap is set)."""
+        return self.head_scale is not None or self.final_logit_softcapping is not None
 
     @property
     def attn_scale(self) -> float:
@@ -158,6 +191,8 @@ class MPTConfig:
             sliding_window_size=attn.pop("sliding_window_size", -1), softmax_scale=attn.pop("softmax_scale", None),
             no_bias=bool(m.pop("no_bias", False)), learned_pos_emb=bool(m.pop("learned_pos_emb", True)),
             norm_type=m.pop("norm_type", "low_precision_layernorm"), norm_eps=float(m.pop("norm_eps", 1e-5)),
+            tie_word_embeddings=m.pop("tie_word_embeddings", True), logit_scale=m.pop("logit_scale", None),
+            final_logit_softcapping=m.pop("final_logit_softcapping", None),
         )
         ffn = dict(m.pop("ffn_config", {}) or {})
         known.update(ffn_type=ffn.pop("ffn_type", "mptmlp"), ffn_act=parse_ffn_act(ffn.pop("ffn_act_fn", None)),
@@ -180,7 +215,8 @@ class MPTConfig:
         per_block = 2 * n * d + (w * d + b * w) + (d * d + b * d) + (f * d + b * f) + (f * d + b * d)
         if self.ffn_gated:
             per_block += f * d + b * f   # gate_proj
-        return V * d + (S * d if self.learned_pos_emb else 0) + L * per_block + n * d
+        head = 0 if self.tie_word_embeddings else V * d   # lm_head.weight
+        return V * d + head + (S * d if self.learned_pos_emb else 0) + L * per_block + n * d
 
     def flops_per_token(self, seq_len: int | None = None) -> float:
         """fwd+bwd model FLOPs per token as SpeedMonitor counts them: 6·N + 12·L·d·S."""
@@ -194,6 +230,25 @@ FFN_TYPES = ("mptmlp", "mptglu")
 NORM_TYPES = {"layernorm": "layernorm", "low_precision_layernorm": "layernorm", "rmsnorm": "rmsnorm",
               "low_precision_rmsnorm": "rmsnorm", "triton_rmsnorm": "rmsnorm"}
 FFN_ACTS = ("gelu", "silu")
+
+
+def _positive(v: Any, key: str) -> float:
+    # a negative scale would reverse the greedy argmax, which the decoder takes on the raw logits (see head_transform)
+    if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(v) or v <= 0:
+        raise ValueError(f"{key} must be a positive finite number or None; got {v!r}")
+    return float(v)
+
+
+def head_transform(x: torch.Tensor, scale: float | None, cap: float | None) -> torch.Tensor:
+    """The LM head's logit transform: ``y = scale · x`` (``logit_scale``), then ``y = cap · tanh(y / cap)``
+    (``final_logit_softcapping``); either may be None. With ``scale > 0`` and ``cap > 0`` (the config refuses anything else)
+    it is strictly increasing, so the argmax of ``y`` is the argmax of ``x``. The module applies it to fp32 logits; the scorer
+    applies it to the target logits it reads, the fused cross-entropy kernel computes the same function per logit."""
+    if scale is not None:
+        x = x * scale
+    if cap is not None:
+        x = cap * torch.tanh(x / cap)
+    return x
 
 
 def parse_ffn_act(spec: dict[str, Any] | None) -> str:
@@ -380,7 +435,7 @@ class MPTTransformer(nn.Module):
 
 
 class MPTForCausalLM(nn.Module):
-    """``transformer.*`` parameter tree + tied LM head + shifted-target CE loss."""
+    """``transformer.*`` parameter tree + LM head (tied to ``wte``, or ``lm_head`` when untied) + shifted-target CE loss."""
 
     def __init__(self, cfg: MPTConfig, device: Any = None, init: bool = True, seed: int | None = None) -> None:
         super().__init__()
@@ -388,6 +443,8 @@ class MPTForCausalLM(nn.Module):
         self.activation_checkpointing = False   # fsdp_config.activation_checkpointing (ref: conf/llm_config/mpt-1b.yaml:88)
         with torch.device(device or "cpu"):
             self.transformer = MPTTransformer(cfg)
+            if not cfg.tie_word_embeddings:   # after the transformer, as in llm-foundry: its seeded init comes last
+                self.lm_head = nn.Linear(cfg.d_model, cfg.vocab_size, bias=False)
         if init:
             self.reset_parameters(seed)
         self._rope_cache: tuple[torch.Tensor, torch.Tensor] | None = None
@@ -473,7 +530,11 @@ class MPTForCausalLM(nn.Module):
 
     def forward(self, input_ids: torch.Tensor, sequence_id: torch.Tensor | None = None) -> torch.Tensor:
         h = self.hidden_states(input_ids, sequence_id)
-        return F.linear(h, self.transformer.wte.weight.to(h.dtype))
+        w = self.transformer.wte.weight if self.cfg.tie_word_embeddings else self.lm_head.weight
+        logits = F.linear(h, w.to(h.dtype))
+        if self.cfg.head_transformed:
+            logits = head_transform(logits.float(), self.cfg.head_scale, self.cfg.final_logit_softcapping)
+        return logits
 
     def loss(self, input_ids: torch.Tensor, labels: torch.Tensor | None = None,
              reduction: str = "mean", sequence_id: torch.Tensor | None = None) -> tuple[torch.Tensor, torch.Tensor]:

@@ -243,9 +243,15 @@ def col_sum(dy: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
 
 
 def cross_entropy(logits: torch.Tensor, targets: torch.Tensor, grad_scale: float, write_grad: bool, stats: torch.Tensor,
-                  row_lse: torch.Tensor | None = None, unigram_logp: torch.Tensor | None = None) -> None:
-    """In place: logits → dlogits (when ``write_grad``); stats[0..3] += (Σloss, #valid, #correct, Σunigram)."""
-    ext().cross_entropy(logits, targets, float(grad_scale), bool(write_grad), stats, row_lse, unigram_logp)
+                  row_lse: torch.Tensor | None = None, unigram_logp: torch.Tensor | None = None, logit_scale: float | None = None,
+                  softcap: float | None = None) -> None:
+    """In place: logits → dlogits (when ``write_grad``); stats[0..3] += (Σloss, #valid, #correct, Σunigram).
+
+    ``logit_scale`` / ``softcap``: the LM head's transform (:func:`photon_b200.models.mpt.head_transform`) applied to every logit
+    before the softmax; the loss and ``row_lse`` are those of the transformed logits, the gradient is w.r.t. the stored ones and
+    ``#correct`` counts the argmax of the stored logits (the transform is increasing). None: no scale / no cap."""
+    ext().cross_entropy(logits, targets, float(grad_scale), bool(write_grad), stats, row_lse, unigram_logp,
+                        1.0 if logit_scale is None else float(logit_scale), 0.0 if softcap is None else float(softcap))
 
 
 _NORM_SCRATCH: dict[int, tuple[torch.Tensor, torch.Tensor]] = {}

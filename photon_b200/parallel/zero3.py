@@ -4,7 +4,8 @@ The reference hands this to PyTorch FSDP through Composer (ref: photon/conf/llm_
 and optimizer state are sharded over the ranks, every block's parameters are all-gathered right before its forward / backward and
 its gradient is reduce-scattered right after. Here, on one NVSwitch domain:
 
-* the flat parameter index space is cut into UNITS (one per transformer block, plus one for embeddings + final norm); every unit
+* the flat parameter index space is cut into UNITS (one per transformer block, one for embeddings + final norm and, for an untied
+  LM head, one for ``lm_head.weight``, which sorts before the blocks); every unit
   is cut into ``world_size`` equal slices (256-aligned, zero padded) and rank r owns slice r of EVERY unit — so every gather and
   every reduction is balanced over the ranks whatever the unit (:class:`UnitPlan`, pure host logic);
 * the persistent state of a rank is its shard only: fp32 masters and their bf16 copy (two planes of a :class:`SymmArena`, readable
@@ -50,7 +51,7 @@ BLOCK_MATRICES = ("attn.Wqkv.weight", "attn.out_proj.weight", "ffn.up_proj.weigh
 
 @dataclass(frozen=True)
 class Unit:
-    name: str           # "block.{i}" or "rest"
+    name: str           # "block.{i}", "rest" or "head"
     lo: int             # span [lo, hi) in the flat index space
     hi: int
     per: int            # slice length (multiple of 256); the padded span is world_size * per >= hi - lo
@@ -74,8 +75,10 @@ class UnitPlan:
         if sorted(first) != list(range(n_layers)):
             raise ValueError(f"layout holds blocks {sorted(first)}, expected 0..{n_layers - 1}")
         starts = sorted(first.values())
-        if starts[0] != 0:
-            raise ValueError("the flat layout is expected to start with the transformer blocks (names sort before norm_f / wpe / wte)")
+        # tensors that sort before the first block (an untied lm_head.weight) form the "head" unit
+        head_end = starts[0]
+        if any(o < head_end and o + ne > head_end for o, ne in zip(layout.offsets, layout.numels)):
+            raise ValueError("a tensor straddles the start of the transformer blocks in the flat layout")
         ends = {s: (starts[k + 1] if k + 1 < len(starts) else last_block_end) for k, s in enumerate(starts)}
         units, off = [], 0
         for b in range(n_layers):               # numeric order = execution order
@@ -87,15 +90,23 @@ class UnitPlan:
         per = _round_up(-(-(hi - lo) // self.world_size), align)
         units.append(Unit("rest", lo, hi, per, off))
         off += per
+        # appended after "rest": block i stays unit i, and a layout without tensors before the blocks plans as it always did
+        self.head: int | None = None
+        if head_end > 0:
+            per = _round_up(-(-head_end // self.world_size), align)
+            self.head = len(units)
+            units.append(Unit("head", 0, head_end, per, off))
+            off += per
         self.units: list[Unit] = units
         self.shard_len = off
-        self.max_block_span = max(u.per for u in units[:-1]) * self.world_size
-        self.rest_span = units[-1].per * self.world_size
+        self.max_block_span = max(u.per for u in units[:n_layers]) * self.world_size
+        self.rest_span = units[n_layers].per * self.world_size
+        self.head_span = units[self.head].per * self.world_size if self.head is not None else 0
         # tensor -> unit
         self.unit_of: list[int] = []
         for n, o in zip(layout.names, layout.offsets):
             m = pat.match(n)
-            self.unit_of.append(int(m.group(1)) if m else n_layers)
+            self.unit_of.append(int(m.group(1)) if m else self.head if o < head_end else n_layers)
         # 1-D parameters, packed: (tensor index, offset in the packed fp32 buffer)
         self.small_index: dict[str, int] = {}
         self.small_offsets: dict[str, int] = {}
@@ -109,6 +120,10 @@ class UnitPlan:
     @property
     def rest(self) -> int:
         return self.n_layers
+
+    def resident_unit(self, u: int) -> bool:
+        """Units held whole in a resident buffer (embeddings + final norm, the untied head) rather than a rotating one."""
+        return u == self.rest or u == self.head
 
     def rel(self, name: str) -> tuple[int, int, int]:
         """(unit index, offset inside the unit's padded span, numel) of a tensor."""
@@ -177,14 +192,17 @@ class UnitPlan:
 
     def bytes_per_rank(self, n_moments: int = 2, fp8: bool = False) -> dict[str, int]:
         """Persistent + transient device bytes of one rank (the memory table in DESIGN.md). ``fp8``: the block units travel as
-        E4M3 (no bf16 block buffers) and the E4M3 shard plane, the amax planes and this rank's partial amax are added."""
+        E4M3 (no bf16 block buffers) and the E4M3 shard plane, the amax planes and this rank's partial amax are added. An untied
+        head unit adds its resident bf16 buffer and fp32 staging plane (bf16 under fp8 too)."""
         S = self.shard_len
         out = {"masters_fp32": 4 * S, "bf16_copy": 2 * S, "grad_shard_fp32": 4 * S, "moments_fp32": 4 * n_moments * S,
-               "unit_weight_buffers_bf16": 2 * 2 * self.max_block_span + 2 * self.rest_span,
-               "grad_staging_fp32": 4 * 2 * self.max_block_span + 4 * self.rest_span, "small_fp32": 4 * self.small_len}
+               "unit_weight_buffers_bf16": 2 * 2 * self.max_block_span + 2 * self.rest_span + 2 * self.head_span,
+               "grad_staging_fp32": 4 * 2 * self.max_block_span + 4 * self.rest_span + 4 * self.head_span,
+               "small_fp32": 4 * self.small_len}
         if fp8:
             n_w = len(self.weight_names)
-            out.update(unit_weight_buffers_bf16=2 * self.rest_span, e4m3_shard=S, unit_weight_buffers_e4m3=2 * self.max_block_span,
+            out.update(unit_weight_buffers_bf16=2 * self.rest_span + 2 * self.head_span, e4m3_shard=S,
+                       unit_weight_buffers_e4m3=2 * self.max_block_span,
                        amax_fp32=4 * (self.world_size + 1) * n_w)
         return out
 
@@ -243,6 +261,8 @@ class NvlZero3Comm:
         planes = {"p32": (pl.shard_len, torch.float32), "w16": (pl.shard_len, torch.bfloat16),
                   "gs0": (pl.max_block_span, torch.float32), "gs1": (pl.max_block_span, torch.float32),
                   "gsr": (pl.rest_span, torch.float32)}
+        if pl.head is not None:
+            planes["gsh"] = (pl.head_span, torch.float32)
         if self.fp8:
             self._pieces = pl.weight_pieces(self.rank)
             self.n_weights = len(pl.weight_names)
@@ -254,6 +274,7 @@ class NvlZero3Comm:
         self.p32.zero_(), self.w16.zero_()
         self.gstage = [ar.plane("gs0"), ar.plane("gs1")]
         self.gstage_rest = ar.plane("gsr")
+        self.gstage_head = ar.plane("gsh") if pl.head is not None else None
         self.gshard = torch.zeros(pl.shard_len, dtype=torch.float32, device=self.dev)
         self.wbuf: list[torch.Tensor] | None = None         # bf16 block units (without fp8)
         self.wbuf8: list[torch.Tensor] | None = None        # E4M3 block units (fp8)
@@ -267,6 +288,8 @@ class NvlZero3Comm:
         else:
             self.wbuf = [torch.zeros(pl.max_block_span, dtype=torch.bfloat16, device=self.dev) for _ in range(2)]
         self.wrest = torch.zeros(pl.rest_span, dtype=torch.bfloat16, device=self.dev)
+        # the untied LM head: resident and bf16, also under fp8 (the head GEMMs stay bf16)
+        self.whead = torch.zeros(pl.head_span, dtype=torch.bfloat16, device=self.dev) if pl.head is not None else None
         self.small32 = torch.zeros(pl.small_len, dtype=torch.float32, device=self.dev)
         self._small_copies = pl.small_copies()
         self.side = torch.cuda.Stream(self.dev)
@@ -280,15 +303,15 @@ class NvlZero3Comm:
     def weight(self, name: str) -> torch.Tensor | None:
         """bf16 view of a gathered weight; None for a block matrix under fp8 (its GEMMs read :meth:`weight8`)."""
         u, rel, n = self.plan.rel(name)
-        if u != self.plan.rest and self.wbuf is None:
+        if not self.plan.resident_unit(u) and self.wbuf is None:
             return None
-        buf = self.wrest if u == self.plan.rest else self.wbuf[u % 2]
+        buf = self.wrest if u == self.plan.rest else self.whead if u == self.plan.head else self.wbuf[u % 2]
         return buf[rel: rel + n].view(self.plan.layout.shapes[self.plan.layout.index(name)])
 
     def weight8(self, name: str) -> torch.Tensor:
         """E4M3 view of a gathered block weight matrix (fp8 only)."""
         u, rel, n = self.plan.rel(name)
-        if self.wbuf8 is None or u == self.plan.rest:
+        if self.wbuf8 is None or self.plan.resident_unit(u):
             raise ValueError(f"{name}: E4M3 weights exist for the block matrices of an fp8 communicator only")
         return self.wbuf8[u % 2][rel: rel + n].view(self.plan.layout.shapes[self.plan.layout.index(name)])
 
@@ -314,9 +337,12 @@ class NvlZero3Comm:
         i, o = self.plan.small_index[name], self.plan.small_offsets[name]
         return self.small32[o: o + self.plan.layout.numels[i]].view(self.plan.layout.shapes[i])
 
+    def _stage(self, u: int) -> torch.Tensor:
+        return self.gstage_rest if u == self.plan.rest else self.gstage_head if u == self.plan.head else self.gstage[u % 2]
+
     def grad(self, name: str) -> torch.Tensor:
         u, rel, n = self.plan.rel(name)
-        buf = self.gstage_rest if u == self.plan.rest else self.gstage[u % 2]
+        buf = self._stage(u)
         return buf[rel: rel + n].view(self.plan.layout.shapes[self.plan.layout.index(name)])
 
     # ------------------------------------------------------------------ all-gather (copy-engine pulls)
@@ -352,11 +378,15 @@ class NvlZero3Comm:
             torch.cuda.current_stream(self.dev).wait_event(self._ready[k])
 
     def ensure_resident(self) -> None:
-        """Embeddings + final norm (bf16) and every 1-D parameter (fp32): pulled once per parameter version."""
+        """Embeddings + final norm (bf16), the untied head (bf16) and every 1-D parameter (fp32): pulled once per parameter
+        version."""
         if self._rest_valid:
             return
         un = self.plan.units[self.plan.rest]
         self._pull(self.wrest, "w16", un.off, un.per, 2)
+        if self.plan.head is not None:
+            un = self.plan.units[self.plan.head]
+            self._pull(self.whead, "w16", un.off, un.per, 2)
         src = self.arena.ptrs("p32")
         for r, soff, doff, n in self._small_copies:
             self.ext.memcpy_async(self.small32.data_ptr() + 4 * doff, src[r] + 4 * soff, 4 * n, self.dev.index)
@@ -364,11 +394,11 @@ class NvlZero3Comm:
 
     # ------------------------------------------------------------------ reduce-scatter (fused NVLink kernel)
     def zero_stage(self, u: int) -> None:
-        (self.gstage_rest if u == self.plan.rest else self.gstage[u % 2]).zero_()
+        self._stage(u).zero_()
 
     def reduce(self, u: int) -> None:
         un, ar = self.plan.units[u], self.arena
-        plane = "gsr" if u == self.plan.rest else ("gs0", "gs1")[u % 2]
+        plane = "gsr" if u == self.plan.rest else "gsh" if u == self.plan.head else ("gs0", "gs1")[u % 2]
         self.ext.zero3_reduce(ar.ctl_ptrs(), ar.rank, ar.devices[0], ar.next_epoch(), ar.ptrs(plane), ar.mc_ptr(plane),
                               self.gshard[un.off: un.off + un.per], un.per)
 
@@ -412,7 +442,7 @@ class NvlZero3Comm:
         """fp32 ``[layout.total]`` on this rank's device, pulled slice by slice from the owners."""
         pl = self.plan
         full = torch.zeros(pl.layout.total, dtype=torch.float32, device=self.dev)
-        tmp = torch.empty(max(pl.max_block_span, pl.rest_span), dtype=torch.float32, device=self.dev)
+        tmp = torch.empty(max(pl.max_block_span, pl.rest_span, pl.head_span), dtype=torch.float32, device=self.dev)
         torch.cuda.current_stream(self.dev).wait_stream(self.side)
         for un in pl.units:
             self._pull(tmp, "p32", un.off, un.per, 4)
