@@ -547,8 +547,9 @@ class B200Engine:
         else:
             self._norm_fwd(h[i], w.g1, w.b1, lw["ln1"], lw["m1"], lw["r1"])
             ops.linear_fwd(lw["ln1"], w.wqkv, w.bqkv, lw["qkv"])
-        if c.clip_qkv:   # attn_config.clip_qkv: clamp the fused projection; remember where the gradient passes
-            torch.logical_and(lw["qkv"] > -c.clip_qkv, lw["qkv"] < c.clip_qkv, out=lw["clipmask"])
+        if c.clip_qkv:   # attn_config.clip_qkv: clamp the fused projection; remember where the gradient passes (inside the
+            # clip or exactly on it, as torch.clamp's backward: a bf16 value lands on ±clip often)
+            torch.logical_and(lw["qkv"] >= -c.clip_qkv, lw["qkv"] <= c.clip_qkv, out=lw["clipmask"])
             lw["qkv"].clamp_(-c.clip_qkv, c.clip_qkv)
         if c.qk_ln:   # q / k are strided inside the fused buffer: normalise contiguous copies
             T = lw["qkv"].shape[0]

@@ -279,10 +279,16 @@ def ffn_desc(cfg: MPTConfig) -> str:
     return f"ffn_config ffn_type={cfg.ffn_type} ffn_act_fn={cfg.ffn_act}"
 
 
-def alibi_slopes(n_heads: int, bias_max: int = 8) -> torch.Tensor:
+def at_least_fp32(x: torch.Tensor) -> torch.Tensor:
+    """``x`` in fp32, or in float64 when it already is: the module's fp32 steps (softmax, cross-entropy, RMSNorm, the head's
+    transform) keep a float64 model in float64 throughout."""
+    return x if x.dtype == torch.float64 else x.float()
+
+
+def alibi_slopes(n_heads: int, bias_max: int = 8, dtype: torch.dtype = torch.float32) -> torch.Tensor:
     """Per-head ALiBi slopes (power-of-two ladder, interleaved for non-pow2 head counts)."""
     p2 = 2 ** math.ceil(math.log2(n_heads))
-    m = torch.arange(1, p2 + 1, dtype=torch.float32) * (bias_max / p2)
+    m = torch.arange(1, p2 + 1, dtype=dtype) * (bias_max / p2)
     slopes = 1.0 / torch.pow(2.0, m)
     if p2 != n_heads:
         slopes = torch.cat([slopes[1::2], slopes[::2]])[:n_heads]
@@ -297,9 +303,10 @@ def window_keep(S: int, window: int, device: Any = None) -> torch.Tensor | None:
     return torch.ones(S, S, dtype=torch.bool, device=device).triu(-window)
 
 
-def rope_tables(seq_len: int, d_head: int, theta: float, device: Any = None) -> tuple[torch.Tensor, torch.Tensor]:
-    inv = 1.0 / (theta ** (torch.arange(0, d_head, 2, dtype=torch.float32, device=device) / d_head))
-    ang = torch.outer(torch.arange(seq_len, dtype=torch.float32, device=device), inv)
+def rope_tables(seq_len: int, d_head: int, theta: float, device: Any = None,
+                dtype: torch.dtype = torch.float32) -> tuple[torch.Tensor, torch.Tensor]:
+    inv = 1.0 / (theta ** (torch.arange(0, d_head, 2, dtype=dtype, device=device) / d_head))
+    ang = torch.outer(torch.arange(seq_len, dtype=dtype, device=device), inv)
     return ang.cos(), ang.sin()
 
 
@@ -311,8 +318,8 @@ def apply_rope(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor) -> torch.T
 
 
 class RMSNorm(nn.Module):
-    """llm-foundry's ``RMSNorm``: ``y = x · rsqrt(mean(x²) + eps) · weight`` in fp32, cast back to the input dtype; ``weight``
-    only, initialised to ones."""
+    """llm-foundry's ``RMSNorm``: ``y = x · rsqrt(mean(x²) + eps) · weight`` in fp32 (float64 for float64 inputs), cast back
+    to the input dtype; ``weight`` only, initialised to ones."""
 
     def __init__(self, d: int, eps: float) -> None:
         super().__init__()
@@ -320,8 +327,8 @@ class RMSNorm(nn.Module):
         self.weight = nn.Parameter(torch.ones(d))
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        xf = x.float()
-        return (xf * torch.rsqrt(xf.pow(2).mean(-1, keepdim=True) + self.eps) * self.weight.float()).to(x.dtype)
+        xf = at_least_fp32(x)
+        return (xf * torch.rsqrt(xf.pow(2).mean(-1, keepdim=True) + self.eps) * at_least_fp32(self.weight)).to(x.dtype)
 
 
 def build_norm(cfg: MPTConfig, d: int, bias: bool) -> nn.Module:
@@ -370,7 +377,7 @@ class MPTAttention(nn.Module):
             if win is not None:
                 mask = mask & win
             att = att.masked_fill(~mask, float("-inf"))
-            o = torch.softmax(att.float(), dim=-1).to(v.dtype) @ v
+            o = torch.softmax(at_least_fp32(att), dim=-1).to(v.dtype) @ v
         else:
             bias = None
             if alibi is not None or doc_keep is not None or win is not None:
@@ -489,15 +496,17 @@ class MPTForCausalLM(nn.Module):
     def _aux(self, S: int, device: torch.device) -> tuple[Any, Any]:
         cfg = self.cfg
         rope = alibi = None
+        # the position tables are fp32, or float64 for a float64 module
+        dt = torch.float64 if self.transformer.wte.weight.dtype == torch.float64 else torch.float32
         if cfg.rope:
-            if self._rope_cache is None or self._rope_cache[0].device != device:
-                self._rope_cache = rope_tables(cfg.max_seq_len, cfg.d_head, cfg.rope_theta, device)
+            if self._rope_cache is None or self._rope_cache[0].device != device or self._rope_cache[0].dtype != dt:
+                self._rope_cache = rope_tables(cfg.max_seq_len, cfg.d_head, cfg.rope_theta, device, dt)
             rope = self._rope_cache
         if cfg.alibi:
-            if self._alibi_cache is None or self._alibi_cache.device != device:
-                sl = alibi_slopes(cfg.n_heads, cfg.alibi_bias_max).to(device)
+            if self._alibi_cache is None or self._alibi_cache.device != device or self._alibi_cache.dtype != dt:
+                sl = alibi_slopes(cfg.n_heads, cfg.alibi_bias_max, dt).to(device)
                 pos = torch.arange(cfg.max_seq_len, device=device)
-                rel = (pos[None, :] - pos[:, None]).clamp(max=0).float()  # -(i-j) for j<=i
+                rel = (pos[None, :] - pos[:, None]).clamp(max=0).to(dt)  # -(i-j) for j<=i
                 self._alibi_cache = (sl[:, None, None] * rel[None])[None]
             alibi = self._alibi_cache
         return rope, alibi
@@ -533,7 +542,7 @@ class MPTForCausalLM(nn.Module):
         w = self.transformer.wte.weight if self.cfg.tie_word_embeddings else self.lm_head.weight
         logits = F.linear(h, w.to(h.dtype))
         if self.cfg.head_transformed:
-            logits = head_transform(logits.float(), self.cfg.head_scale, self.cfg.final_logit_softcapping)
+            logits = head_transform(at_least_fp32(logits), self.cfg.head_scale, self.cfg.final_logit_softcapping)
         return logits
 
     def loss(self, input_ids: torch.Tensor, labels: torch.Tensor | None = None,
@@ -542,7 +551,7 @@ class MPTForCausalLM(nn.Module):
         boundary stays in the loss."""
         logits = self.forward(input_ids, sequence_id)
         targets = shift_labels(input_ids if labels is None else labels)
-        flat = F.cross_entropy(logits.float().view(-1, logits.shape[-1]), targets.view(-1),
+        flat = F.cross_entropy(at_least_fp32(logits).view(-1, logits.shape[-1]), targets.view(-1),
                                ignore_index=-100, reduction="sum")
         n = (targets != -100).sum()
         return (flat / n.clamp(min=1) if reduction == "mean" else flat), n
