@@ -759,7 +759,7 @@ void cast_bf16(const Tensor& src, Tensor& dst) {
 }
 void fused_optimizer(Tensor& p, const Tensor& g, Tensor& m, Tensor& v, c10::optional<Tensor> shadow, int kind, bool first_step, double lr,
                      double beta1, double beta2, double eps, double decay, double clip, double step_size, double inv_sqrt_bc2,
-                     const c10::optional<Tensor>& grad_mult) {
+                     const c10::optional<Tensor>& grad_mult, double wd) {
   check_f32(p, "p");
   check_f32(g, "g");
   TORCH_CHECK(p.numel() % 4 == 0, "flat buffers must be multiples of 4 elements");
@@ -782,7 +782,7 @@ void fused_optimizer(Tensor& p, const Tensor& g, Tensor& m, Tensor& v, c10::opti
   c10::cuda::CUDAGuard guard(p.device());
   pb::OptimHyper h;
   h.kind = kind, h.first_step = first_step ? 1 : 0;
-  h.lr = float(lr), h.beta1 = float(beta1), h.beta2 = float(beta2), h.eps = float(eps), h.decay = float(decay);
+  h.lr = float(lr), h.beta1 = float(beta1), h.beta2 = float(beta2), h.eps = float(eps), h.decay = float(decay), h.wd = float(wd);
   h.clip = std::isfinite(clip) ? float(clip) : std::numeric_limits<float>::infinity();
   h.step_size = float(step_size), h.inv_sqrt_bc2 = float(inv_sqrt_bc2);
   pb::fused_optimizer(p.data_ptr<float>(), g.data_ptr<float>(), kind != 2 ? m.data_ptr<float>() : nullptr, kind != 2 ? v.data_ptr<float>() : nullptr,
@@ -955,7 +955,7 @@ void ddp_zero_step(const std::vector<int64_t>& ctl_ptrs, int rank, int device, i
                    const std::vector<int64_t>& param_ptrs, const std::vector<int64_t>& shadow_ptrs, Tensor m, Tensor v, int64_t lo, int64_t hi,
                    int64_t kind, bool first_step, double lr, double beta1, double beta2, double eps, double decay, double clip,
                    double step_size, double inv_sqrt_bc2, double max_norm, double grad_mult, c10::optional<Tensor> out_norm,
-                   int64_t grads_mc, int64_t params_mc, int64_t shadow_mc) {
+                   int64_t grads_mc, int64_t params_mc, int64_t shadow_mc, double wd) {
   c10::cuda::CUDAGuard guard(static_cast<c10::DeviceIndex>(device));
   pb::CommCtl c = make_ctl(ctl_ptrs, rank);
   pb::ZeroStepArgs a{};
@@ -968,7 +968,7 @@ void ddp_zero_step(const std::vector<int64_t>& ctl_ptrs, int rank, int device, i
   a.m = m.data_ptr<float>(), a.v = v.data_ptr<float>();
   a.lo = lo, a.hi = hi;
   a.h.kind = int(kind), a.h.first_step = first_step ? 1 : 0;
-  a.h.lr = float(lr), a.h.beta1 = float(beta1), a.h.beta2 = float(beta2), a.h.eps = float(eps), a.h.decay = float(decay);
+  a.h.lr = float(lr), a.h.beta1 = float(beta1), a.h.beta2 = float(beta2), a.h.eps = float(eps), a.h.decay = float(decay), a.h.wd = float(wd);
   a.h.clip = float(clip), a.h.step_size = float(step_size), a.h.inv_sqrt_bc2 = float(inv_sqrt_bc2);
   a.max_norm = float(max_norm), a.grad_mult = float(grad_mult);
   a.grads_mc = reinterpret_cast<const float*>(grads_mc);
@@ -1034,7 +1034,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("flat_l2_norm", &flat_l2_norm);
   m.def("axpby", &axpby);
   m.def("cast_bf16", &cast_bf16);
-  m.def("fused_optimizer", &fused_optimizer);
+  // wd: ADOPT's coupled weight decay (decouple: false), after the other scalars so that calls without it keep their meaning
+  m.def("fused_optimizer", &fused_optimizer, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("shadow"), py::arg("kind"),
+        py::arg("first_step"), py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("decay"), py::arg("clip"),
+        py::arg("step_size"), py::arg("inv_sqrt_bc2"), py::arg("grad_mult"), py::arg("wd") = 0.0);
   m.def("ipc_alloc", &ipc_alloc);
   m.def("ipc_get_handle", &ipc_get_handle);
   m.def("ipc_open_handle", &ipc_open_handle);
@@ -1061,7 +1064,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("param_ptrs"), py::arg("shadow_ptrs"), py::arg("m"), py::arg("v"), py::arg("lo"), py::arg("hi"), py::arg("kind"),
         py::arg("first_step"), py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("decay"), py::arg("clip"),
         py::arg("step_size"), py::arg("inv_sqrt_bc2"), py::arg("max_norm"), py::arg("grad_mult"), py::arg("out_norm") = py::none(),
-        py::arg("grads_mc") = 0, py::arg("params_mc") = 0, py::arg("shadow_mc") = 0);
+        py::arg("grads_mc") = 0, py::arg("params_mc") = 0, py::arg("shadow_mc") = 0, py::arg("wd") = 0.0);
   m.def("set_wsum", &set_wsum);
   m.def("ctl_sums_word_offset", &pb::ctl_sums_word_offset);
   m.def("launch_count", &launch_count);

@@ -10,6 +10,7 @@ struct OptimHyper {
   int first_step;    // ADOPT: step 0 only seeds v = g^2
   float lr, beta1, beta2, eps;
   float decay;         // multiplicative weight decay factor applied to p (1 = none)
+  float wd;            // ADOPT with coupled decay (decouple: false): the gradient becomes g + wd * p (0 = none)
   float clip;          // ADOPT: step^0.25 clamp on the normalised gradient (inf = off)
   float step_size;     // AdamW: lr / (1 - beta1^t)
   float inv_sqrt_bc2;  // AdamW: 1 / sqrt(1 - beta2^t)

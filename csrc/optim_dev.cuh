@@ -11,17 +11,21 @@ __device__ __forceinline__ void optim_update4(float (&pp)[4], const float (&gg)[
 #pragma unroll
     for (int k = 0; k < 4; ++k) pp[k] = pp[k] * h.decay - h.lr * gg[k];
   } else if (h.kind == 0) {  // ADOPT
+    // coupled weight decay enters the gradient before anything reads it: the step-0 seed of v as well as the update
+    float g[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) g[k] = h.wd != 0.f ? fmaf(h.wd, pp[k], gg[k]) : gg[k];
     if (h.first_step) {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) vv[k] = gg[k] * gg[k];
+      for (int k = 0; k < 4; ++k) vv[k] = g[k] * g[k];
     } else {
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        float ng = gg[k] / fmaxf(sqrtf(vv[k]), h.eps);
+        float ng = g[k] / fmaxf(sqrtf(vv[k]), h.eps);
         ng = fminf(fmaxf(ng, -h.clip), h.clip);
         mm[k] = mm[k] + (1.0f - h.beta1) * (ng - mm[k]);
         pp[k] = pp[k] * h.decay - h.lr * mm[k];
-        vv[k] = h.beta2 * vv[k] + (1.0f - h.beta2) * gg[k] * gg[k];
+        vv[k] = h.beta2 * vv[k] + (1.0f - h.beta2) * g[k] * g[k];
       }
     }
   } else {  // DecoupledAdamW

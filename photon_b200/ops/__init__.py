@@ -289,10 +289,12 @@ def optimizer_hyper(opt: Any, lr: float) -> dict[str, Any]:
     """Per-step scalar arguments of the fused optimizer kernels for a :class:`FlatOptimizer` at learning rate ``lr``."""
     kind = _KIND[opt.name]
     first = kind == 0 and opt.step_count == 0
-    decay, clip, step_size, inv_sqrt_bc2 = 1.0, float("inf"), 0.0, 1.0
+    decay, wd, clip, step_size, inv_sqrt_bc2 = 1.0, 0.0, float("inf"), 0.0, 1.0
     if kind == 0:
         if opt.weight_decay and getattr(opt, "decouple", True):
             decay = 1.0 - lr * opt.weight_decay
+        elif opt.weight_decay:      # coupled: the kernel adds wd * p to the gradient (before the step-0 seed of v too)
+            wd = opt.weight_decay
         if opt.clip_exp is not None and not first:
             clip = float(opt.step_count) ** opt.clip_exp
     elif kind == 1:
@@ -303,7 +305,7 @@ def optimizer_hyper(opt: Any, lr: float) -> dict[str, Any]:
     else:
         decay = 1.0 - lr * opt.weight_decay if opt.weight_decay else 1.0
     return dict(kind=kind, first=first, lr=float(lr), beta1=opt.beta1, beta2=opt.beta2, eps=opt.eps, decay=float(decay),
-                clip=float(clip), step_size=float(step_size), inv_sqrt_bc2=float(inv_sqrt_bc2))
+                wd=float(wd), clip=float(clip), step_size=float(step_size), inv_sqrt_bc2=float(inv_sqrt_bc2))
 
 
 def fused_optimizer_step(opt: Any, lr: float, grad_mult: torch.Tensor | float | None) -> None:
@@ -316,7 +318,8 @@ def fused_optimizer_step(opt: Any, lr: float, grad_mult: torch.Tensor | float | 
         gm = gm.to(torch.float32).reshape(1)
     params, grads, shadow = opt.local_views()   # the whole flat buffer, or this rank's slice when the state is sharded
     ext().fused_optimizer(params, grads, opt.exp_avg, opt.exp_avg_sq, shadow, h["kind"], h["first"], h["lr"],
-                          h["beta1"], h["beta2"], h["eps"], h["decay"], h["clip"], h["step_size"], h["inv_sqrt_bc2"], gm)
+                          h["beta1"], h["beta2"], h["eps"], h["decay"], h["clip"], h["step_size"], h["inv_sqrt_bc2"], gm,
+                          wd=h["wd"])
 
 
 # ---------------------------------------------------------------------------- attention

@@ -96,7 +96,7 @@ class NvlZeroComm:
                                 opt.exp_avg, opt.exp_avg_sq, lo, hi, h["kind"], h["first"], h["lr"], h["beta1"], h["beta2"], h["eps"],
                                 h["decay"], h["clip"], h["step_size"], h["inv_sqrt_bc2"],
                                 float(max_norm) if max_norm is not None else -1.0, float(inv_scale), self.norm,
-                                ar.mc_ptr("grads"), ar.mc_ptr("params"), ar.mc_ptr("shadow"))
+                                ar.mc_ptr("grads"), ar.mc_ptr("params"), ar.mc_ptr("shadow"), wd=h["wd"])
         opt.lr = float(lr)
         opt.step_count += 1
         return self.norm[0]

@@ -253,12 +253,14 @@ def _f32(v: float) -> float:
 
 def optim_step(kind: int, p: torch.Tensor, g: torch.Tensor, m: torch.Tensor, v: torch.Tensor, hyper: dict,
                grad_mult: float | None = None):
-    """One step of ``optim_update4`` in fp64. ``hyper``: first, lr, beta1, beta2, eps, decay, clip, step_size, inv_sqrt_bc2
-    (rounded to fp32 here, as the binding does). kind 0 = ADOPT, 1 = DecoupledAdamW, 2 = SGD.
+    """One step of ``optim_update4`` in fp64. ``hyper``: first, lr, beta1, beta2, eps, decay, wd (optional, 0 if absent),
+    clip, step_size, inv_sqrt_bc2 (rounded to fp32 here, as the binding does). kind 0 = ADOPT, 1 = DecoupledAdamW, 2 = SGD.
 
     Returns (p, m, v, tol): ``tol[k]`` bounds the kernel's error in plane k after one step from the same state. Each update
     line contributes ``OPTIM_ULPS`` fp32 ulps of its largest term (``_line``), and a line that reads a plane computed on an
-    earlier line inherits that plane's error: ADOPT's p reads the new m (``lr * tol_m``), AdamW's p reads the new m and v."""
+    earlier line inherits that plane's error: ADOPT's p reads the new m (``lr * tol_m``), AdamW's p reads the new m and v.
+    ADOPT's coupled weight decay (``wd``) is a line of its own, ``G + wd * p``, whose error every later line reads: through
+    the normalised gradient (divided by ``max(sqrt v, eps)``) into m, and as ``2 |G|`` times it into v."""
     h = {k: (_f32(val) if isinstance(val, float) and math.isfinite(val) else val) for k, val in hyper.items()}
     P, M, Vv = p.to(F64).clone(), m.to(F64).clone(), v.to(F64).clone()
     gm = _f32(grad_mult) if grad_mult is not None else 1.0
@@ -270,19 +272,24 @@ def optim_step(kind: int, p: torch.Tensor, g: torch.Tensor, m: torch.Tensor, v: 
         tp = _line(P, step, P1)
         P = P1
     elif kind == 0:
+        t_g = torch.zeros_like(G)
+        if h.get("wd", 0.0):
+            G1 = G + h["wd"] * P
+            t_g = _line(G, h["wd"] * P, G1)
+            G = G1
         if h["first"]:
             Vv = G * G
-            tv = _line(Vv)
+            tv = _line(Vv) + 2 * G.abs() * t_g
         else:
             ng = G / torch.clamp(torch.sqrt(Vv), min=h["eps"])
             ng = ng.clamp(-h["clip"], h["clip"])
-            t_ng = _line(ng)                                    # approximate sqrt and division
+            t_ng = _line(ng) + t_g / torch.clamp(torch.sqrt(Vv), min=h["eps"])   # approximate sqrt and division
             M1 = M + (1.0 - h["beta1"]) * (ng - M)
             tm = _line(M, ng, M1) + (1.0 - h["beta1"]) * t_ng
             P1 = P * h["decay"] - h["lr"] * M1
             tp = _line(P, h["lr"] * M1, P1) + h["lr"] * tm
             V1 = h["beta2"] * Vv + (1.0 - h["beta2"]) * G * G
-            tv = _line(Vv, G * G, V1)
+            tv = _line(Vv, G * G, V1) + (1.0 - h["beta2"]) * 2 * G.abs() * t_g
             P, M, Vv = P1, M1, V1
     else:
         P0 = P * h["decay"]

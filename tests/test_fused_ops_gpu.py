@@ -452,12 +452,15 @@ def test_embedding(d, B, mode):
 
 
 # =============================================================================================== optimizer
-def _hyper(kind, step, lr=3e-2, b1=0.9, b2=0.99, eps=1e-6, wd=0.1, clip_exp=0.25):
+def _hyper(kind, step, lr=3e-2, b1=0.9, b2=0.99, eps=1e-6, wd=0.1, clip_exp=0.25, coupled=False):
     t = step + 1
-    h = dict(first=False, lr=lr, beta1=b1, beta2=b2, eps=eps, decay=1.0, clip=math.inf, step_size=0.0, inv_sqrt_bc2=1.0)
+    h = dict(first=False, lr=lr, beta1=b1, beta2=b2, eps=eps, decay=1.0, wd=0.0, clip=math.inf, step_size=0.0, inv_sqrt_bc2=1.0)
     if kind == 0:
         h["first"] = step == 0
-        h["decay"] = 1.0 - lr * wd
+        if coupled:                                    # decouple: false — wd * p joins the gradient
+            h["wd"] = wd
+        else:
+            h["decay"] = 1.0 - lr * wd
         if step > 0:
             h["clip"] = float(step) ** clip_exp
     elif kind == 1:
@@ -471,36 +474,37 @@ def _hyper(kind, step, lr=3e-2, b1=0.9, b2=0.99, eps=1e-6, wd=0.1, clip_exp=0.25
 
 def _optim_call(kind, p, g, m, v, shadow, h, gm):
     _ops().ext().fused_optimizer(p, g, m, v, shadow, kind, h["first"], h["lr"], h["beta1"], h["beta2"], h["eps"], h["decay"],
-                                 h["clip"], h["step_size"], h["inv_sqrt_bc2"], gm)
+                                 h["clip"], h["step_size"], h["inv_sqrt_bc2"], gm, wd=h["wd"])
 
 
 @pytest.mark.parametrize("with_shadow", [True, False])
 @pytest.mark.parametrize("with_gm", [True, False])
 @pytest.mark.parametrize("n", [4, 4100, (1 << 22) + 4])
-@pytest.mark.parametrize("kind", [0, 1, 2], ids=["adopt", "adamw", "sgd"])
-def test_fused_optimizer(kind, n, with_gm, with_shadow):
+@pytest.mark.parametrize("kind,coupled", [(0, False), (1, False), (2, False), (0, True)], ids=["adopt", "adamw", "sgd", "adopt_coupled"])
+def test_fused_optimizer(kind, coupled, n, with_gm, with_shadow):
     """``optim_kernel`` for 5 steps against ``fused_oracle.optim_step`` from the kernel's own state each step: ADOPT's first
     step (only v is seeded) and a clip ``step**0.25`` that binds (v was seeded from small or zero gradients), AdamW's bias
-    corrections, SGD without moment planes, weight decay, grad_mult, zero gradients (ADOPT's ``max(sqrt v, eps)``), a size
-    that is not a multiple of the grid stride. The bf16 shadow equals ``p.to(bf16)`` bitwise."""
+    corrections, SGD without moment planes, weight decay (ADOPT's also coupled: added to the gradient), grad_mult, zero
+    gradients (ADOPT's ``max(sqrt v, eps)``), a size that is not a multiple of the grid stride. The bf16 shadow equals
+    ``p.to(bf16)`` bitwise."""
     p = torch.randn(n, device=DEV, generator=_gen(n))
     m = torch.zeros(n, device=DEV) if kind != 2 else torch.empty(0, device=DEV)
     v = torch.zeros(n, device=DEV) if kind != 2 else torch.empty(0, device=DEV)
     sbuf, shadow = _guarded((n,), torch.bfloat16) if with_shadow else (None, None)
     gm = torch.tensor([0.5], device=DEV) if with_gm else None
-    what = f"fused_optimizer kind={kind} n={n} grad_mult={with_gm} shadow={with_shadow}"
+    what = f"fused_optimizer kind={kind} coupled={coupled} n={n} grad_mult={with_gm} shadow={with_shadow}"
     bound_seen = False
     for step in range(5):
         g = torch.randn(n, device=DEV, generator=_gen(step)) * (0.1 if step == 0 else 1.0)
         g[::7] = 0.0                                   # zero every step: v stays 0 there
         if step == 0:
             g[3::11] = 0.0                             # zero only at the seeding step: g / eps later, clipped
-        h = _hyper(kind, step)
+        h = _hyper(kind, step, coupled=coupled)
         state = (p.clone(), m.clone(), v.clone())
         P, M, V, tol = fo.optim_step(kind, p, g, m if kind != 2 else p, v if kind != 2 else p, h,
                                        grad_mult=0.5 if with_gm else None)
         if kind == 0 and step > 0:
-            G = g.to(F64) * (0.5 if with_gm else 1.0)
+            G = g.to(F64) * (0.5 if with_gm else 1.0) + h["wd"] * p.to(F64)
             bound_seen |= bool((G.abs() / v.to(F64).sqrt().clamp(min=h["eps"]) > h["clip"]).any())
         _optim_call(kind, p, g, m, v, shadow, h, gm)
         tag = f"{what} step {step}"

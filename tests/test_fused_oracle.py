@@ -83,9 +83,11 @@ class _Flat:
         self.grads = torch.zeros(n)
 
 
-@pytest.mark.parametrize("name,kind", [("adopt", 0), ("decoupled_adamw", 1), ("sgd", 2)])
-def test_optim_step_matches_torch_path(name, kind):
-    """``optim_step`` (fp64, the kernel's line order) and the fp32 torch path of FlatOptimizer take the same steps."""
+@pytest.mark.parametrize("name,kind,decouple", [("adopt", 0, True), ("decoupled_adamw", 1, True), ("sgd", 2, True), ("adopt", 0, False)],
+                         ids=["adopt-0", "decoupled_adamw-1", "sgd-2", "adopt_coupled_decay-0"])
+def test_optim_step_matches_torch_path(name, kind, decouple):
+    """``optim_step`` (fp64, the kernel's line order) and the fp32 torch path of FlatOptimizer take the same steps; ADOPT also
+    with ``decouple: false``, where the weight decay is added to the gradient."""
     from photon_b200 import ops
     from photon_b200.train.optim import build_optimizer
 
@@ -96,7 +98,7 @@ def test_optim_step_matches_torch_path(name, kind):
     # beta2 = 0.99 those two differ by 8 fp32 ulps of 1 - beta2 before any arithmetic happens
     cfg = dict(name=name, lr=3e-2, betas=[0.875, 0.9921875], eps=1e-6, weight_decay=0.1)
     if name == "adopt":
-        cfg["clip_exp"] = 0.25
+        cfg.update(clip_exp=0.25, decouple=decouple)
     opt = build_optimizer(cfg, flat, use_kernel=False)
     for step in range(5):
         g = torch.randn(n) * (10.0 if step == 1 else 1.0)
