@@ -479,7 +479,7 @@ __global__ void __launch_bounds__(512) zero3_fp8_requant_kernel(const Zero3Requa
     if (blockIdx.x == 0) {
       const long long r = a.roles[j];
       a.meta[r] = s;
-      a.meta[a.n_roles + r] = 1.0f / s;
+      a.meta[a.n_roles + r] = inv_scale(s);
       a.meta[2 * a.n_roles + r] = m;
     }
   }

@@ -219,7 +219,7 @@ __global__ void __launch_bounds__(256) seg_quant_kernel(const __nv_bfloat16* __r
   const float s = weight_scale(a, fmax);
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     scale[blockIdx.y] = s;
-    scale_inv[blockIdx.y] = 1.0f / s;
+    scale_inv[blockIdx.y] = inv_scale(s);
   }
   const uint4* p = reinterpret_cast<const uint4*>(src + off);
   uint2* q = reinterpret_cast<uint2*>(dst + off);
@@ -243,9 +243,9 @@ __global__ void update_scales_kernel(float* __restrict__ scale, float* __restric
     float m = 0.f;
     for (int i = 0; i < H; ++i) m = fmaxf(m, hist[(long long)r * H + i]);
     if (m > 0.f && m < 3.0e38f) {   // no observation yet (or a non-finite one): keep the scale
-      const float s = fmax[r] / (m * margin_mult);
+      const float s = scale_of(fmax[r], m * margin_mult);
       scale[r] = s;
-      scale_inv[r] = 1.0f / s;
+      scale_inv[r] = inv_scale(s);
     }
   }
   __syncthreads();

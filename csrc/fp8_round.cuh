@@ -30,7 +30,11 @@ __device__ __forceinline__ float amax8(const float (&f)[8], float m) {
   for (int k = 0; k < 8; ++k) m = fmaxf(m, fabsf(f[k]));
   return m;
 }
+// Scales are the recipe's quotients rounded to nearest (photon_b200/train/fp8.py): the build's --use_fast_math would otherwise
+// turn these divisions into approximate reciprocals, a few ulp away from fmax / amax and from the exact inverse of the scale.
+__device__ __forceinline__ float scale_of(float fmax, float amax) { return __fdiv_rn(fmax, amax); }
+__device__ __forceinline__ float inv_scale(float s) { return __frcp_rn(s); }
 // per-tensor current scaling: the E4M3 scale of a weight from its amax (1 when the tensor is all zeros or not finite)
-__device__ __forceinline__ float weight_scale(float amax, float fmax) { return (amax > 0.f && amax < 3.0e38f) ? fmax / amax : 1.0f; }
+__device__ __forceinline__ float weight_scale(float amax, float fmax) { return (amax > 0.f && amax < 3.0e38f) ? scale_of(fmax, amax) : 1.0f; }
 
 }  // namespace pb

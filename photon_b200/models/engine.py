@@ -138,7 +138,8 @@ class B200Engine:
         kernels = dict(kernels or {})
         # amp_fp8 (ref: scripts/centralised_training.sh:91, Composer amp_fp8 -> TransformerEngine): the four GEMMs of every block
         # and their dgrad / wgrad run on fp8 wgmma (E4M3 activations / weights, E5M2 gradients, per-tensor
-        # scaling, fp32 accumulation); LayerNorm, attention, residuals, LM head, loss and optimizer stay bf16 / fp32
+        # scaling, accumulation in the tensor cores' reduced fp8 precision: tests/fp8_oracle.py); LayerNorm, attention, residuals,
+        # LM head, loss and optimizer stay bf16 / fp32
         self.fp8 = precision == "amp_fp8"
         if zero3 is not None and bool(getattr(zero3, "fp8", False)) != self.fp8:
             raise ValueError(f"precision={precision} needs NvlZero3Comm(..., fp8={self.fp8}): block units are gathered as "
@@ -818,8 +819,14 @@ class B200Engine:
         targets = shift_labels(ids).reshape(-1)
         self._stats.zero_()
         if self.fp8:
+            # evaluation casts with the training scales and leaves the delayed-scaling state as it found it: the amax its
+            # forward records would otherwise be merged into the next training step's history slot, so how often a run
+            # evaluates would change its training scales
+            amax = self.fp8_meta[2, : self._n_dyn].clone()
             self._fp8_prologue(train=False)
         self._forward(ids, ws, sequence_id)
+        if self.fp8:
+            self.fp8_meta[2, : self._n_dyn].copy_(amax)
         self._head(ws, targets, 0.0, train=False)
         st = self._stats.clone()
         out = {"loss_sum": st[0], "n_tokens": st[1], "n_correct": st[2]}

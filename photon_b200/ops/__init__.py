@@ -140,7 +140,8 @@ def gemm_fp8(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, meta: torch.Te
              accumulate: bool = False, alpha: float = 1.0, cluster: int = 0, out8: torch.Tensor | None = None,
              role_out: int = -1) -> torch.Tensor:
     """``out = epilogue(alpha / (scale[role_a] * scale[role_b]) * A8 @ B8^T)`` — 1-byte operands (E4M3 / E5M2 per operand) on
-    fp8 ``wgmma`` (MN-major operands are transposed to K-major first), fp32 accumulation. ``meta`` = float32 ``[3, n_roles]`` (scale, 1/scale, amax) on the device;
+    fp8 ``wgmma`` (MN-major operands are transposed to K-major first), accumulated in fp32 registers at the tensor cores' reduced fp8
+    precision (about 2^-10 of Σ|a·b|, see tests/fp8_oracle.py). ``meta`` = float32 ``[3, n_roles]`` (scale, 1/scale, amax) on the device;
     the de-scales are read by the kernel, so nothing here touches the host. ``EPI_GELU_GRAD_Q8`` writes ``out8`` (E4M3,
     scaled by ``scale[role_out]``, amax recorded) and ``out2`` = gelu'; ``out`` is then unused (pass ``out2``)."""
     ext().gemm_fp8(a, b, out, int(a_mn), int(b_mn), int(epi), int(a_fmt), int(b_fmt), meta, int(role_a), int(role_b), bias, aux, out2,
